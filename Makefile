@@ -1,6 +1,6 @@
-# Builds the sm_100a CUDA library (C ABI) and the stand-alone kernel test drivers.
+# Builds the sm_90a CUDA library (C ABI) and the stand-alone kernel test drivers.
 NVCC      ?= nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall
 CSRC      := segtran_b200/csrc
 LIB_SRCS  := $(filter-out $(CSRC)/test_%.cu,$(wildcard $(CSRC)/*.cu))

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the Segtran hot path on B200 (contract: see the task statement / DESIGN.md §Measurement).
+"""Benchmark of the Segtran hot path on an H100 (see DESIGN.md §Measurement).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 1..5] [--scaling weak|strong]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W
 
@@ -146,7 +147,7 @@ def synthetic_batch(c, B, device, seed):
 
 
 # ----------------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md recipe)
+# clocks sampler (nvidia-smi queries, read-only)
 # ----------------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -184,7 +185,7 @@ class ClockSampler(threading.Thread):
 # ----------------------------------------------------------------------------------------------------------
 def oracle_step_factory(c, B, device="cpu"):
     """One training step (fwd + loss + bwd + clip + BertAdam) of the reference FORMULATION on `device` for B samples of
-    config c, with the same seed-defined initial weights as the B200 arm (the shell's own state_dict feeds the oracle)."""
+    config c, with the same seed-defined initial weights as the CUDA arm (the shell's own state_dict feeds the oracle)."""
     from oracle import segtran_oracle as O
     from oracle import train_oracle as T
     net = build_net(c, "cpu")
@@ -229,7 +230,7 @@ def oracle_step_factory(c, B, device="cpu"):
 
 
 def time_oracle_cpu(c, B, steps, warmup, budget_s):
-    """Times the CPU oracle at the workload's own per-GPU batch (same config as the B200 arm).  The number of warm-up /
+    """Times the CPU oracle at the workload's own per-GPU batch (same config as the CUDA arm).  The number of warm-up /
     timed steps is cut to fit the budget, down to timing a single step; only if even one full-size step does not fit is
     the batch reduced (and the line says so).  On many-core hosts PyTorch's CPU kernels can be slower with every core
     than with a few dozen threads, so a second thread count is probed and the faster one kept (`cores` = threads used)."""
@@ -328,7 +329,7 @@ def run_reference(args):
 
 
 # ----------------------------------------------------------------------------------------------------------
-# B200 arm
+# CUDA arm (the segtran_b200 kernels)
 # ----------------------------------------------------------------------------------------------------------
 class KernelTimer:
     """CUDA-event timing of individual C-ABI calls on the launching stream (for the roofline of the dominant kernel)."""
@@ -410,6 +411,25 @@ class KernelTimer:
         return agg
 
 
+DUMP_MAX_ELEMS = 3 << 20          # per array: 12 MB of float32, five arrays stay under 64 MB
+
+
+def dump_outputs(d, arrays):
+    """DIR/<name>.npy in float32 for each array; one with more than DUMP_MAX_ELEMS elements is replaced by its values at
+    a fixed, seeded sample of flat indices (the same indices for the same size), so that two builds compare element for
+    element."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_MAX_ELEMS:
+            # sorted seeded indices (with repeats), drawn on the host and gathered on the device before the copy
+            g = torch.Generator(device="cpu").manual_seed(20240601)
+            idx = torch.randint(flat.numel(), (DUMP_MAX_ELEMS,), generator=g).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(d, name + ".npy"), flat.float().cpu().numpy())
+
+
 def bucket_checksum(params):
     """Integer checksum of the parameter bits (identical on every rank iff the parameters are)."""
     acc = torch.zeros(2, dtype=torch.int64, device=params[0].device)
@@ -461,11 +481,14 @@ def run_b200(args):
         [{"params": hp, "lr": TRAIN["lr"], "weight_decay": TRAIN["decay"]}], warmup=TRAIN["warmup"],
         t_total=TRAIN["t_total"], grad_clip=TRAIN["grad_clip"], bucket=bucket)
 
+    last = {}
+
     def compute():
         bucket.zero()
         feat.grad = None
         curr.grad = None
         logits = net.hot_path(feat, curr, None, sp)
+        last["logits"] = logits                 # (inside a captured graph: the graph's output buffer, rewritten per replay)
         loss, _, _ = seg_loss(logits, Y, pw, cw, TRAIN["dice_w"])         # train3d.py:731-756
         loss.backward()
         if world > 1 and not args.no_overlap:
@@ -525,6 +548,10 @@ def run_b200(args):
         dist.all_reduce(lo, op=dist.ReduceOp.MIN)
         dist.all_reduce(hi, op=dist.ReduceOp.MAX)
         checksum_agree = bool(torch.equal(lo, hi))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"loss": loss.detach().reshape(1), "logits": last["logits"].detach(),
+                                         "feat_grad": feat.grad, "curr_grad": curr.grad,
+                                         "params": torch.cat([q.detach().reshape(-1) for q in hp])})
 
     # ---- the same K steps again with a CUDA-event pair around every C-ABI call (per-kernel durations for the
     #      roofline; the extra event records cost host time, so this pass is not the headline number) ----
@@ -612,36 +639,30 @@ def run_b200(args):
         kname, (kms, kwork, kcount) = top
         bf16 = precision == "bf16"
         if kname == "sx_gemm":
-            # TF32 operands: the tensor-core peak is half the measured dense bf16 figure
-            src = "measured" if "bf16_tflops_sustained" in peaks else "fallback"
-            peak = peaks.get("bf16_tflops_sustained", 1400.0) / (1.0 if bf16 else 2.0)
+            # TF32 operands: the tensor-core peak is half the dense bf16 figure (without a measured figure: the H100 SXM
+            # data sheet's 989 TFLOP/s dense bf16 at 700 W — an upper bound, not a rate this card was seen to reach)
+            src = "measured" if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet"
+            peak = peaks.get("bf16_tflops_sustained", 989.0) / (1.0 if bf16 else 2.0)
             ach = kwork / (kms * 1e-3) / 1e12
             # the executed count is lower than the reference formulation's (SURVEY §8d: ref_gflop per sample forward, x3
-            # for fwd+bwd) because of the re-associated in-squeeze and mid Linear (DESIGN §4.5)
+            # for fwd+bwd) because of the re-associated in-squeeze and mid Linear (DESIGN §4.1)
             ref_flops = c["ref_gflop"] * 1e9 * 3 * B * args.steps
-            roof = {"bound": "tensor", "kernel": "sx_gemm_kernel (tcgen05 kind::%s)" % ("f16/bf16" if bf16 else "tf32"),
+            roof = {"bound": "tensor", "kernel": "sx_gemm_kernel (wgmma %s)" % ("bf16" if bf16 else "tf32"),
                     "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
                     "achieved_reference_formulation": ref_flops / (kms * 1e-3) / 1e12,
                     "executed_tflop_per_step": kwork / args.steps / 1e12,
                     "peak_source": "%s bf16 sustained%s" % (src, "" if bf16 else " / 2 (tf32 rate)"), "launches": kcount,
                     "share_of_step": kms / total_ms}
-            hbm_peak = peaks.get("hbm_gbs", 6570.0)
+            hbm_peak = peaks.get("hbm_gbs", 3350.0)
             pl = timer.gemm_roofline(peak, hbm_peak)
             for v in pl.values():
                 if isinstance(v, dict):
                     v["ms"] /= args.steps
             roof["per_launch"] = pl
             roof["algorithmic_bytes_per_launch"] = sum(timer.gemm_bytes) / max(len(timer.gemm_bytes), 1)
-            try:        # DRAM bytes of the GEMM launches of a step from an ncu capture of this command (profiles/, per launch)
-                tr = json.load(open(os.path.join(ROOT, "profiles", "gemm_dram_traffic.json")))
-                if args.config == 4 and not bf16:
-                    roof["traffic"] = tr["dram_bytes_per_launch"]
-                    roof["traffic_source"] = tr.get("source", "profiles/gemm_dram_traffic.json")
-            except Exception:
-                pass
         else:
-            src = "measured" if "hbm_gbs" in peaks else "fallback"
-            peak = peaks.get("hbm_gbs", 6650.0)
+            src = "measured" if "hbm_gbs" in peaks else "H100 SXM data sheet"
+            peak = peaks.get("hbm_gbs", 3350.0)
             ach = kwork / (kms * 1e-3) / 1e9
             roof = {"bound": "hbm", "kernel": kname, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                     "traffic": None, "peak_source": src, "launches": kcount, "share_of_step": kms / total_ms}
@@ -655,7 +676,7 @@ def run_b200(args):
                 "vs_baseline": None, "dtype": precision, "data": "synthetic",
                 "config": {"workload": workload_name(c, B), "baseline_config": args.config,
                            "global_batch": world * B, "tokens_per_sample": N, "parallelism": "dp%d" % world,
-                           "l2": "inputs (%.2f GB/step) exceed the 126 MB L2; no explicit flush" % (
+                           "l2": "inputs (%.2f GB/step) exceed the 50 MB L2; no explicit flush" % (
                                (feat.numel() + curr.numel() + Y.numel()) * 4 / 1e9),
                            "grad_bucket_bytes": bucket.bytes(),
                            "launch": "cuda-graph replay of fwd+loss+bwd" if use_graph else "eager",
@@ -663,7 +684,7 @@ def run_b200(args):
                                "one NCCL all-reduce after the step" if args.no_overlap else
                                "NCCL all-reduce of bucket ranges issued at layer milestones inside the (captured) step"),
                            "attention": "unfused (GEMM + softmax kernels)" if args.no_fused_attn else
-                                        "fused tcgen05 scores+softmax kernel (sx_attn)",
+                                        "fused wgmma scores+softmax kernel (sx_attn)",
                            "loss": "BCEWithLogits(pos_weight) + per-class Dice on the full-size logits (train3d.py:731-756)",
                            "optimizer": None if opt is None else "FlatBertAdam on the hot-path parameters incl. --gradclip "
                                                                  "0.1 (optimization.py:90-164, train3d.py:760-762), in the step"},
@@ -761,6 +782,9 @@ def main():
     ap.add_argument("--no-fused-attn", action="store_true", help="squeeze-out attention as separate GEMM + softmax kernels")
     ap.add_argument("--no-overlap", action="store_true", help="N>1: one all-reduce of the whole bucket after the step")
     ap.add_argument("--no-graph", action="store_true", help="enqueue every kernel from Python instead of replaying a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step computed (loss, logits, input gradients, "
+                         "updated parameters) as DIR/<name>.npy")
     args = ap.parse_args()
     wd = float(os.environ.get("SEGTRAN_BENCH_WATCHDOG_S", "0"))
     if wd == 0 and args.impl != "reference" and int(os.environ.get("WORLD_SIZE", "1")) > 1:

@@ -1,5 +1,5 @@
 /*
- * segtran_b200 — C ABI of the B200-native Squeeze-and-Expansion hot path.
+ * segtran_b200 — C ABI of the H100-native (sm_90a) Squeeze-and-Expansion hot path.
  *
  * The reference (askerlee/segtran) is pure Python/PyTorch and has no FFI layer: the drop-in
  * boundary is the nn.Module contract of code/networks/segtran_shared.py (SegtranFusionEncoder
@@ -11,12 +11,15 @@
  * Conventions
  *  - every pointer is a caller-owned DEVICE pointer (tensor.data_ptr()); nothing is retained
  *    after the call returns; scratch is passed in explicitly by the caller;
+ *  - `part, part_floats`: scratch for per-CTA partial sums, which a second kernel adds in a fixed order, so results are
+ *    bit-identical from run to run; a larger scratch allows more CTAs (up to the machine's width); it must not be in
+ *    use by another stream while the call runs;
  *  - every call is asynchronous on the cudaStream_t given (passed as void*);
  *  - return 0 on success, negative on error; sx_last_error() returns a thread-local message;
  *  - no global mutable state apart from one-time function-attribute setup (thread safe: the
  *    autograd engine calls backward entry points from its own worker thread);
  *  - the device is the current CUDA context's device (torch sets it); never assumed to be 0.
- *  - there is NO CPU fallback: a missing GPU / non-sm_100 device is an error.
+ *  - there is NO CPU fallback: a missing GPU / non-sm_90 device is an error.
  */
 #ifndef SEGTRAN_B200_H_
 #define SEGTRAN_B200_H_
@@ -46,7 +49,7 @@ const char* sx_last_error(void);
 int sx_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* ---------------------------------------------------------------------------------------------
- * Batched GEMM on tcgen05 tensor cores (TMA-staged operands, fp32 accumulators in TMEM):
+ * Batched GEMM on the wgmma tensor cores (TMA-staged operands, fp32 accumulators in registers):
  *     C[z1][z0][m][n] = epilogue( alpha * sum_k A[z1][z0][m][k] * B[z1][z0][n][k] )
  * Replaces every dense contraction on the path: the Q/K/V projections (segtran_shared.py:559-560,
  * :414), Q.K^T (:566), P.V (:447), MMSharedMid's shared Linear (:243), MMPrivateOutput's grouped
@@ -89,7 +92,11 @@ typedef struct {
   const float* addend;           /* optional fp32 tensor in C's layout: C = epilogue(alpha*A.B^T + addend); used by the
                                     error-compensated 3-pass TF32 mode (A_hi B_hi + A_lo B_hi + A_hi B_lo) */
   float* colsum;                 /* optional [N] fp32: += column sums of the stored values over all rows and batch slices
-                                    (a bias gradient that would otherwise need its own pass over the output) */
+                                    (a bias gradient that would otherwise need its own pass over the output; float atomics,
+                                    so the order of the additions varies: sx_colsum on the output is the ordered form) */
+  float* part;                   /* split_k > 1: scratch for the partial tiles (summed in split order); split_k is lowered
+                                    to what part_floats holds (128*128 floats per output tile and split), to 1 if NULL */
+  int64_t part_floats;
 } sx_gemm_args;
 
 int sx_gemm(const sx_gemm_args* args, void* stream);
@@ -97,11 +104,11 @@ int sx_gemm(const sx_gemm_args* args, void* stream);
 /* ---------------------------------------------------------------------------------------------
  * Fused attention probabilities of the squeeze-out stage (csrc/sx_attn.cu):
  *     P[b][m] = dropout( softmax_keys( min(alpha * Q[b,:,m] K[b,:,m]^T, clip) ) )
- * One persistent tcgen05 kernel replaces segtran_shared.py:566-567 (Q.K^T / sqrt(d)), :569-580 (max statistics and
- * conditional clamp), :601 (softmax) and :605 (attention dropout): the scores stay in TMEM, the softmax runs on the
- * tcgen05.ld fragments, only P is written (plus the raw scaled scores S when the backward needs them).  More than 256
- * keys do not fit one TMEM accumulator per row block: the scores are then produced twice (statistics launch, then
- * probabilities launch, both over (row block, key chunk) tiles) instead of being written and re-read.
+ * One persistent wgmma kernel replaces segtran_shared.py:566-567 (Q.K^T / sqrt(d)), :569-580 (max statistics and
+ * conditional clamp), :601 (softmax) and :605 (attention dropout): the scores stay in registers, the softmax runs on
+ * the accumulator fragments, only P is written (plus the raw scaled scores S when the backward needs them).  More than
+ * 128 keys do not fit one accumulator per row block: the scores are then produced twice (a statistics pass, then a
+ * probabilities pass over the key chunks of the same row block) instead of being written and re-read.
  * Q [Bq][U1][M*d] (q_bstride = 0: one query bank shared by the batch), K [B][U2][M*d]; mode m uses columns
  * [m*d, (m+1)*d).  P, S: [B][M][U1][ldp] fp32, ldp % 4 == 0.  lse, rowmax: [B][M][U1] (natural-log units; rowmax is
  * the max of the raw row).  stat: device scratch of three 32-bit words, ZERO-initialised by the caller: [0] the running
@@ -129,8 +136,6 @@ typedef struct {
   uint32_t _pad;
   uint64_t drop_seed;
   const uint64_t* drop_seed_dev;
-  float* scratch;                /* U2 > 256 only: B*M*ceil(U1/256)*ceil(U2/256)*1536 floats of partial row statistics */
-  int64_t scratch_floats;
 } sx_attn_probs_args;
 int sx_attn_probs_fwd(const sx_attn_probs_args* args, void* stream);
 
@@ -156,7 +161,7 @@ int sx_pos_lsinu_fwd(const float* pos, const float* posmax, int64_t R, int32_t p
                      int32_t C, float* pe, void* stream);
 /* dpe [R,C] -> dW [C,pd], db [C] accumulated (+=); de_scratch [R,C] is caller-provided scratch. */
 int sx_pos_lsinu_bwd(const float* pos, const float* posmax, int64_t R, int32_t pd, const float* W, const float* b,
-                     int32_t C, const float* dpe, float* de_scratch, float* dW, float* db, void* stream);
+                     int32_t C, const float* dpe, float* de_scratch, float* dW, float* db, float* part, int64_t part_floats, void* stream);
 
 /* Fused prologue of SegtranFusionEncoder.forward (segtran_shared.py:916, :930-934, :944-946):
  *   h = mask * dropout( LN( LN_{g,b}(x) + posw * pe[..., :C] ) ),  x [B,N,C] fp32, pe rows of length C0,
@@ -168,7 +173,7 @@ int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, const float
 int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32_t N, int32_t C, const float* g, const float* b,
                     const float* pe, int32_t C0, int64_t pe_bstride, float posw, const float* mask, float drop_p,
                     uint64_t seed, const uint64_t* seed_dev, const float* stats, float* dx, float* dg, float* db, float* dpe,
-                    float* dt_scratch /* [B*N*C] or NULL */, void* stream);
+                    float* dt_scratch /* [B*N*C] or NULL */, float* part, int64_t part_floats, void* stream);
 
 /* Row softmax with the reference's conditional clamp and attention dropout (segtran_shared.py:578-580, :601-605):
  *   if (*amax > clip) S = clamp(S, -clip, clip);  P = dropout(softmax(S)).  S [R,L] fp32 (row stride lds),
@@ -186,7 +191,7 @@ int sx_softmax_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, co
 int sx_layernorm_fwd(const float* x, int64_t R, int32_t C, const float* g, const float* b, void* y, int32_t y_dtype,
                      int32_t round_tf32, float* stats, void* stream);
 int sx_layernorm_bwd(const float* dy, const float* x, int64_t R, int32_t C, const float* g, const float* stats,
-                     void* dx, int32_t dx_dtype, int32_t round_tf32, float* dg, float* db, void* stream);
+                     void* dx, int32_t dx_dtype, int32_t round_tf32, float* dg, float* db, float* part, int64_t part_floats, void* stream);
 
 /* MMPrivateOutput tail + LearnedSoftAggregate (segtran_shared.py:273-274, :318-325):
  *   Yn = LN_{g,b}(dropout(Y));  w = softmax_modes(Yn.ws + bs);  out = sum_m w_m Yn_m
@@ -197,7 +202,7 @@ int sx_ln_softaggr_fwd(const float* Y, int32_t B, int32_t M, int32_t N, int32_t 
 int sx_ln_softaggr_bwd(const float* dout, const float* Y, int32_t B, int32_t M, int32_t N, int32_t F, const float* g,
                        const float* b, const float* ws, float drop_p, uint64_t seed, const uint64_t* seed_dev, const float* stats,
                        const float* wts, void* dY, int32_t dy_dtype, int32_t round_tf32, float* dg, float* db,
-                       float* dws, float* dbs, float* dscore_scratch /* [B*M*N] or NULL */, void* stream);
+                       float* dws, float* dbs, float* dscore_scratch /* [B*M*N] or NULL */, float* part, int64_t part_floats, void* stream);
 
 /* LearnedSoftAggregate on its own (segtran_shared.py:318-325; the no-FFN branch :453 with M modes — the Polyformer layer):
  *   w = softmax_modes(x_m . ws + bs);  out = sum_m w_m x_m.   x [B,M,N,F] -> out [B,N,F], wts [B,M,N].
@@ -220,17 +225,17 @@ int sx_split_tf32(const float* x, int64_t n, float* hi, float* lo, void* stream)
 int sx_split_tf32_cat(const float* x, int32_t Z1, int32_t Z0, int32_t R, int32_t K, int64_t sz1, int64_t sz0, int64_t sr,
                       int64_t sk, int32_t Kp, int32_t role, float* out, void* stream);
 /* out[c] += sum_r X[r,c]   (bias gradients) */
-int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, int64_t ld, float* out, void* stream);
+int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, int64_t ld, float* out, float* part, int64_t part_floats, void* stream);
 /* out[0] += sum_i x[i]*y[i]  and  y = alpha * (*alpha_dev) * x : a linear loss head for benchmarks / checksums */
 int sx_dot(const float* x, const float* y, int64_t n, float* out, void* stream);
 int sx_scale(const float* x, int64_t n, const float* alpha_dev, float alpha, float* y, void* stream);
 /* out[z0][c] += sum_{z1,r} X[z1][z0][r][c]  (per-mode bias gradient of MMPrivateOutput in one launch) */
 int sx_colsum_batched(const float* X, int32_t Z1, int64_t stride_z1, int32_t Z0, int64_t stride_z0, int64_t R, int32_t C,
-                      int64_t ld, float* out, void* stream);
+                      int64_t ld, float* out, float* part, int64_t part_floats, void* stream);
 /* y = a + b  (residual connection of MMSharedOutput, segtran_shared.py:305) */
 int sx_add(const float* a, const float* b, int64_t n, float* y, void* stream);
 /* out[r % out_mod] += sum_c X[r,c]  (class-bias gradient of the head: rows = (batch, class)) */
-int sx_rowsum(const float* X, int64_t R, int64_t C, int64_t ld, int32_t out_mod, float* out, void* stream);
+int sx_rowsum(const float* X, int64_t R, int64_t C, int64_t ld, int32_t out_mod, float* out, float* part, int64_t part_floats, void* stream);
 /* batched transpose [Z,R,C] -> [Z,C,R] fp32: token flatten / scatter (segtran3d.py:328-330, :478-480) */
 int sx_transpose(const float* in, int64_t Z, int32_t R, int32_t C, float* out, void* stream);
 

@@ -282,9 +282,81 @@ def gen_infer():
     torch.save(dict(kind="infer", cases=cases), os.path.join(OUT, "infer_sw.pt"))
 
 
+def _digest(t):
+    """(shape, dtype, sha256 of the bytes): two tensors with the same digest are torch.equal."""
+    import hashlib
+    t = t.detach().contiguous().cpu()
+    return tuple(t.shape), str(t.dtype), hashlib.sha256(t.numpy().tobytes()).hexdigest()
+
+
+# (dims, modes, attractors, pos_dim, qk_have_bias) of the seeded-initialisation cases in tests/test_modules_cpu.py
+INIT_CASES = [([64, 64], 4, 16, 3, True), ([64, 64, 32], 4, 8, 2, False)]
+
+
+def gen_live():
+    """live_ref.pt: what the tests that once imported the reference directly compared against — the seeded
+    initialisation of SegtranFusionEncoder (parameter names + per-tensor digests) and one train-mode forward."""
+    ns = R.load()
+    init = []
+    for dims, M, A, pd, qkb in INIT_CASES:
+        cfg = R.encoder_config(ns.shared, dims=dims, num_modes=M, num_attractors=A, pos_dim=pd, qk_have_bias=qkb)
+        ref = R.build_encoder(cfg, seed=3)
+        init.append(dict(case=(dims, M, A, pd, qkb), keys=list(ref.state_dict().keys()),
+                         param_names=[n for n, _ in ref.named_parameters()],
+                         digests={k: _digest(v) for k, v in ref.state_dict().items()}))
+    dims = [32, 32, 16]
+    cfg = R.encoder_config(ns.shared, dims=dims, num_modes=2, num_attractors=5, pos_dim=2, qk_have_bias=True)
+    enc = R.build_encoder(cfg, seed=11).train()
+    torch.manual_seed(12)
+    x = torch.randn(3, 20, 32)
+    pos = O.voxels_pos_for_grid((4, 5), (8, 8), 3)
+    mask = torch.ones(3, 20, 1, dtype=torch.bool)
+    with R.quiet():
+        y = enc(x, pos, mask, torch.Size((4, 5)))
+    train = dict(dims=dims, state_dict={k: v.detach().clone() for k, v in enc.state_dict().items()}, x=x, out=y.detach())
+    torch.save(dict(kind="live_ref", init=init, train_mode=train, shell=gen_shell_init()), os.path.join(OUT, "live_ref.pt"))
+
+
+def gen_shell_init():
+    """The reference Segtran3d shell of the seg3d_tiny fixture built from seed 3: digests of its non-backbone state_dict,
+    and the torch RNG state right after its I3D backbone is constructed and right after init_weights has visited the
+    backbone — what a stand-in backbone has to reproduce for the shell's other modules to draw the same numbers."""
+    ns = R.load()
+    import networks.aj_i3d.aj_i3d as aj
+    ns.shared.bb2feat_dims["i3d-tiny"] = [8, 16, 24, 32, 48]
+    fx = torch.load(os.path.join(OUT, "seg3d_tiny.pt"), map_location="cpu", weights_only=False)
+    states = {}
+    orig_init, orig_apply = aj.InceptionI3d.__init__, aj.InceptionI3d.apply
+
+    def init(self, *a, **k):
+        orig_init(self, *a, **k)
+        states.setdefault("built", torch.get_rng_state())
+
+    def apply(self, fn):
+        out = orig_apply(self, fn)
+        states.setdefault("applied", torch.get_rng_state())
+        return out
+
+    aj.InceptionI3d.__init__, aj.InceptionI3d.apply = init, apply
+    try:
+        torch.manual_seed(3)
+        with R.quiet():
+            ns.seg3d.CONFIG.update_config(Namespace(**fx["args"]))
+            ref = ns.seg3d.Segtran3d(ns.seg3d.CONFIG)
+    finally:
+        aj.InceptionI3d.__init__, aj.InceptionI3d.apply = orig_init, orig_apply
+    sd = ref.state_dict()
+    return dict(keys=sorted(sd.keys()), backbone_keys=sum(k.startswith("backbone.") for k in sd),
+                digests={k: _digest(v) for k, v in sd.items() if not k.startswith("backbone.")},
+                rng_built=states["built"], rng_applied=states["applied"])
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(4)
+    if len(sys.argv) > 1 and sys.argv[1] == "live":
+        gen_live()
+        return
     if len(sys.argv) > 1 and sys.argv[1] == "train":
         gen_train()
         return

@@ -1,4 +1,4 @@
-"""segtran_b200 — B200-native (sm_100a) implementation of Segtran's Squeeze-and-Expansion hot path.
+"""segtran_b200 — H100-native (sm_90a) implementation of Segtran's Squeeze-and-Expansion hot path.
 
     segtran_b200.networks.segtran_shared   drop-in SegtranFusionEncoder & friends (reference module surface)
     segtran_b200.networks.segtran3d / 2d   drop-in Segtran3d / Segtran2d shells

@@ -35,7 +35,8 @@ class sx_gemm_args(C.Structure):
                 ("alpha", C.c_float), ("bias_mode", C.c_int32), ("bias", C.c_void_p), ("bias_stride_z0", C.c_int64),
                 ("bias_stride_z1", C.c_int64), ("act", C.c_int32), ("accumulate", C.c_int32), ("preact", C.c_void_p),
                 ("split_k", C.c_int32), ("_pad2", C.c_int32), ("amax", C.c_void_p), ("drop_p", C.c_float),
-                ("_pad3", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("addend", C.c_void_p), ("colsum", C.c_void_p)]
+                ("_pad3", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("addend", C.c_void_p), ("colsum", C.c_void_p),
+                ("part", C.c_void_p), ("part_floats", C.c_int64)]
 
 
 class sx_attn_probs_args(C.Structure):
@@ -44,8 +45,7 @@ class sx_attn_probs_args(C.Structure):
                 ("K", C.c_void_p), ("k_ld", C.c_int64), ("k_bstride", C.c_int64), ("alpha", C.c_float),
                 ("clip", C.c_float), ("P", C.c_void_p), ("S", C.c_void_p), ("ldp", C.c_int64), ("lse", C.c_void_p),
                 ("rowmax", C.c_void_p), ("stat", C.c_void_p), ("diag", C.c_void_p), ("drop_p", C.c_float),
-                ("_pad", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p),
-                ("scratch", C.c_void_p), ("scratch_floats", C.c_int64)]
+                ("_pad", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p)]
 
 
 _P, _I, _L, _F, _U64, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64, C.c_double
@@ -57,15 +57,15 @@ _PROTOS = {
     "sx_attn_probs_fwd": [C.POINTER(sx_attn_probs_args), _P],
     "sx_reduce_max": [_P, _L, _P, _P],
     "sx_pos_lsinu_fwd": [_P, _P, _L, _I, _P, _P, _I, _P, _P],
-    "sx_pos_lsinu_bwd": [_P, _P, _L, _I, _P, _P, _I, _P, _P, _P, _P, _P],
+    "sx_pos_lsinu_bwd": [_P, _P, _L, _I, _P, _P, _I, _P, _P, _P, _P, _P, _L, _P],
     "sx_prologue_fwd": [_P, _L, _I, _I, _P, _P, _P, _I, _L, _F, _P, _F, _U64, _P, _P, _I, _I, _P, _P],
-    "sx_prologue_bwd": [_P, _P, _L, _I, _I, _P, _P, _P, _I, _L, _F, _P, _F, _U64, _P, _P, _P, _P, _P, _P, _P, _P],
+    "sx_prologue_bwd": [_P, _P, _L, _I, _I, _P, _P, _P, _I, _L, _F, _P, _F, _U64, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P],
     "sx_softmax_fwd": [_P, _L, _I, _L, _P, _F, _F, _U64, _P, _P, _I, _L, _I, _P, _P, _P],
     "sx_softmax_bwd": [_P, _L, _P, _L, _P, _L, _I, _P, _F, _F, _U64, _P, _L, _P, _I, _L, _I, _P],
     "sx_layernorm_fwd": [_P, _L, _I, _P, _P, _P, _I, _I, _P, _P],
-    "sx_layernorm_bwd": [_P, _P, _L, _I, _P, _P, _P, _I, _I, _P, _P, _P],
+    "sx_layernorm_bwd": [_P, _P, _L, _I, _P, _P, _P, _I, _I, _P, _P, _P, _L, _P],
     "sx_ln_softaggr_fwd": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _F, _U64, _P, _P, _P, _P, _P],
-    "sx_ln_softaggr_bwd": [_P, _P, _I, _I, _I, _I, _P, _P, _P, _F, _U64, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P],
+    "sx_ln_softaggr_bwd": [_P, _P, _I, _I, _I, _I, _P, _P, _P, _F, _U64, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _L, _P],
     "sx_softaggr_fwd": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P],
     "sx_softaggr_bwd": [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P],
     "sx_gelu_bwd": [_P, _P, _I, _L, _F, _U64, _P, _P, _I, _I, _P],
@@ -76,12 +76,12 @@ _PROTOS = {
     "sx_sw_finalize": [_P, _P, _I, _L, _I, _P, _P],
     "sx_split_tf32": [_P, _L, _P, _P, _P],
     "sx_split_tf32_cat": [_P, _I, _I, _I, _I, _L, _L, _L, _L, _I, _I, _P, _P],
-    "sx_colsum": [_P, _I, _L, _I, _L, _P, _P],
+    "sx_colsum": [_P, _I, _L, _I, _L, _P, _P, _L, _P],
     "sx_transpose": [_P, _L, _I, _I, _P, _P],
-    "sx_colsum_batched": [_P, _I, _L, _I, _L, _L, _I, _L, _P, _P],
+    "sx_colsum_batched": [_P, _I, _L, _I, _L, _L, _I, _L, _P, _P, _L, _P],
     "sx_dot": [_P, _P, _L, _P, _P],
     "sx_add": [_P, _P, _L, _P, _P],
-    "sx_rowsum": [_P, _L, _L, _L, _I, _P, _P],
+    "sx_rowsum": [_P, _L, _L, _L, _I, _P, _P, _L, _P],
     "sx_scale": [_P, _L, _P, _F, _P, _P],
     "sx_head_contract_fwd": [_P, _P, _P, _I, _I, _L, _I, _P, _I, _P],
     "sx_head_contract_bwd_data": [_P, _P, _I, _I, _L, _I, _P, _P],
@@ -129,8 +129,8 @@ def check(rc, what):
 
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
-_LAUNCHES = {"sx_pos_lsinu_bwd": 2, "sx_ln_softaggr_bwd": 1, "sx_prologue_bwd": 2, "sx_layernorm_bwd": 2, "sx_gemm_debug_set": 0,
-             "sx_attn_probs_fwd": 3}
+_LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
+             "sx_attn_probs_fwd": 2, "sx_colsum": 2, "sx_colsum_batched": 2}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing
 

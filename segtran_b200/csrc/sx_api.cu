@@ -27,6 +27,6 @@ extern "C" int sx_device_info(int* sm_count, int* cc_major, int* cc_minor) {
   if (sm_count) *sm_count = n;
   if (cc_major) *cc_major = ma;
   if (cc_minor) *cc_minor = mi;
-  SX_REQUIRE(ma == 10, "segtran_b200 needs an sm_100 (B200) device, found sm_%d%d", ma, mi);
+  SX_REQUIRE(ma == 9 && mi == 0, "segtran_b200 needs an sm_90 (H100) device, found sm_%d%d", ma, mi);
   return 0;
 }

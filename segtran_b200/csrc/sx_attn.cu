@@ -3,21 +3,19 @@
 //   P[b][m] = dropout( softmax_rows( min( alpha * Q[b,:,m] K[b,:,m]^T , clip ) ) )
 //
 // i.e. reference segtran_shared.py:566-567 (Q.K^T / sqrt(d)), :569-580 (max statistics, conditional clamp), :601
-// (softmax over the keys) and :605 (attention dropout) in ONE persistent tcgen05 kernel: the scores never leave the
-// SM — they are accumulated in TMEM, read back with tcgen05.ld in the 32x32b distribution (one thread = one query
-// row), and the row max / sum / exp / dropout / TF32 rounding run on those fragments.  Only P (and, for training, the
-// raw scores the backward recomputes P from) is written, through swizzled staging tiles and TMA bulk stores.
+// (softmax over the keys) and :605 (attention dropout) in ONE persistent wgmma kernel: the scores never leave the SM —
+// they are accumulated in registers (wgmma fragments: a query row is spread over the four threads of a quad), and the
+// row max / sum / exp / dropout / TF32 rounding run on those fragments.  Only P (and, for training, the raw scores the
+// backward recomputes P from) is written.
 //
-// Work decomposition (CTA pairs, tcgen05 cta_group::2): an item is (batch b, mode m, block of 256 query rows); the
-// pair owns the item's complete rows, so the softmax statistics are thread-local:
-//   keys <= 256 : one 256x256 accumulator holds the whole row block: statistics and probabilities come from the same
-//                 TMEM-resident scores (single pass);
-//   keys  > 256 : a [128 x keys] fp32 row block per CTA exceeds the 512 TMEM columns (cfg 4: 1024 keys, cfg 5: 2048),
-//                 so the scores are produced twice: pass 0 keeps only the running (max, sum) of each row, pass 1
-//                 recomputes each 256-key chunk and emits exp2(s - max) / sum.  The recomputation costs d/F of the
-//                 P.V contraction that follows (cfg 4: 25 %) and replaces the S write + S read + P write of the unfused
-//                 path (three passes over the [B,M,N,A] tensor) by one P write.
-// The accumulators are double buffered (2 x 256 TMEM columns): the softmax of chunk j overlaps the MMAs of chunk j+1.
+// Work decomposition: an item is (batch b, mode m, block of 128 query rows); the CTA owns the item's complete rows
+// (two consumer warpgroups of 64 rows), so the softmax statistics need only quad shuffles:
+//   keys <= 128 : the scores of the row block are one accumulator: statistics and probabilities come from the same
+//                 registers (single pass);
+//   keys  > 128 : the scores are produced twice: pass 0 keeps only the running (max, sum) of each row over the 128-key
+//                 chunks, pass 1 recomputes each chunk and emits exp2(s - max) / sum.  The recomputation costs d/F of the
+//                 P.V contraction that follows and replaces the S write + S read + P write of an unfused path by one
+//                 P write.
 //
 // Clamp (segtran_shared.py:578-580: `if scores.max() > clip: scores = clamp(scores, -clip, clip)`): the upper clamp
 // is applied unconditionally — an element above clip implies the global maximum is above clip, so this is exactly the
@@ -27,19 +25,13 @@
 #include "sx_common.cuh"
 #include "sx_tc.cuh"
 
-long long sx_attn_dbg = 0;                  // bring-up: 1 = skip the TMA stores, 2 = skip staging + stores
-long long sx_attn_mode = 1;                 // bring-up knob (sx_gemm_debug_set "attn_mode"): 1 = one launch, 2 = two tile launches
-
 namespace {
 using namespace sxtc;
 
-constexpr int NUM_THREADS = 384;          // warps 0-3: TMA / MMA / TMEM alloc / idle; warps 4-11: softmax epilogue
-constexpr int NUM_EPI_WARPS = 8;
-constexpr int STAGES = 4;                 // 4 x (16 KB of Q rows + 16 KB = this CTA's half of the key chunk)
-constexpr int STAGE_BYTES = 2 * A_STAGE_BYTES;
-constexpr int STG_BYTES = 2 * 4096;       // per epilogue warp: two 32x32 fp32 staging tiles for the TMA stores
-constexpr int XCH_FLOATS = 2 * 2 * 3 * BM;   // [item parity][column half][m, l, raw max][row]
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + NUM_EPI_WARPS * STG_BYTES + XCH_FLOATS * 4 + 1024 /*align*/ + 256;
+constexpr int NUM_THREADS = 384;          // warpgroup 0: TMA producer; warpgroups 1-2: MMA + softmax, 64 rows each
+constexpr int STAGES = 4;                 // 4 x (16 KB of Q rows + 16 KB of keys), 32 elements of d each
+constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256;
 constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
 
 // order-preserving float -> uint map with key(x) > 0 for every finite x, so a ZERO-initialised word is the identity of
@@ -54,21 +46,15 @@ __device__ __forceinline__ float ordered_val(unsigned int k) {
 
 struct AttnParams {
   int B, M, U1, U2, d;
-  int tiles_m, tiles_n, num_kb, npass, items;
-  int nwork, nsub;                // work items per launch and accumulator tiles per item (see phase)
-  int phase;                      // 0: whole row block in one accumulator (keys <= 256): statistics + probabilities;
-                                  // 3: item = row block, 2 * tiles_n tiles: pass 0 statistics, pass 1 probabilities;
-                                  // 1: statistics of one (row block, key chunk) tile -> partial (max, sum, raw max);
-                                  // 2: probabilities of one tile from the combined partials
-  float* part;                    // phases 1/2: [items][tiles_n][2 halves][3][256 rows] partial row statistics
+  int tiles_m, tiles_n, num_kb, items, nsub;
   int q_bcast;                    // Q has batch 1 (shared by the batch)
   float alpha2, clip2;            // alpha * log2(e), clip * log2(e)
   float alpha, clip;
+  float* P;
+  float* S;                       // raw scaled scores (may be null)
   float* lse;                     // [B][M][U1]  natural-log LSE of the clamped row
   float* rowmax;                  // [B][M][U1]  max of the raw scaled row (may be null)
   float* stat;                    // zero-initialised; [0] ordered_key(max raw scaled score), [1] += rows whose max < -(clip - 104)
-  int store_s;
-  int dbg;
   long long ldp;                  // row pitch of P (and S) in elements, multiple of 4
   float drop_p;
   unsigned long long drop_seed;
@@ -77,50 +63,27 @@ struct AttnParams {
 };
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmS,
-                     const AttnParams p) {
-  const uint32_t rank = sx::cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cid = (int)(blockIdx.x >> 1), ncl = (int)(gridDim.x >> 1);
-
+sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* stg = smem + STAGES * STAGE_BYTES;
-  float* xch = reinterpret_cast<float*>(stg + NUM_EPI_WARPS * STG_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xch + XCH_FLOATS);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     sx::tma_prefetch_desc(&tmQ);
     sx::tma_prefetch_desc(&tmK);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < STAGES; ++s) {
       sx::mbar_init(&full_bar[s], 1);
-      sx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      sx::mbar_init(&tfull_bar[a], 1);
-      sx::mbar_init(&tempty_bar[a], NUM_EPI_WARPS * 2);        // both CTAs' epilogue warps release the leader's MMA
+      sx::mbar_init(&empty_bar[s], 2);
     }
     sx::fence_barrier_init();
   }
-  if (warp == 2) {
-    sx::tmem_alloc2(tmem_slot, TMEM_COLS);
-    sx::tmem_relinquish2();
-  }
-  sx::tc_fence_before();
-  sx::cluster_sync();
-  sx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
   auto decode = [&](int it, int& b, int& m, int& mb) {
     mb = it % p.tiles_m; it /= p.tiles_m;
@@ -128,290 +91,174 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     b = it / p.M;
   };
 
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-    if (warp == 0) {
-      // ===================== TMA producer (both CTAs: own 128 query rows + own half of the key chunk) ==============
-      if (sx::elect_one()) {
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int w = cid; w < p.nwork; w += ncl) {
-          int b, m, mb;
-          decode(p.nsub == 1 ? w / p.tiles_n : w, b, m, mb);
-          const int m0 = mb * 2 * BM + (int)rank * BM;
-          const int qb = p.q_bcast ? 0 : b;
-          for (int sub = 0; sub < p.nsub; ++sub) {
-            const int nb = p.nsub == 1 ? w % p.tiles_n : sub % p.tiles_n;
-            const int n0 = nb * BN + (int)rank * (BN / 2);
-            for (int kb = 0; kb < p.num_kb; ++kb) {
-              sx::mbar_wait(&empty_bar[stage], phase ^ 1);
-              if (leader) sx::mbar_expect_tx(&full_bar[stage], STAGE_BYTES * 2);
-              uint8_t* sa = smem + stage * STAGE_BYTES;
-              sx::tma_load_4d_pair(sa, &tmQ, &full_bar[stage], kb * 32, m0, m, qb, sx::kEvictLast);
-              sx::tma_load_4d_pair(sa + A_STAGE_BYTES, &tmK, &full_bar[stage], kb * 32, n0, m, b, sx::kEvictLast);
-              if (++stage == STAGES) { stage = 0; phase ^= 1; }
-            }
-          }
-        }
-      }
-    } else if (warp == 1 && leader) {
-      // ===================== MMA issuer (leader CTA) =====================
-      constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) |
-                                 ((uint32_t)((2 * BM) >> 4) << 24);          // F32 acc, TF32 x TF32, K-major, 256 x 256
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");   // the producer hands its registers over
+    // ===================== TMA producer: per chunk and k-block, 128 query rows + 128 keys =====================
+    if (warp == 0 && sx::elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      int it = 0;
-      for (int w = cid; w < p.nwork; w += ncl)
-        for (int sub = 0; sub < p.nsub; ++sub, ++it) {
-          const int acc = it & 1;
-          const uint32_t acc_phase = (it >> 1) & 1;
-          sx::mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-          sx::tc_fence_after();
-          const uint32_t tmem_d = tmem_base + acc * BN;
+      for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+        int b, m, mb;
+        decode(it, b, m, mb);
+        const int qb = p.q_bcast ? 0 : b;
+        for (int sub = 0; sub < p.nsub; ++sub) {
+          const int nb = sub % p.tiles_n;
           for (int kb = 0; kb < p.num_kb; ++kb) {
-            sx::mbar_wait(&full_bar[stage], phase);
-            sx::tc_fence_after();
-            if (sx::elect_one()) {
-              const uint32_t sa = sx::smem_u32(smem + stage * STAGE_BYTES);
-              const uint64_t da = make_smem_desc(sa, 16, 1024, 1, 2u);
-              const uint64_t db = make_smem_desc(sa + A_STAGE_BYTES, 16, 1024, 1, 2u);
-#pragma unroll
-              for (int k = 0; k < KSTEPS; ++k)
-                sx::umma_pair<true>(tmem_d, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb > 0 || k > 0) ? 1u : 0u);
-              sx::umma_commit_pair(&empty_bar[stage]);
-              if (kb == p.num_kb - 1) sx::umma_commit_pair(&tfull_bar[acc]);
-            }
-            __syncwarp();
+            sx::mbar_wait(&empty_bar[stage], phase ^ 1);
+            sx::mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
+            uint8_t* sa = smem + stage * STAGE_BYTES;
+            sx::tma_load_4d(sa, &tmQ, &full_bar[stage], kb * 32, mb * BM, m, qb, sx::kEvictLast);
+            sx::tma_load_4d(sa + A_STAGE_BYTES, &tmK, &full_bar[stage], kb * 32, nb * BN, m, b, sx::kEvictLast);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
-    }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;" ::: "memory");
-    // ===================== softmax epilogue =====================
-    // thread = one query row (TMEM lane 32q + lane); the two warps of a lane quarter split the 256 key columns of a
-    // chunk into halves (h) of four 32-column fragments each
-    const int q = warp & 3;
-    const int h = (warp - 4) >> 2;
-    const int rloc = q * 32 + lane;                       // row inside this CTA's 128
-    uint8_t* mystg = stg + (warp - 4) * STG_BYTES;
-    int sbuf = 0;
-    int it = 0;
-    float gmax = -3.0e38f;
-    int lowrows = 0;
-    const uint32_t p16 = sx::drop_p16(p.drop_p);
-    const float keep_scale = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
-    const unsigned long long dseed = p.drop_seed + (p.drop_seed_dev ? *p.drop_seed_dev : 0ull);
-    const uint32_t mul0 = sx::drop_mul(0), mul1 = sx::drop_mul(1);
-    const uint32_t key0 = sx::drop_key(dseed, 0), key1 = sx::drop_key(dseed, 1);
-
-    // one 32 x 32 fp32 tile of this warp (thread = row `lane`, f[0..31] = 32 consecutive columns) -> swizzled staging
-    // tile -> two 16-row TMA bulk stores (clipped at the tensor edge by the hardware)
-    auto stage_store = [&](const CUtensorMap* tm, const float (&f)[32], int col0, int row0, int z0, int z1) {
-      if (p.dbg == 2) return;
-      uint8_t* buf = mystg + (sbuf & 1) * 4096;
-      if (lane == 0) sx::tma_store_wait_read<1>();         // the group issued two tiles ago has released this buffer
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(buf + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-            make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]);
-      sx::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0 && p.dbg != 1) {
-        sx::tma_store_4d(tm, buf, col0, row0, z0, z1);
-        sx::tma_store_4d(tm, buf + 2048, col0, row0 + 16, z0, z1);
-        sx::tma_store_commit();
       }
-      ++sbuf;
+    }
+    return;
+  }
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  // ===================== consumers: scores (wgmma) -> softmax on the fragments =====================
+  // thread: rows 8h + lane/4 (h = 0, 1) of its warp's 16; columns 8j + 2(lane%4) + e of each 128-key chunk
+  const int cw = wg - 1;
+  const int wtid = threadIdx.x & 127;
+  const int wq = warp & 3;
+  const int tr = lane >> 2;
+  const int tc = (lane & 3) * 2;
+  int stage = 0;
+  uint32_t phase = 0;
+  float gmax = -3.0e38f;
+  int lowrows = 0;
+  const uint32_t p16 = sx::drop_p16(p.drop_p);
+  const float keep_scale = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
+  const unsigned long long dseed = p.drop_seed + (p.drop_seed_dev ? *p.drop_seed_dev : 0ull);
+  // this thread's column pair is elements (tc & 2, tc & 2 + 1) of a 4-element hash group: one word per pair
+  const uint32_t dmul = sx::drop_mul((tc >> 1) & 1), dkey = sx::drop_key(dseed, (tc >> 1) & 1);
+  float acc[64];
+
+  for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
+    int b, m, mb;
+    decode(it, b, m, mb);
+    int grow[2];
+    long long rowflat[2];
+    float rm[2], rl[2], rraw[2], rcp[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      grow[h] = mb * BM + cw * 64 + wq * 16 + 8 * h + tr;
+      rowflat[h] = ((long long)b * p.M + m) * p.U1 + grow[h];
+      rm[h] = -3.0e38f; rl[h] = 0.f; rraw[h] = -3.0e38f; rcp[h] = 0.f;
+    }
+
+    // running statistics of the row over one chunk (log2 units; quad-uniform after the shuffles)
+    auto chunk_stats = [&](int nb) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float cm = -3.0e38f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (nb * BN + 8 * j + tc + e < p.U2) cm = fmaxf(cm, acc[4 * j + 2 * h + e]);
+        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 1));
+        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 2));
+        cm *= p.alpha2;                                       // alpha2 > 0: the max commutes with the scaling
+        rraw[h] = fmaxf(rraw[h], cm);
+        const float mn = fmaxf(rm[h], fminf(cm, p.clip2));
+        float s = 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (nb * BN + 8 * j + tc + e < p.U2) s += sx::ex2_approx(fminf(acc[4 * j + 2 * h + e] * p.alpha2, p.clip2) - mn);
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        rl[h] = rl[h] * sx::ex2_approx(rm[h] - mn) + s;
+        rm[h] = mn;
+      }
     };
-
-    int item_par = 0;
-    for (int w = cid; w < p.nwork; w += ncl, item_par ^= 1) {
-      const int item = p.nsub == 1 ? w / p.tiles_n : w;
-      int b, m, mb;
-      decode(item, b, m, mb);
-      const int grow = mb * 2 * BM + (int)rank * BM + rloc;      // this thread's query row
-      const int wrow0 = mb * 2 * BM + (int)rank * BM + q * 32;   // first row of this warp
-      const long long rowflat = ((long long)b * p.M + m) * p.U1 + grow;
-      float rm = -3.0e38f, rl = 0.f, rraw = -3.0e38f;            // running max (clamped), sum, raw max — log2 units
-      float inv_l = 0.f, rcp_l = 0.f;                           // exponent offset max + log2(sum) of this row; 1/sum
-      float* xm = xch + item_par * (2 * 3 * BM);
-
-      // statistics of one TMEM-resident chunk (this thread's 4 fragments).  Lean form: one max, one FFMA, one EX2 and one
-      // add per score; the clamp only enters through a warp-uniform slow path taken when some row exceeds it
-      auto chunk_stats = [&](uint32_t taddr, int nb) {
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          const int col0 = nb * BN + h * 128 + c * 32;
-          if (col0 >= p.U2) break;                                // warp-uniform
-          uint32_t v[32];
-          sx::tmem_ld32(taddr + (uint32_t)(h * 128 + c * 32), v);
-          sx::tmem_ld_wait();
-          if (col0 + 32 > p.U2) {                                 // ragged key count: mask the tail columns
+    // final (max, sum, raw max) of the rows -> 1/sum; lse / rowmax / global statistics
+    auto publish = [&]() {
 #pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (col0 + i >= p.U2) v[i] = 0xFF7FFFFFu;           // -FLT_MAX
-          }
-          float cm = __uint_as_float(v[0]);
-#pragma unroll
-          for (int i = 1; i < 32; ++i) cm = fmaxf(cm, __uint_as_float(v[i]));
-          cm *= p.alpha2;                                         // alpha2 > 0: the max commutes with the scaling
-          rraw = fmaxf(rraw, cm);
-          const float mn = fmaxf(rm, fminf(cm, p.clip2));
-          float acc0 = 0.f, acc1 = 0.f;
-          if (__any_sync(0xffffffffu, cm > p.clip2)) {
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              acc0 += sx::ex2_approx(fminf(__uint_as_float(v[i]) * p.alpha2, p.clip2) - mn);
-              acc1 += sx::ex2_approx(fminf(__uint_as_float(v[i + 1]) * p.alpha2, p.clip2) - mn);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              acc0 += sx::ex2_approx(fmaf(__uint_as_float(v[i]), p.alpha2, -mn));
-              acc1 += sx::ex2_approx(fmaf(__uint_as_float(v[i + 1]), p.alpha2, -mn));
-            }
-          }
-          rl = rl * sx::ex2_approx(rm - mn) + (acc0 + acc1);
-          rm = mn;
-        }
-      };
-      // final (max, sum, raw max) of the row -> 1/sum, and once per row: lse / rowmax / global statistics
-      auto publish = [&](bool once) {
-        inv_l = rm + __log2f(rl);                                 // P = 2^(s2 - max - log2(sum)): no per-element multiply
-        rcp_l = 1.f / rl;                                         // (clamped rows keep the two-step form: |max| = 721)
-        if (once && grow < p.U1) {
-          gmax = fmaxf(gmax, rraw);
-          if (h == 0) {
-            p.lse[rowflat] = (rm + __log2f(rl)) * LN2;
-            if (p.rowmax) p.rowmax[rowflat] = rraw * LN2;
-            if (rraw * LN2 < -(p.clip - 104.f)) ++lowrows;
+      for (int h = 0; h < 2; ++h) {
+        rcp[h] = 1.f / rl[h];
+        if (grow[h] < p.U1) {
+          gmax = fmaxf(gmax, rraw[h]);
+          if ((lane & 3) == 0) {
+            p.lse[rowflat[h]] = (rm[h] + __log2f(rl[h])) * LN2;
+            if (p.rowmax) p.rowmax[rowflat[h]] = rraw[h] * LN2;
+            if (rraw[h] * LN2 < -(p.clip - 104.f)) ++lowrows;
           }
         }
-      };
-      // phase 1: this thread's (max, sum, raw max) over its half of one key chunk -> global partials
-      auto store_partial = [&](int nb) {
-        float* pp = p.part + ((((long long)item * p.tiles_n + nb) * 2 + h) * 3) * (2 * BM) + (int)rank * BM + rloc;
-        pp[0] = rm; pp[2 * BM] = rl; pp[4 * BM] = rraw;
-      };
-      // phase 2: combine the partials of every key chunk and half of this thread's row
-      auto load_partials = [&]() {
-        const float* pp = p.part + ((long long)item * p.tiles_n * 2 * 3) * (2 * BM) + (int)rank * BM + rloc;
-        float mx = -3.0e38f, rw = -3.0e38f;
-        for (int j = 0; j < 2 * p.tiles_n; ++j) {
-          mx = fmaxf(mx, pp[(long long)(j * 3) * (2 * BM)]);
-          rw = fmaxf(rw, pp[(long long)(j * 3 + 2) * (2 * BM)]);
-        }
-        float l = 0.f;
-        for (int j = 0; j < 2 * p.tiles_n; ++j)
-          l += pp[(long long)(j * 3 + 1) * (2 * BM)] * sx::ex2_approx(pp[(long long)(j * 3) * (2 * BM)] - mx);
-        rm = mx; rl = l; rraw = rw;
-      };
-      // both column halves of a row -> the row's final (max, 1/sum); publishes lse / rowmax
-      auto finish_stats = [&]() {
-        xm[(h * 3 + 0) * BM + rloc] = rm;
-        xm[(h * 3 + 1) * BM + rloc] = rl;
-        xm[(h * 3 + 2) * BM + rloc] = rraw;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        const float om = xm[((h ^ 1) * 3 + 0) * BM + rloc], ol = xm[((h ^ 1) * 3 + 1) * BM + rloc];
-        const float oraw = xm[((h ^ 1) * 3 + 2) * BM + rloc];
-        const float mn = fmaxf(rm, om);
-        rl = rl * sx::ex2_approx(rm - mn) + ol * sx::ex2_approx(om - mn);
-        rm = mn;
-        rraw = fmaxf(rraw, oraw);
-        publish(true);
-      };
-      // probabilities of one TMEM-resident chunk -> P (and the raw scores -> S)
-      auto chunk_probs = [&](uint32_t taddr, int nb) {
-#pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
-          const int col0 = nb * BN + h * 128 + c * 32;
-          if (col0 >= p.U2) break;
-          uint32_t v[32];
-          sx::tmem_ld32(taddr + (uint32_t)(h * 128 + c * 32), v);
-          sx::tmem_ld_wait();
-          float f[32];
-          if (p.store_s) {
+      }
+    };
+    // probabilities of one chunk -> P (and the raw scores -> S)
+    auto chunk_probs = [&](int nb) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]) * p.alpha;
-            stage_store(&tmS, f, col0, wrow0, m, b);
+      for (int h = 0; h < 2; ++h) {
+        if (grow[h] >= p.U1) continue;
+        const long long roff = rowflat[h] * p.ldp;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = nb * BN + 8 * j + tc;
+          if (col >= p.U2) continue;
+          const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (p.S) {
+            if (col + 1 < p.U2) *reinterpret_cast<float2*>(p.S + roff + col) = make_float2(v0 * p.alpha, v1 * p.alpha);
+            else p.S[roff + col] = v0 * p.alpha;
           }
-          if (__any_sync(0xffffffffu, rraw > p.clip2)) {          // some row of this warp was clamped (rare)
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              f[i] = sx::ex2_approx(fminf(__uint_as_float(v[i]) * p.alpha2, p.clip2) - rm) * rcp_l;
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) f[i] = sx::ex2_approx(fmaf(__uint_as_float(v[i]), p.alpha2, -inv_l));
-          }
+          float f0 = sx::ex2_approx(fminf(v0 * p.alpha2, p.clip2) - rm[h]) * rcp[h];
+          float f1 = sx::ex2_approx(fminf(v1 * p.alpha2, p.clip2) - rm[h]) * rcp[h];
           if (p.drop_p > 0.f) {
-            const unsigned long long g0 = (unsigned long long)((rowflat * p.ldp + col0) >> 2);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const uint32_t w0 = sx::drop_word_k(mul0, key0, g0 + j), w1 = sx::drop_word_k(mul1, key1, g0 + j);
-              f[4 * j + 0] = (w0 & 0xFFFFu) >= p16 ? f[4 * j + 0] * keep_scale : 0.f;
-              f[4 * j + 1] = (w0 >> 16) >= p16 ? f[4 * j + 1] * keep_scale : 0.f;
-              f[4 * j + 2] = (w1 & 0xFFFFu) >= p16 ? f[4 * j + 2] * keep_scale : 0.f;
-              f[4 * j + 3] = (w1 >> 16) >= p16 ? f[4 * j + 3] * keep_scale : 0.f;
-            }
+            const uint32_t w = sx::drop_word_k(dmul, dkey, (unsigned long long)((roff + col) >> 2));
+            f0 = (w & 0xFFFFu) >= p16 ? f0 * keep_scale : 0.f;
+            f1 = (w >> 16) >= p16 ? f1 * keep_scale : 0.f;
           }
           if (p.round_tf32) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) f[i] = sx::round_tf32(f[i]);
+            f0 = sx::round_tf32(f0);
+            f1 = sx::round_tf32(f1);
           }
-          stage_store(&tmP, f, col0, wrow0, m, b);
+          if (col + 1 < p.U2) *reinterpret_cast<float2*>(p.P + roff + col) = make_float2(f0, f1);
+          else p.P[roff + col] = f0;
         }
-      };
-      auto release = [&](int acc) {
-        sx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) sx::mbar_arrive_leader(&tempty_bar[acc]);
-      };
+      }
+    };
 
-      for (int sub = 0; sub < p.nsub; ++sub, ++it) {
-        const int nb_t = p.nsub == 1 ? w % p.tiles_n : sub % p.tiles_n;
-        const int acc = it & 1;
-        sx::mbar_wait(&tfull_bar[acc], (it >> 1) & 1);
-        sx::tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
-        if (p.phase == 0) {                       // the whole row block is resident: statistics, then probabilities
-          chunk_stats(taddr, nb_t);
-          finish_stats();
-          chunk_probs(taddr, nb_t);
-        } else if (p.phase == 1) {                // tile phases: partial statistics -> global
-          chunk_stats(taddr, nb_t);
-          store_partial(nb_t);
-        } else if (p.phase == 2) {                // tile phases: probabilities from the combined partials
-          load_partials();
-          publish(nb_t == 0);
-          chunk_probs(taddr, nb_t);
-        } else if (sub < p.tiles_n) {             // phase 3, row-block items: pass 0 keeps the running statistics ...
-          chunk_stats(taddr, nb_t);
-          if (sub == p.tiles_n - 1) finish_stats();
-        } else {                                  // ... pass 1 recomputes each chunk and emits the probabilities
-          chunk_probs(taddr, nb_t);
-        }
-        release(acc);
+    for (int sub = 0; sub < p.nsub; ++sub) {
+      const int nb = sub % p.tiles_n;
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        sx::mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = sx::smem_u32(smem + stage * STAGE_BYTES);
+        const uint32_t qa = sa + (uint32_t)(cw * 64 * BKB), ka = sa + A_STAGE_BYTES;
+        sx::acc_fence(acc);
+        sx::wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          sx::wgmma_tf32(acc, sx::gmma_desc(qa + kk * 32, 16, 1024), sx::gmma_desc(ka + kk * 32, 16, 1024),
+                         (kb > 0 || kk > 0) ? 1u : 0u);
+        sx::wgmma_commit();
+        sx::wgmma_wait<0>();
+        sx::acc_fence(acc);
+        if (wtid == 0) sx::mbar_arrive(&empty_bar[stage]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      if (p.nsub == 1) {                        // the whole row block is resident: statistics, then probabilities
+        chunk_stats(nb);
+        publish();
+        chunk_probs(nb);
+      } else if (sub < p.tiles_n) {             // pass 0 keeps the running statistics ...
+        chunk_stats(nb);
+        if (sub == p.tiles_n - 1) publish();
+      } else {                                  // ... pass 1 recomputes each chunk and emits the probabilities
+        chunk_probs(nb);
       }
     }
-    gmax = sx::warp_max(gmax);
-    if (lane == 0 && gmax > -3.0e38f) atomicMax(reinterpret_cast<unsigned int*>(&p.stat[0]), ordered_key(gmax * LN2));
-    if (h == 0) {
-      int lr = lowrows;
+  }
+  gmax = sx::warp_max(gmax);
+  if (lane == 0 && gmax > -3.0e38f) atomicMax(reinterpret_cast<unsigned int*>(&p.stat[0]), ordered_key(gmax * LN2));
+  int lr = lowrows;
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) lr += __shfl_xor_sync(0xffffffffu, lr, o);
-      if (lane == 0 && lr > 0) atomicAdd(&p.stat[1], (float)lr);
-    }
-    if (lane == 0) sx::tma_store_wait_all();
-  }
-
-  sx::tc_fence_before();
-  sx::cluster_sync();
-  if (warp == 2) {
-    sx::tc_fence_after();
-    sx::tmem_dealloc2(tmem_base, TMEM_COLS);
-  }
+  for (int o = 16; o > 0; o >>= 1) lr += __shfl_xor_sync(0xffffffffu, lr, o);
+  if (lane == 0 && lr > 0) atomicAdd(&p.stat[1], (float)lr);
 }
 
 // diag[0] = running max of the scores, diag[1] += 1 when the clamp fired, diag[2] += rows the lower clamp could have
@@ -439,25 +286,22 @@ extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, void* stream) {
   SX_REQUIRE((reinterpret_cast<uintptr_t>(a->P) & 15) == 0 && (!a->S || (reinterpret_cast<uintptr_t>(a->S) & 15) == 0),
              "sx_attn_probs_fwd: outputs must be 16-byte aligned");
   const int sms = sm_count_cached();
-  SX_REQUIRE(sms >= 2, "sx_attn_probs_fwd: no CUDA device (this library has no CPU fallback)");
+  SX_REQUIRE(sms > 0, "sx_attn_probs_fwd: no CUDA device (this library has no CPU fallback)");
 
   AttnParams p{};
   p.B = a->B; p.M = a->M; p.U1 = a->U1; p.U2 = a->U2; p.d = a->d;
-  p.tiles_m = sx_ceil_div(a->U1, 2 * BM);
+  p.tiles_m = sx_ceil_div(a->U1, BM);
   p.tiles_n = sx_ceil_div(a->U2, BN);
   p.num_kb = sx_ceil_div(a->d, 32);
-  p.npass = p.tiles_n == 1 ? 1 : 2;
-  const long long part_floats = p.tiles_n == 1 ? 0 : (long long)a->B * a->M * p.tiles_m * p.tiles_n * 2 * 3 * (2 * BM);
-  p.part = a->scratch;
+  p.nsub = p.tiles_n == 1 ? 1 : 2 * p.tiles_n;
   const long long items = (long long)a->B * a->M * p.tiles_m;
   SX_REQUIRE(items < (1ll << 30), "sx_attn_probs_fwd: too many row blocks");
   p.items = (int)items;
   p.q_bcast = a->q_bstride == 0 && a->B > 1;
   p.alpha = a->alpha; p.clip = a->clip;
   p.alpha2 = a->alpha * LOG2E; p.clip2 = a->clip * LOG2E;
+  p.P = reinterpret_cast<float*>(a->P); p.S = reinterpret_cast<float*>(a->S);
   p.lse = a->lse; p.rowmax = a->rowmax; p.stat = a->stat;
-  p.store_s = a->S != nullptr;
-  p.dbg = (int)sx_attn_dbg;
   p.ldp = a->ldp;
   p.drop_p = a->drop_p; p.drop_seed = a->drop_seed;
   p.drop_seed_dev = reinterpret_cast<const unsigned long long*>(a->drop_seed_dev);
@@ -469,47 +313,18 @@ extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, void* stream) {
   ok.ptr = a->K; ok.major = SX_MAJOR_K; ok.ld = a->k_ld; ok.stride_z0 = a->d; ok.stride_z1 = a->k_bstride;
   if (a->M == 1) { oq.stride_z0 = 0; ok.stride_z0 = 0; }
   if (a->B == 1) { oq.stride_z1 = 0; ok.stride_z1 = 0; }
-  CUtensorMap tq, tk, tp, ts;
+  CUtensorMap tq, tk;
   int rc = make_map(&tq, oq, 4, a->U1, a->d, a->M, a->B, BM, "Q");
   if (rc) return rc;
-  rc = make_map(&tk, ok, 4, a->U2, a->d, a->M, a->B, BN / 2, "K");
+  rc = make_map(&tk, ok, 4, a->U2, a->d, a->M, a->B, BN, "K");
   if (rc) return rc;
-  const long long sz0 = (long long)a->U1 * a->ldp, sz1 = sz0 * a->M;
-  rc = make_out_map(&tp, a->P, a->U2, a->U1, a->M, a->B, a->ldp, sz0, sz1);
-  if (rc) return rc;
-  if (a->S) {
-    rc = make_out_map(&ts, a->S, a->U2, a->U1, a->M, a->B, a->ldp, sz0, sz1);
-    if (rc) return rc;
-  } else {
-    ts = tp;
-  }
 
   SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel, SMEM_BYTES));
-  // keys <= 256: one launch (phase 0).  Otherwise either ONE launch whose work items are whole row blocks (phase 3: both
-  // passes of a block on the same CTA pair, statistics stay in registers) or TWO launches over (row block, key chunk)
-  // tiles (phases 1, 2: finer load balance, partial statistics through global memory); knob "attn_mode" (1 / 2 launches)
-  const bool two = p.tiles_n > 1 && sx_attn_mode == 2 && a->scratch && a->scratch_floats >= part_floats;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = SMEM_BYTES;
-  cfg.stream = reinterpret_cast<cudaStream_t>(stream);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  for (int ph = (p.tiles_n == 1 ? 0 : (two ? 1 : 3)); ph <= (p.tiles_n == 1 ? 0 : (two ? 2 : 3)); ++ph) {
-    p.phase = ph;
-    p.nsub = ph == 3 ? 2 * p.tiles_n : 1;
-    p.nwork = ph == 3 ? p.items : p.items * p.tiles_n;
-    const int pairs = p.nwork < sms / 2 ? p.nwork : sms / 2;
-    cfg.gridDim = dim3(2 * pairs);
-    SX_CHECK_CUDA(cudaLaunchKernelEx(&cfg, sx_attn_probs_kernel, tq, tk, tp, ts, p));
-  }
+  const int grid = p.items < sms ? p.items : sms;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  sx_attn_probs_kernel<<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tq, tk, p);
   SX_CHECK_CUDA(cudaGetLastError());
-  attn_diag_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a->stat, a->clip, a->diag);
+  attn_diag_kernel<<<1, 1, 0, st>>>(a->stat, a->clip, a->diag);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

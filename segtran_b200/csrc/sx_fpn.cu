@@ -187,7 +187,7 @@ gn_bwd_apply_kernel(const float* __restrict__ dy, const float* __restrict__ x, i
 }
 
 int chunks_for(long long work, int rows) {
-  const long long want = std::max<long long>(1, (148LL * 16) / std::max(rows, 1));
+  const long long want = std::max<long long>(1, (sm_count_cached() * 16ll) / std::max(rows, 1));
   return (int)std::max<long long>(1, std::min<long long>(sx_ceil_div(work, 256 * 4), want));
 }
 

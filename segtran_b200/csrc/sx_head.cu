@@ -525,7 +525,7 @@ extern "C" int sx_head_contract_bwd_weight(const float* dL, const float* curr, i
 
 static int ew_grid(long long total) {
   long long g = (total + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > sm_count_cached() * 16ll) g = sm_count_cached() * 16ll;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -628,7 +628,7 @@ extern "C" int sx_token_scores_bwd(const float* dt, const float* W, int32_t B, i
   SX_REQUIRE(F % 4 == 0 && (reinterpret_cast<uintptr_t>(dvf) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0,
              "sx_token_scores_bwd: F must be a multiple of 4 and W/dvf 16-byte aligned");
   const long long T = (long long)B * N, total = T * (F / 4);
-  const int grid = (int)std::min<long long>(sx_ceil_div(total, 256), 148LL * 16);
+  const int grid = (int)std::min<long long>(sx_ceil_div(total, 256), sm_count_cached() * 16ll);
   token_scores_bwd_kernel<<<grid, 256, 0, ST(stream)>>>(dt, W, T, N, F, K, dvf);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;

@@ -68,7 +68,7 @@ extern "C" int sx_sw_accumulate(const float* scores, int32_t K, int32_t dx, int3
              "sx_sw_accumulate: window [%d+%d, %d+%d, %d+%d] outside the %dx%dx%d volume", x0, dx, y0, dy, z0, dz, H, W, D);
   const long long pv = (long long)dx * dy * dz;
   long long blocks = (pv + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count_cached() * 8) blocks = sm_count_cached() * 8;
   sw_accumulate_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(scores, K, dx, dy, dz, preds, cnt, H, W, D,
                                                                                          x0, y0, z0);
   SX_CHECK_CUDA(cudaGetLastError());
@@ -78,7 +78,7 @@ extern "C" int sx_sw_accumulate(const float* scores, int32_t K, int32_t dx, int3
 extern "C" int sx_sw_finalize(float* preds, const float* cnt, int32_t K, int64_t V, int32_t brats, float* hard, void* stream) {
   SX_REQUIRE(K > 0 && V > 0 && (!brats || K == 4), "sx_sw_finalize: the BraTS consistency rule needs 4 classes (got %d)", K);
   long long blocks = (V + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count_cached() * 8) blocks = sm_count_cached() * 8;
   sw_finalize_kernel<<<(int)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(preds, cnt, K, V, brats ? 1 : 0, hard);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;

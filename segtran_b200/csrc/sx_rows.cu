@@ -11,6 +11,27 @@ namespace {
 constexpr int ROW_WARPS = 8;
 constexpr float LN_EPS = 1e-12f;     // every LayerNorm on the path (segtran_shared.py:263, :371, :885, :888, :984)
 
+// Deterministic cross-CTA sums.  A kernel whose CTAs each hold partial column sums stores them in its slot (= CTA index
+// along the reduced dimension) of the caller's scratch `part`, laid out [slot][stride]; part_reduce then adds the slots
+// in slot order into the destinations.  Float atomics would add them in whatever order the CTAs finish, and the
+// last-bit differences grow through TF32 rounding and the optimiser: two runs of the same step on the same inputs would
+// not agree.  The number of slots adapts to the scratch size (part_floats / stride).
+
+struct PartDst {                                                 // slot row = concatenation of up to 4 destination arrays
+  float* p[4];
+  int n[4];
+};
+
+__global__ void part_reduce_kernel(const float* __restrict__ part, int slots, int stride, int total, PartDst d) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+    int a = 0, c = i;
+    while (c >= d.n[a]) { c -= d.n[a]; ++a; }
+    float s = 0.f;
+    for (int g = 0; g < slots; ++g) s += part[(long long)g * stride + i];
+    if (d.p[a]) d.p[a][c] += s;
+  }
+}
+
 template <typename T> __device__ __forceinline__ float ldf(const T* p);
 template <> __device__ __forceinline__ float ldf<float>(const float* p) { return *p; }
 template <> __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
@@ -108,10 +129,9 @@ __global__ void pos_lsinu_bwd_kernel(const float* __restrict__ pos, const float*
   }
 }
 
-// out[c*pd + j] += sum_r de[r,c] * pos[r,j]/posmax   (j < pd) ; outb[c] += sum_r de[r,c]
+// dW[c*pd + j] += sum_r de[r,c] * pos[r,j]/posmax   (j < pd) ; db[c] += sum_r de[r,c]  (slot blockIdx.y of `part`)
 __global__ void pos_param_grad_kernel(const float* __restrict__ de, const float* __restrict__ pos,
-                                      const float* __restrict__ posmax, int R, int pd, int C, float* __restrict__ dW,
-                                      float* __restrict__ db) {
+                                      const float* __restrict__ posmax, int R, int pd, int C, float* __restrict__ part) {
   const int c = blockIdx.x * 32 + threadIdx.x;      // blockDim = (32, 8)
   const float inv = 1.f / *posmax;
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
@@ -124,12 +144,13 @@ __global__ void pos_param_grad_kernel(const float* __restrict__ de, const float*
   __shared__ float s[8][4][33];
   for (int j = 0; j < 4; ++j) s[threadIdx.y][j][threadIdx.x] = acc[j];
   __syncthreads();
-  if (threadIdx.y == 0 && c < C) {
+  if (threadIdx.y == 0 && c < C) {                // slot blockIdx.y: [dW (C*pd) | db (C)]
+    float* slot = part + (long long)blockIdx.y * (C * pd + C);
     for (int j = 0; j < 4; ++j) {
       float t = 0.f;
       for (int y = 0; y < 8; ++y) t += s[y][j][threadIdx.x];
-      if (j == 3) atomicAdd(&db[c], t);
-      else if (j < pd) atomicAdd(&dW[c * pd + j], t);
+      if (j == 3) slot[C * pd + c] = t;
+      else if (j < pd) slot[c * pd + j] = t;
     }
   }
 }
@@ -689,10 +710,11 @@ __global__ void colsum_batched_kernel(const float* __restrict__ X, int Z1, long 
 }
 
 // float4 flavour of both column sums: lane = 4 consecutive columns (512 B per warp and row), 4 rows in flight per thread.
-// out[z0*C + c] += sum_{z1,r} X[z1*sz1 + z0*sz0 + r*ld + c];  blockDim (32, 8), grid (C/128, row blocks, Z0)
+// out[z0*C + c] += sum_{z1,r} X[z1*sz1 + z0*sz0 + r*ld + c];  blockDim (32, 8), grid (C/128, row blocks, Z0); the partial
+// sums of row block y go to slot y of `part` ([Z0 * C]) and part_reduce adds them into out
 __global__ void __launch_bounds__(256)
 colsum_v4_kernel(const float* __restrict__ X, int Z1, long long sz1, long long sz0, long long R, int C, long long ld,
-                 float* __restrict__ out) {
+                 float* __restrict__ part) {
   const int c = (blockIdx.x * 32 + threadIdx.x) * 4;
   const int z0 = blockIdx.z;
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -724,8 +746,8 @@ colsum_v4_kernel(const float* __restrict__ X, int Z1, long long sz1, long long s
       const float4 u = s4[y][threadIdx.x];
       t.x += u.x; t.y += u.y; t.z += u.z; t.w += u.w;
     }
-    float* o = out + (long long)z0 * C + c;
-    atomicAdd(o, t.x); atomicAdd(o + 1, t.y); atomicAdd(o + 2, t.z); atomicAdd(o + 3, t.w);
+    // slot blockIdx.y: [Z0 * C]
+    *reinterpret_cast<float4*>(part + (long long)blockIdx.y * gridDim.z * C + (long long)z0 * C + c) = t;
   }
 }
 
@@ -763,13 +785,16 @@ __global__ void dot_kernel(const float* __restrict__ x, const float* __restrict_
   }
 }
 
-// out[r % out_mod] += sum_c X[r, c]: one block per row
-__global__ void rowsum_kernel(const float* __restrict__ X, long long C, long long ld, int out_mod, float* out) {
-  const long long r = blockIdx.x;
-  const float* x = X + r * ld;
+// out[j] += sum_{r = j mod out_mod} sum_c X[r, c]: block (j, y) sums column chunk y of those rows in a fixed order into
+// slot y of `part` ([out_mod]); part_reduce adds the slots
+__global__ void rowsum_kernel(const float* __restrict__ X, long long R, long long C, long long ld, int out_mod,
+                              float* __restrict__ part) {
+  const long long cs = (C + gridDim.y - 1) / gridDim.y, c0 = blockIdx.y * cs, c1 = c0 + cs < C ? c0 + cs : C;
   float acc = 0.f;
-  for (long long c = (long long)blockIdx.y * blockDim.x + threadIdx.x; c < C; c += (long long)gridDim.y * blockDim.x)
-    acc += x[c];
+  for (long long r = blockIdx.x; r < R; r += out_mod) {
+    const float* x = X + r * ld;
+    for (long long c = c0 + threadIdx.x; c < c1; c += blockDim.x) acc += x[c];
+  }
   acc = sx::warp_sum(acc);
   __shared__ float s[32];
   if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = acc;
@@ -777,7 +802,7 @@ __global__ void rowsum_kernel(const float* __restrict__ X, long long C, long lon
   if (threadIdx.x < 32) {
     acc = threadIdx.x < (blockDim.x >> 5) ? s[threadIdx.x] : 0.f;
     acc = sx::warp_sum(acc);
-    if (threadIdx.x == 0) atomicAdd(&out[r % out_mod], acc);
+    if (threadIdx.x == 0) part[(long long)blockIdx.y * out_mod + blockIdx.x] = acc;
   }
 }
 
@@ -795,6 +820,17 @@ __global__ void scale_kernel(const float* __restrict__ x, long long n, const flo
     y[i] = a * x[i];
 }
 
+// dst arrays += the sum of `slots` slot rows of part (row pitch `stride` >= the summed array lengths), in slot order
+int part_reduce(const float* part, int slots, int stride, PartDst d, cudaStream_t st) {
+  const int total = d.n[0] + d.n[1] + d.n[2] + d.n[3];
+  part_reduce_kernel<<<sx_ceil_div(total, 256), 256, 0, st>>>(part, slots, stride, total, d);
+  SX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// most slots of pitch `stride` that fit a scratch of part_floats floats
+int part_slots(int64_t part_floats, long long stride) { return (int)std::min<long long>(part_floats / stride, 1 << 30); }
+
 int grid_for_rows(long long rows, int per_block, int sms) {
   long long g = (rows + per_block - 1) / per_block;
   long long cap = (long long)sms * 8;
@@ -804,14 +840,8 @@ int grid_for_rows(long long rows, int per_block, int sms) {
 }
 
 int sms_cached() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 1;
-  }
-  return n;
+  const int n = sm_count_cached();
+  return n > 0 ? n : 1;
 }
 
 template <typename K>
@@ -844,7 +874,7 @@ extern "C" int sx_pos_lsinu_fwd(const float* pos, const float* posmax, int64_t R
 
 extern "C" int sx_pos_lsinu_bwd(const float* pos, const float* posmax, int64_t R, int32_t pd, const float* W,
                                 const float* b, int32_t C, const float* dpe, float* de_scratch, float* dW, float* db,
-                                void* stream) {
+                                float* part, int64_t part_floats, void* stream) {
   SX_REQUIRE(pd >= 1 && pd <= 3, "sx_pos_lsinu_bwd: pos_dim %d not in 1..3", pd);
   const size_t smem = (size_t)ROW_WARPS * 2 * C * 4;
   SX_REQUIRE(smem <= 200 * 1024, "sx_pos_lsinu_bwd: C=%d too large", C);
@@ -853,9 +883,11 @@ extern "C" int sx_pos_lsinu_bwd(const float* pos, const float* posmax, int64_t R
       pos, posmax, (int)R, pd, W, b, C, dpe, de_scratch);
   SX_CHECK_CUDA(cudaGetLastError());
   dim3 grid(sx_ceil_div(C, 32), 16), blk(32, 8);
-  pos_param_grad_kernel<<<grid, blk, 0, ST(stream)>>>(de_scratch, pos, posmax, (int)R, pd, C, dW, db);
+  SX_REQUIRE(part && part_floats >= 16ll * (C * pd + C), "sx_pos_lsinu_bwd: needs %lld floats of scratch",
+             16ll * (C * pd + C));
+  pos_param_grad_kernel<<<grid, blk, 0, ST(stream)>>>(de_scratch, pos, posmax, (int)R, pd, C, part);
   SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return part_reduce(part, 16, C * pd + C, PartDst{{dW, db, nullptr, nullptr}, {C * pd, C, 0, 0}}, ST(stream));
 }
 
 extern "C" int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, const float* g, const float* b,
@@ -895,20 +927,25 @@ extern "C" int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, 
 extern "C" int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32_t N, int32_t C, const float* g,
                                const float* b, const float* pe, int32_t C0, int64_t pe_bstride, float posw,
                                const float* mask, float drop_p, uint64_t seed, const uint64_t* seed_dev, const float* stats, float* dx, float* dg,
-                               float* db, float* dpe, float* dt_scratch, void* stream) {
+                               float* db, float* dpe, float* dt_scratch, float* part, int64_t part_floats, void* stream) {
   if (C % 4 == 0 && C <= 2048 && C0 % 4 == 0 && pe_bstride % 4 == 0 && al16(dh) && al16(x) && al16(dx) && al16(pe) && al16(g) &&
       al16(b) && (!dpe || (dt_scratch && al16(dt_scratch) && al16(dpe)))) {
     // CTA-per-row kernel: x / dh read once, dx (and dt, when the positional-code gradient needs it) written once, dg / db
     // accumulated in registers
     const long long R = (long long)B * N;
     float* dt = dpe ? dt_scratch : nullptr;
+    auto pgrid = [&](int tt) {
+      return (int)std::min<long long>(std::min<long long>(R, (long long)sms_cached() * (768 / tt)), part_slots(part_floats, 2 * C));
+    };
+    SX_REQUIRE(part && part_floats >= 2ll * C, "sx_prologue_bwd: needs at least %lld floats of scratch", 2ll * C);
 #define SX_LAUNCH(NV_, TT_)                                                                                             \
-  prologue_bwd_cta<NV_, TT_><<<(int)std::min<long long>(R, (long long)sms_cached() * (768 / TT_)), TT_, 0, ST(stream)>>>( \
+  prologue_bwd_cta<NV_, TT_><<<pgrid(TT_), TT_, 0, ST(stream)>>>(                                                    \
       dh, x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, stats, dx, dt, \
-      dg, db)
+      part)
     if (C <= 512) SX_LAUNCH(1, 128); else if (C <= 1024) SX_LAUNCH(2, 128); else SX_LAUNCH(2, 256);
 #undef SX_LAUNCH
     SX_CHECK_CUDA(cudaGetLastError());
+    if (part_reduce(part, pgrid(C <= 1024 ? 128 : 256), 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream))) return -2;
     if (dpe) {
       pos_grad_from_dt_fast<<<grid_for_rows((long long)N * (C / 4), 256, sms_cached()), 256, 0, ST(stream)>>>(
           dt_scratch, (int)B, N, C, C0, pe_bstride, posw, dpe);
@@ -930,10 +967,13 @@ extern "C" int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32
     int gy = (int)((R + 8 * 64 - 1) / (8 * 64));
     const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128));
     if (gy > cap) gy = cap;
+    gy = std::min(gy, part_slots(part_floats, 2 * C));
+    SX_REQUIRE(part && gy >= 1, "sx: needs at least %lld floats of scratch", 2ll * C);
     if (gy < 1) gy = 1;
     dim3 grid2(sx_ceil_div(C, 128), gy), blk(32, 8);
-    ln_param_grad_cols_fast<<<grid2, blk, 0, ST(stream)>>>(dt_scratch, x, R, C, stats, 4, dg, db);
+    ln_param_grad_cols_fast<<<grid2, blk, 0, ST(stream)>>>(dt_scratch, x, R, C, stats, 4, part);
     SX_CHECK_CUDA(cudaGetLastError());
+    if (part_reduce(part, gy, 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream))) return -2;
     if (dpe) {
       pos_grad_from_dt_fast<<<grid_for_rows((long long)N * (C / 4), 256, sms_cached()), 256, 0, ST(stream)>>>(
           dt_scratch, (int)B, N, C, C0, pe_bstride, posw, dpe);
@@ -1062,7 +1102,7 @@ extern "C" int sx_layernorm_fwd(const float* x, int64_t R, int32_t C, const floa
 
 extern "C" int sx_layernorm_bwd(const float* dy, const float* x, int64_t R, int32_t C, const float* g,
                                 const float* stats, void* dx, int32_t dx_dtype, int32_t round_tf32, float* dg, float* db,
-                                void* stream) {
+                                float* part, int64_t part_floats, void* stream) {
   if (dx_dtype == SX_F32 && C % 4 == 0 && nv_for(C) && al16(dy) && al16(x) && al16(dx) && al16(g)) {
     const int grid = grid_for_rows(R, FAST_WARPS, sms_cached() * 2);
 #define SX_LAUNCH(NV_)                                                                                         \
@@ -1074,10 +1114,13 @@ extern "C" int sx_layernorm_bwd(const float* dy, const float* x, int64_t R, int3
     int gy = (int)((R + 8 * 64 - 1) / (8 * 64));
     const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128));
     if (gy > cap) gy = cap;
+    gy = std::min(gy, part_slots(part_floats, 2 * C));
+    SX_REQUIRE(part && gy >= 1, "sx: needs at least %lld floats of scratch", 2ll * C);
     if (gy < 1) gy = 1;
     dim3 grid2(sx_ceil_div(C, 128), gy), blk(32, 8);
-    ln_param_grad_cols_fast<<<grid2, blk, 0, ST(stream)>>>(dy, x, R, C, stats, 2, dg, db);
+    ln_param_grad_cols_fast<<<grid2, blk, 0, ST(stream)>>>(dy, x, R, C, stats, 2, part);
     SX_CHECK_CUDA(cudaGetLastError());
+    if (part_reduce(part, gy, 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream))) return -2;
     return 0;
   }
   const size_t smem = (size_t)(2 + 2 * ROW_WARPS) * C * 4;
@@ -1139,23 +1182,25 @@ extern "C" int sx_ln_softaggr_fwd(const float* Y, int32_t B, int32_t M, int32_t 
 extern "C" int sx_ln_softaggr_bwd(const float* dout, const float* Y, int32_t B, int32_t M, int32_t N, int32_t F,
                                   const float* g, const float* b, const float* ws, float drop_p, uint64_t seed, const uint64_t* seed_dev,
                                   const float* stats, const float* wts, void* dY, int32_t dy_dtype, int32_t round_tf32,
-                                  float* dg, float* db, float* dws, float* dbs, float* dscore_scratch, void* stream) {
+                                  float* dg, float* db, float* dws, float* dbs, float* dscore_scratch, float* part, int64_t part_floats, void* stream) {
   SX_REQUIRE(M >= 1 && M <= MAX_MODES, "sx_ln_softaggr_bwd: num_modes %d not in 1..%d", M, MAX_MODES);
   if (dy_dtype == SX_F32 && F % 4 == 0 && F <= 2048 && (M == 1 || M == 2 || M == 4) && al16(Y) && al16(dout) && al16(dY) &&
       al16(g) && al16(b) && al16(ws)) {
     // CTA-per-token kernel: Y and dout read once, dY written once, column gradients accumulated in registers
     const long long T = (long long)B * N;
-    const int grid = (int)std::min<long long>(T, (long long)sms_cached() * (F <= 1024 ? 3 : 2));
+    const int grid = (int)std::min<long long>(std::min<long long>(T, (long long)sms_cached() * (F <= 1024 ? 3 : 2)),
+                                              part_slots(part_floats, 3 * F + 4));
+    SX_REQUIRE(part && grid >= 1, "sx_ln_softaggr_bwd: needs at least %lld floats of scratch", 3ll * F + 4);
 #define SX_LAUNCH(NV_, MM_, TT_)                                                                                        \
   ln_softaggr_bwd_cta<NV_, MM_, TT_><<<grid, TT_, 0, ST(stream)>>>(dout, Y, B, N, F, g, b, ws, drop_p, seed,            \
                                                                     (const unsigned long long*)seed_dev, stats, wts,    \
-                                                                    (float*)dY, round_tf32, dg, db, dws, dbs)
+                                                                    (float*)dY, round_tf32, part)
 #define SX_MODES(NV_, TT_) do { if (M == 4) SX_LAUNCH(NV_, 4, TT_); else if (M == 2) SX_LAUNCH(NV_, 2, TT_); else SX_LAUNCH(NV_, 1, TT_); } while (0)
     if (F <= 512) SX_MODES(1, 128); else if (F <= 1024) SX_MODES(2, 128); else SX_MODES(2, 256);
 #undef SX_MODES
 #undef SX_LAUNCH
     SX_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return part_reduce(part, grid, 3 * F + 4, PartDst{{dg, db, dws, dbs}, {F, F, F, 1}}, ST(stream));
   }
   if (dy_dtype == SX_F32 && dscore_scratch && F % 4 == 0 && nv_for(F) && al16(Y) && al16(dout) && al16(dY) && al16(g) &&
       al16(b) && al16(ws)) {
@@ -1249,7 +1294,7 @@ extern "C" int sx_softaggr_bwd(const float* dout, const float* x, int32_t B, int
 extern "C" int sx_split_tf32(const float* x, int64_t n, float* hi, float* lo, void* stream) {
   if (n <= 0) return 0;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > sms_cached() * 16) blocks = sms_cached() * 16;
   split_tf32_kernel<<<(int)blocks, 256, 0, ST(stream)>>>(x, n, hi, lo);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -1265,7 +1310,7 @@ extern "C" int sx_split_tf32_cat(const float* x, int32_t Z1, int32_t Z0, int32_t
   return 0;
 }
 
-extern "C" int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, int64_t ld, float* out, void* stream) {
+extern "C" int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, int64_t ld, float* out, float* part, int64_t part_floats, void* stream) {
   int gy = (int)((R + 255) / 256);
   if (gy > 64) gy = 64;
   if (gy < 1) gy = 1;
@@ -1274,8 +1319,11 @@ extern "C" int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, i
     int gy4 = (int)((R + 127) / 128);
     const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128));
     if (gy4 > cap) gy4 = cap;
-    if (gy4 < 1) gy4 = 1;
-    colsum_v4_kernel<<<dim3(sx_ceil_div(C, 128), gy4, 1), blk, 0, ST(stream)>>>((const float*)X, 1, 0, 0, R, C, ld, out);
+    gy4 = std::min(gy4, part_slots(part_floats, C));
+    SX_REQUIRE(part && gy4 >= 1, "sx_colsum: needs at least %d floats of scratch", C);
+    colsum_v4_kernel<<<dim3(sx_ceil_div(C, 128), gy4, 1), blk, 0, ST(stream)>>>((const float*)X, 1, 0, 0, R, C, ld, part);
+    SX_CHECK_CUDA(cudaGetLastError());
+    return part_reduce(part, gy4, C, PartDst{{out, nullptr, nullptr, nullptr}, {C, 0, 0, 0}}, ST(stream));
   } else if (x_dtype == SX_F32)
     colsum_kernel<float><<<grid, blk, 0, ST(stream)>>>((const float*)X, R, C, ld, out);
   else
@@ -1310,18 +1358,20 @@ extern "C" int sx_scale(const float* x, int64_t n, const float* alpha_dev, float
   return 0;
 }
 
-extern "C" int sx_rowsum(const float* X, int64_t R, int64_t C, int64_t ld, int32_t out_mod, float* out, void* stream) {
+extern "C" int sx_rowsum(const float* X, int64_t R, int64_t C, int64_t ld, int32_t out_mod, float* out, float* part, int64_t part_floats, void* stream) {
   SX_REQUIRE(R >= 1 && R <= 2147483647ll && out_mod >= 1, "sx_rowsum: bad shape");
-  int chunks = (int)((C + 16383) / 16384);                 // long rows are split over several blocks
-  if (chunks > 64) chunks = 64;
-  if (chunks < 1) chunks = 1;
-  rowsum_kernel<<<dim3((unsigned)R, chunks), 512, 0, ST(stream)>>>(X, C, ld, out_mod, out);
+  SX_REQUIRE(part && part_floats >= out_mod, "sx_rowsum: needs at least %d floats of scratch", out_mod);
+  // column chunks: enough blocks for the machine, at least 512 columns each, as many slots as the scratch holds
+  long long chunks = sx_ceil_div((long long)sms_cached() * 8, out_mod);
+  chunks = std::min<long long>(chunks, sx_ceil_div(C, 512));
+  chunks = std::max<long long>(1, std::min<long long>({chunks, 65535ll, (long long)part_slots(part_floats, out_mod)}));
+  rowsum_kernel<<<dim3((unsigned)out_mod, (unsigned)chunks), 512, 0, ST(stream)>>>(X, R, C, ld, out_mod, part);
   SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return part_reduce(part, (int)chunks, out_mod, PartDst{{out, nullptr, nullptr, nullptr}, {out_mod, 0, 0, 0}}, ST(stream));
 }
 
 extern "C" int sx_colsum_batched(const float* X, int32_t Z1, int64_t stride_z1, int32_t Z0, int64_t stride_z0, int64_t R,
-                                 int32_t C, int64_t ld, float* out, void* stream) {
+                                 int32_t C, int64_t ld, float* out, float* part, int64_t part_floats, void* stream) {
   SX_REQUIRE(Z0 >= 1 && Z0 <= 65535 && Z1 >= 1, "sx_colsum_batched: bad batch dims");
   int gy = (int)((R + 255) / 256);
   if (gy > 32) gy = 32;
@@ -1331,8 +1381,11 @@ extern "C" int sx_colsum_batched(const float* X, int32_t Z1, int64_t stride_z1, 
     int gy4 = (int)((R + 127) / 128);
     const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128) * Z0);
     if (gy4 > cap) gy4 = cap;
-    if (gy4 < 1) gy4 = 1;
-    colsum_v4_kernel<<<dim3(sx_ceil_div(C, 128), gy4, Z0), blk, 0, ST(stream)>>>(X, Z1, stride_z1, stride_z0, R, C, ld, out);
+    gy4 = std::min(gy4, part_slots(part_floats, (long long)Z0 * C));
+    SX_REQUIRE(part && gy4 >= 1, "sx_colsum_batched: needs at least %lld floats of scratch", (long long)Z0 * C);
+    colsum_v4_kernel<<<dim3(sx_ceil_div(C, 128), gy4, Z0), blk, 0, ST(stream)>>>(X, Z1, stride_z1, stride_z0, R, C, ld, part);
+    SX_CHECK_CUDA(cudaGetLastError());
+    return part_reduce(part, gy4, Z0 * C, PartDst{{out, nullptr, nullptr, nullptr}, {Z0 * C, 0, 0, 0}}, ST(stream));
   } else
     colsum_batched_kernel<<<grid, blk, 0, ST(stream)>>>(X, Z1, stride_z1, stride_z0, R, C, ld, out);
   SX_CHECK_CUDA(cudaGetLastError());

@@ -2,9 +2,9 @@
 // segtran_shared.py:273-274, :318-325).  One 128- or 256-thread CTA owns one token: thread t holds columns 4t + 4 TT i (i < NV)
 // of ALL MM mode rows in registers, so every row of Y is read from HBM exactly once (the warp-per-token kernels re-read
 // each row two to three times and, at the 2-D widths F = 1792 / 2048, keep 64+ row registers per lane and drop to 8 warps
-// per SM: 0.9 TB/s measured at cfg 3), statistics are block reductions batched over the modes (one barrier per batch),
-// and the backward accumulates the LayerNorm / score-weight column gradients in registers across the tokens a CTA visits
-// (one atomicAdd per column per CTA at the end) instead of a second column-parallel kernel that reads Y again.
+// per SM), statistics are block reductions batched over the modes (one barrier per batch), and the backward accumulates
+// the LayerNorm / score-weight column gradients in registers across the tokens a CTA visits (stored once per CTA in its
+// slot of the caller's partial-sum scratch and summed in slot order by part_reduce) instead of a second column-parallel kernel that reads Y again.
 // Included by sx_rows.cu inside its anonymous namespace (after sx_rows_fast.cuh).
 #pragma once
 
@@ -152,8 +152,7 @@ __global__ void __launch_bounds__(TT, TT == 256 ? 2 : 3)
 ln_softaggr_bwd_cta(const float* __restrict__ dout, const float* __restrict__ Y, int B, int N, int F, const float* __restrict__ g,
                     const float* __restrict__ b, const float* __restrict__ ws, float drop_p, unsigned long long seed,
                     const unsigned long long* __restrict__ seed_dev, const float* __restrict__ stats,
-                    const float* __restrict__ wts, float* __restrict__ dY, int rnd, float* __restrict__ dg, float* __restrict__ db,
-                    float* __restrict__ dws, float* __restrict__ dbs) {
+                    const float* __restrict__ wts, float* __restrict__ dY, int rnd, float* __restrict__ part) {
   seed += seed_dev ? *seed_dev : 0ull;
   __shared__ float red[2 * (TT / 32) * 2 * MM];
   int par = 0;
@@ -268,17 +267,18 @@ ln_softaggr_bwd_cta(const float* __restrict__ dout, const float* __restrict__ Y,
       }
     }
   }
-  // column gradients: one atomic per column per CTA
+  // column gradients: this CTA's partial sums -> its slot [dg (F) | db (F) | dws (F) | dbs (1)], added by part_reduce
+  float* slot = part + (long long)blockIdx.x * (3 * F + 4);      // (slot rows stay 16-byte aligned)
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int c = 4 * tid + 4 * TT * i;
     if (c < F) {
-      atomicAdd(dg + c, ag[i].x); atomicAdd(dg + c + 1, ag[i].y); atomicAdd(dg + c + 2, ag[i].z); atomicAdd(dg + c + 3, ag[i].w);
-      atomicAdd(db + c, ab[i].x); atomicAdd(db + c + 1, ab[i].y); atomicAdd(db + c + 2, ab[i].z); atomicAdd(db + c + 3, ab[i].w);
-      atomicAdd(dws + c, aw[i].x); atomicAdd(dws + c + 1, aw[i].y); atomicAdd(dws + c + 2, aw[i].z); atomicAdd(dws + c + 3, aw[i].w);
+      *reinterpret_cast<float4*>(slot + c) = ag[i];
+      *reinterpret_cast<float4*>(slot + F + c) = ab[i];
+      *reinterpret_cast<float4*>(slot + 2 * F + c) = aw[i];
     }
   }
-  if (tid == 0 && dbs_acc != 0.f) atomicAdd(dbs, dbs_acc);
+  if (tid == 0) slot[3 * F] = dbs_acc;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -360,14 +360,14 @@ prologue_fwd_cta(const float* __restrict__ x, long long R, int N, int C, const f
 }
 
 // dx from dh; dt (the gradient at the inner LayerNorm's input, needed by the positional-code gradient) is written to
-// dt_out; dg[c] += sum_r dt * xhat1, db[c] += sum_r dt accumulated in registers, one atomicAdd per column per CTA
+// dt_out; dg[c] += sum_r dt * xhat1, db[c] += sum_r dt accumulated in registers, stored once per CTA in its scratch slot
 template <int NV, int TT>
 __global__ void __launch_bounds__(TT, 768 / TT)
 prologue_bwd_cta(const float* __restrict__ dh, const float* __restrict__ x, long long R, int N, int C, const float* __restrict__ g,
                  const float* __restrict__ b, const float* __restrict__ pe, int C0, long long pe_bstride, float posw,
                  const float* __restrict__ mask, float drop_p, unsigned long long seed,
                  const unsigned long long* __restrict__ seed_dev, const float* __restrict__ stats, float* __restrict__ dx,
-                 float* __restrict__ dt_out, float* __restrict__ dg, float* __restrict__ db) {
+                 float* __restrict__ dt_out, float* __restrict__ part) {
   seed += seed_dev ? *seed_dev : 0ull;
   __shared__ float red[2 * (TT / 32) * 2];
   int par = 0;
@@ -435,12 +435,14 @@ prologue_bwd_cta(const float* __restrict__ dh, const float* __restrict__ x, long
       }
     }
   }
+  // this CTA's partial sums -> its slot [dg (C) | db (C)], added by part_reduce
+  float* slot = part + (long long)blockIdx.x * (2 * C);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int c = 4 * tid + 4 * TT * i;
     if (c < C) {
-      atomicAdd(dg + c, ag[i].x); atomicAdd(dg + c + 1, ag[i].y); atomicAdd(dg + c + 2, ag[i].z); atomicAdd(dg + c + 3, ag[i].w);
-      atomicAdd(db + c, ab[i].x); atomicAdd(db + c + 1, ab[i].y); atomicAdd(db + c + 2, ab[i].z); atomicAdd(db + c + 3, ab[i].w);
+      *reinterpret_cast<float4*>(slot + c) = ag[i];
+      *reinterpret_cast<float4*>(slot + C + c) = ab[i];
     }
   }
 }

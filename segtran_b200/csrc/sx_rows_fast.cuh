@@ -511,10 +511,11 @@ prologue_bwd_rows_fast(const float* __restrict__ dh, const float* __restrict__ x
 }
 
 // column part of a LayerNorm-type backward:  dg[c] += sum_r dy[r,c] * (x[r,c]-mean_r)*rstd_r ; db[c] += sum_r dy[r,c]
+// (per row-block partials into slot blockIdx.y of `part`, [dg | db]; part_reduce adds them)
 // stats rows have `sstride` floats with mean/rstd at offsets 0/1.  block (32 lanes x 8 row slots), lane owns 4 columns.
 __global__ void __launch_bounds__(256)
 ln_param_grad_cols_fast(const float* __restrict__ dy, const float* __restrict__ x, long long R, int C,
-                        const float* __restrict__ stats, int sstride, float* __restrict__ dg, float* __restrict__ db) {
+                        const float* __restrict__ stats, int sstride, float* __restrict__ part) {
   const int c = (blockIdx.x * 32 + threadIdx.x) * 4;
   float4 ag = make_float4(0.f, 0.f, 0.f, 0.f), ab = ag;
   if (c < C)
@@ -551,8 +552,8 @@ ln_param_grad_cols_fast(const float* __restrict__ dy, const float* __restrict__ 
       const float4 u = s[threadIdx.y][y][threadIdx.x];
       t.x += u.x; t.y += u.y; t.z += u.z; t.w += u.w;
     }
-    float* dst = threadIdx.y == 0 ? dg : db;
-    atomicAdd(dst + c, t.x); atomicAdd(dst + c + 1, t.y); atomicAdd(dst + c + 2, t.z); atomicAdd(dst + c + 3, t.w);
+    // slot blockIdx.y: [dg (C) | db (C)], added by part_reduce
+    *reinterpret_cast<float4*>(part + (long long)blockIdx.y * (2 * C) + threadIdx.y * C + c) = t;
   }
 }
 

@@ -1,5 +1,5 @@
-// Shared pieces of the tcgen05 / TMA kernels (sx_gemm.cu, sx_attn.cu): tile constants, UMMA shared-memory descriptors,
-// tensor-map construction, per-device caches.
+// Shared pieces of the wgmma / TMA kernels (sx_gemm.cu, sx_attn.cu): tile constants, tensor-map construction,
+// per-device caches.
 #pragma once
 #include <mutex>
 
@@ -7,26 +7,11 @@
 
 namespace sxtc {
 
-constexpr int BM = 128;          // tile rows   (UMMA M)
-constexpr int BN = 256;          // tile cols   (UMMA N)
+constexpr int BM = 128;          // tile rows   (two consumer warpgroups x wgmma M = 64)
+constexpr int BN = 128;          // tile cols   (wgmma N)
 constexpr int BKB = 128;         // bytes of K per stage row (one 128B swizzle span)
-constexpr int KSTEPS = 4;        // UMMA instructions per stage (each covers 32 bytes of K)
 constexpr int A_STAGE_BYTES = BM * BKB;       // 16 KB
-constexpr int TMEM_COLS = 512;
-
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t version, uint32_t layout_type) {
-  // cute::UMMA::SmemDescriptor: start[0,14) lbo[16,30) sbo[32,46) version[46,48) layout_type[61,64)
-  //   layout_type 2 = SWIZZLE_128B (16-byte chunks), 1 = SWIZZLE_128B_BASE32B (32-byte chunks; the only layout the
-  //   tensor core accepts for MN-major 32-bit (tf32) operands, cutlass sm100_common.inl:92)
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)(version & 0x3) << 46;
-  d |= (uint64_t)(layout_type & 0x7) << 61;
-  return d;
-}
+constexpr int B_STAGE_BYTES = BN * BKB;       // 16 KB
 
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -76,9 +61,7 @@ static int make_map(CUtensorMap* tm, const sx_operand& op, int es, int rows, int
   gstr[1] = op.stride_z0 ? (cuuint64_t)op.stride_z0 * es : dflt;
   gstr[2] = op.stride_z1 ? (cuuint64_t)op.stride_z1 * es : (gstr[1] * gdim[2]);
   CUtensorMapDataType dt = (es == 4) ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  // MN-major fp32 (tf32) operands use the 32-byte-atom flavour of the 128-byte swizzle (UMMA SWIZZLE_128B_BASE32B)
-  const CUtensorMapSwizzle sw = (es == 4 && op.major == SX_MAJOR_MN) ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B
-                                                                     : CU_TENSOR_MAP_SWIZZLE_128B;
+  const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = enc(tm, dt, 4, const_cast<void*>(op.ptr), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   SX_REQUIRE(r == CUDA_SUCCESS,
@@ -87,39 +70,6 @@ static int make_map(CUtensorMap* tm, const sx_operand& op, int es, int rows, int
              (unsigned long long)gdim[3], (unsigned long long)gstr[0], (unsigned long long)gstr[1],
              (unsigned long long)gstr[2], box[0], box[1]);
   return 0;
-}
-
-// fp32 output tensor [Z1][Z0][M][N] (row pitch ldc; c_sz1 == 0 with Z1 > 1: all z1 slices address one output) as a 4-D
-// tensor map with 32-column x 16-row boxes, 128-byte swizzle
-static int make_out_map(CUtensorMap* tm, void* ptr, int N, int M, int Z0, int Z1, long long ldc, long long c_sz0,
-                        long long c_sz1) {
-  PFN_encodeTiled enc = get_encode();
-  SX_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available (no CUDA driver?)");
-  const bool z1_reduced = Z1 > 1 && c_sz1 == 0;
-  cuuint64_t gdim[4] = {(cuuint64_t)N, (cuuint64_t)M, (cuuint64_t)Z0, (cuuint64_t)(z1_reduced ? 1 : Z1)};
-  cuuint64_t gstr[3];
-  gstr[0] = (cuuint64_t)ldc * 4;
-  gstr[1] = Z0 > 1 ? (cuuint64_t)c_sz0 * 4 : gstr[0] * gdim[1];
-  gstr[2] = (Z1 > 1 && !z1_reduced) ? (cuuint64_t)c_sz1 * 4 : gstr[1] * gdim[2];
-  cuuint32_t box[4] = {32, 16, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  SX_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(C) failed: %d (N %d M %d ldc %lld)", (int)r, N, M, ldc);
-  return 0;
-}
-
-// SM count of the CURRENT device (cached per device ordinal: a process may drive several GPUs)
-static int sm_count_cached() {
-  static int n[64] = {0};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 0;
-  if (n[dev] == 0) {
-    int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0;
-    n[dev] = v;
-  }
-  return n[dev];
 }
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is a per-(kernel, device) setting: done once for each pair (the

@@ -240,7 +240,7 @@ extern "C" int sx_seg_loss_fwd(const float* logits, const float* mask, int32_t B
   const int vec4 = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(logits) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(mask) & 15) == 0);
   const long long work = vec4 ? V / 4 : V;
-  const int chunks = (int)std::max<long long>(1, std::min<long long>(sx_ceil_div(work, 256 * 4), (148LL * 8) / (B * K) + 1));
+  const int chunks = (int)std::max<long long>(1, std::min<long long>(sx_ceil_div(work, 256 * 4), (sm_count_cached() * 8ll) / (B * K) + 1));
   dim3 grid(chunks, B * K);
   seg_loss_fwd_kernel<<<grid, 256, 0, ST(stream)>>>(logits, mask, V, K, pos_weight, sums, vec4);
   SX_CHECK_CUDA(cudaGetLastError());
@@ -256,7 +256,7 @@ extern "C" int sx_seg_loss_bwd(const float* logits, const float* mask, int32_t B
   const int vec4 = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(logits) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(mask) & 15) == 0) && ((reinterpret_cast<uintptr_t>(dlogits) & 15) == 0);
   const long long work = vec4 ? V / 4 : V;
-  const int chunks = (int)std::max<long long>(1, std::min<long long>(sx_ceil_div(work, 256 * 4), (148LL * 8) / (B * K) + 1));
+  const int chunks = (int)std::max<long long>(1, std::min<long long>(sx_ceil_div(work, 256 * 4), (sm_count_cached() * 8ll) / (B * K) + 1));
   dim3 grid(chunks, B * K);
   seg_loss_bwd_kernel<<<grid, 256, 0, ST(stream)>>>(logits, mask, V, K, pos_weight, coef, ce_scale, gout, dlogits, vec4);
   SX_CHECK_CUDA(cudaGetLastError());

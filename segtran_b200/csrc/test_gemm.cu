@@ -311,8 +311,8 @@ int main(int argc, char** argv) {
   }
   if (ksweep) {
     const int Ks[] = {128, 256, 512, 1024, 2048, 4096};
-    for (int kk : Ks) perf(T, K_, K_, 128 * 74, 256 * 20, kk, 1);      // 1480 tiles = exactly 10 waves of 148
-    for (int kk : Ks) perf(H, K_, K_, 128 * 74, 256 * 20, kk, 1);
+    for (int kk : Ks) perf(T, K_, K_, 128 * 66, 128 * 20, kk, 1);      // 1320 tiles = exactly 10 waves of 132
+    for (int kk : Ks) perf(H, K_, K_, 128 * 66, 128 * 20, kk, 1);
     return 0;
   }
   if (do_perf) {

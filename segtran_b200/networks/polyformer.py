@@ -1,4 +1,4 @@
-"""Polyformer layer on the B200 kernels (SURVEY.md §8 f.3): the reference's code/networks/polyformer.py:8-106 — a squeezed
+"""Polyformer layer on the H100 kernels (SURVEY.md §8 f.3): the reference's code/networks/polyformer.py:8-106 — a squeezed
 attention block WITHOUT the expansion FFN (both CrossAttFeatTrans run multi-mode, their value modes are soft-aggregated,
 segtran_shared.py:452-457) applied to a 2x average-pooled CNN feature map and added back to it.
 

@@ -1,4 +1,4 @@
-"""Segtran2d shell on the B200 hot path — same module surface as the reference's code/networks/segtran2d.py.
+"""Segtran2d shell on the H100 hot path — same module surface as the reference's code/networks/segtran2d.py.
 
 Backbone (ResNet / EfficientNet) and the in-/out-FPN pyramids stay stock PyTorch/cuDNN (out of the hot path);
 token flatten, the Squeeze-and-Expansion stack and the pixel-wise head (collapsed form) run on segtran_b200 kernels.
@@ -178,7 +178,7 @@ class Segtran2d(SegtranInitWeights):
     def _pyramid(feats, layers, convs, norms, scheme, start):
         """conv1x1(curr) (+) bilinear(higher) -> norm, bottom-up over `layers` (reference segtran3d.py:299-313, :347-359 /
         segtran2d.py:244-257, :286-300).  On CUDA with GroupNorm and TMA-legal shapes each stage is the fused
-        ops.fpn_stage (conv + bias + add in one tcgen05 GEMM, two-pass GroupNorm); otherwise the stock modules run."""
+        ops.fpn_stage (conv + bias + add in one wgmma GEMM, two-pass GroupNorm); otherwise the stock modules run."""
         cur = feats[start]
         for layer in layers:
             conv, norm = convs[layer], norms[layer + 1]
@@ -199,7 +199,7 @@ class Segtran2d(SegtranInitWeights):
         return tuple(self.backbone(batch))
 
     def hot_path(self, feat_fpn, curr_feat, vmask, out_size, B0=None, MOD=0):
-        """The B200 segment: token flatten -> Squeeze-and-Expansion stack -> scatter -> collapsed pixel-wise head
+        """The CUDA segment: token flatten -> Squeeze-and-Expansion stack -> scatter -> collapsed pixel-wise head
         (reference segtran2d.py:264-269, :362-436 minus the FPN pyramids).
         feat_fpn [B,C0,H2,W2], curr_feat [B,Cf,H1,W1], vmask [B,N] or None, out_size = (H,W) -> logits."""
         B, C0, H2, W2 = feat_fpn.shape

@@ -1,4 +1,4 @@
-"""Segtran3d shell on the B200 hot path — same module surface as the reference's code/networks/segtran3d.py.
+"""Segtran3d shell on the H100 hot path — same module surface as the reference's code/networks/segtran3d.py.
 
 What runs where
   * CNN backbone (I3D) and the in-/out-FPN pyramids (1x1x1 conv + trilinear + GroupNorm): stock PyTorch/cuDNN
@@ -200,7 +200,7 @@ class Segtran3d(SegtranInitWeights):
     def _pyramid(feats, layers, convs, norms, scheme, start):
         """conv1x1(curr) (+) trilinear(higher) -> norm, bottom-up over `layers` (reference segtran3d.py:299-313, :347-359 /
         segtran2d.py:244-257, :286-300).  On CUDA with GroupNorm and TMA-legal shapes each stage is the fused
-        ops.fpn_stage (conv + bias + add in one tcgen05 GEMM, two-pass GroupNorm); otherwise the stock modules run."""
+        ops.fpn_stage (conv + bias + add in one wgmma GEMM, two-pass GroupNorm); otherwise the stock modules run."""
         cur = feats[start]
         for layer in layers:
             conv, norm = convs[layer], norms[layer + 1]
@@ -239,7 +239,7 @@ class Segtran3d(SegtranInitWeights):
                              self.out_fpn_layers[0])
 
     def hot_path(self, feat_fpn, curr_feat, vmask, out_size):
-        """The B200 segment of the forward: token flatten -> Squeeze-and-Expansion stack -> scatter -> collapsed
+        """The CUDA segment of the forward: token flatten -> Squeeze-and-Expansion stack -> scatter -> collapsed
         voxel-wise head (reference segtran3d.py:326-332, :442-498 minus the FPN pyramids).
         feat_fpn [B,C0,D2,H2,W2], curr_feat [B,Cf,D1,H1,W1], vmask [B,N] or None, out_size = (H,W,D) -> logits."""
         B, C0, D2, H2, W2 = feat_fpn.shape

@@ -1,9 +1,9 @@
-"""B200-native Squeeze-and-Expansion transformer stack — drop-in module surface.
+"""H100-native Squeeze-and-Expansion transformer stack — drop-in module surface.
 
 Mirrors the nn.Module contract of the reference's ``code/networks/segtran_shared.py`` (class names,
 constructor signatures, sub-module / parameter names and creation order, so that
 ``torch.manual_seed(s)`` + construction gives the reference's initial weights and reference
-checkpoints load with ``load_state_dict``), while every forward runs on the sm_100a kernels in
+checkpoints load with ``load_state_dict``), while every forward runs on the sm_90a kernels in
 ``segtran_b200/csrc`` through ``segtran_b200.ops``.  There is no PyTorch fallback inside the stack.
 
 Supported configuration = the one the reference's drivers force (train3d.py:174-178, train2d.py:245-249):
@@ -109,7 +109,7 @@ class SegtranConfig:
 
 
 def _unsupported(what):
-    raise NotImplementedError("segtran_b200: %s is an ablation path the B200 build does not implement "
+    raise NotImplementedError("segtran_b200: %s is an ablation path this build does not implement "
                               "(use the reference module for it)" % what)
 
 
@@ -391,7 +391,7 @@ class CrossAttFeatTrans(nn.Module):
         diag_call = self.training and (self.call_count + 1) % self.attn_diag_cycles == 0     # prints avg-attn: needs S
         if ops.attn_fusion_enabled() and not self.keep_attn_scores and not diag_call and q.is_cuda and \
                 self.attention_mode_dim % 4 == 0 and self.out_trans.supports_fused_attention():
-            # fused squeeze-out attention: scores / clamp / softmax / dropout inside one tcgen05 kernel
+            # fused squeeze-out attention: scores / clamp / softmax / dropout inside one wgmma kernel
             self.attention_scores = None
             if self.training:
                 self.call_count += 1

@@ -1,5 +1,5 @@
 """Tensor-level operators of the hot path: thin wrappers that allocate outputs with torch, launch the
-sm_100a kernels through the C ABI on torch's current stream, and wire them into autograd.
+sm_90a kernels through the C ABI on torch's current stream, and wire them into autograd.
 
 PyTorch is used for device memory, streams and the autograd tape only; every arithmetic step below is
 one of the library's own kernels (no ATen math on the path, no fallbacks).
@@ -52,9 +52,8 @@ def get_precision() -> str:
 # A tag mapped to "tf32x3" runs its FORWARD product as one launch over K-concatenated hi/lo operand splits (three TF32
 # partial products, fp32-grade result); "tf32" is one pass on TF32-rounded operands; backward products are always single
 # pass (gradients are held to 3e-3, not 1e-3).  The default keeps the small forward contractions exact: they feed every
-# token through the attractor bank, so their rounding error is shared by all outputs — measured at full size
-# (profiles/r2_precision_policy.txt): forward max-rel error 0.67-1.12e-3 -> 0.45-0.68e-3 on configs 1-3, while making the
-# token-row projections or the in-squeeze products 3-pass as well changes nothing.
+# token through the attractor bank, so their rounding error is shared by all outputs; making the token-row projections or
+# the in-squeeze products 3-pass as well does not change the full-size forward error.
 _POLICY = {"small": "tf32x3", "smallwide": "tf32", "proj": "tf32", "insq": "tf32", "big": "tf32"}
 
 
@@ -330,10 +329,24 @@ def _bf16_view(t4: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def _pick_split_k(M, N, K, Z, bk=32, sms=148, epi=10):
-    """Split-K factor for a GEMM whose tile count does not fill the machine: minimise
-    rounds(tiles*sk / SMs) * (k-blocks per unit + epilogue cost in k-block units)."""
-    tiles = ((M + 127) // 128) * ((N + 255) // 256) * Z
+_PART_FLOATS = 8 << 20          # 32 MB per (device, stream)
+_part_bufs = {}
+
+
+def _part_args(device):
+    """(pointer, floats) of the scratch the library's ordered partial sums use (split-K partial tiles, per-CTA column
+    sums).  One buffer per (device, stream): calls on one stream run in order, calls on different streams never share."""
+    key = (device.index if device.index is not None else torch.cuda.current_device(), torch.cuda.current_stream(device).cuda_stream)
+    t = _part_bufs.get(key)
+    if t is None:
+        t = _part_bufs[key] = torch.empty(_PART_FLOATS, device=device, dtype=torch.float32)
+    return t.data_ptr(), t.numel()
+
+
+def _pick_split_k(M, N, K, Z, bk=32, sms=132, epi=10):
+    """Split-K factor for a GEMM whose 128 x 128 tile count does not fill the machine (132 SMs on an H100 SXM):
+    minimise rounds(tiles*sk / SMs) * (k-blocks per unit + epilogue cost in k-block units)."""
+    tiles = ((M + 127) // 128) * ((N + 127) // 128) * Z
     nkb = (K + bk - 1) // bk
     if tiles >= 2 * sms or nkb < 16:
         return 1
@@ -413,6 +426,8 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
         g.act = L.SX_ACT_GELU_BWD
         g.preact = gelu_bwd.data_ptr()
     g.split_k = split_k
+    if split_k > 1:
+        g.part, g.part_floats = _part_args(a.device)
     g.accumulate = 1 if (accumulate or reduce_z1 or split_k > 1) else 0
     if preact is not None:
         g.preact = preact.data_ptr()
@@ -421,14 +436,16 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
     g.drop_p = drop_p
     g.drop_seed, g.drop_seed_dev = _seed_args(seed)
     if colsum is not None:
-        if colsum.dtype != torch.float32 or colsum.numel() != N or not colsum.is_contiguous():
-            raise L.SxError("gemm_nt: colsum must be a contiguous fp32 [N] tensor")
-        g.colsum = colsum.data_ptr()
+        if colsum.dtype != torch.float32 or colsum.numel() != N or not colsum.is_contiguous() or accumulate or reduce_z1:
+            raise L.SxError("gemm_nt: colsum must be a contiguous fp32 [N] tensor, without accumulate / reduce_z1")
     if addend is not None:
         if addend.dtype != torch.float32 or tuple(addend.shape[-2:]) != (M, N) or _as4(addend).stride() != o4.stride():
             raise L.SxError("gemm_nt: addend must be an fp32 tensor in the output's layout")
         g.addend = addend.data_ptr()
     L.call("sx_gemm", C.byref(g), _stream())
+    if colsum is not None:                   # column sums of the stored values, in a fixed order (sx_colsum)
+        o2 = o4.view(-1, N)
+        L.call("sx_colsum", o2.data_ptr(), L.SX_F32, o2.shape[0], N, o2.stride(0), colsum.data_ptr(), *_part_args(o2.device), _stream())
     if round_after and fresh:                # (caller-provided accumulators are gradient buffers: never rounded)
         L.call("sx_convert", out.data_ptr(), L.SX_F32, out.numel(), out.data_ptr(), L.SX_F32, 1, _stream())
     return out
@@ -441,7 +458,7 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] = N
             reduce_z1: bool = False, gelu_bwd: Optional[torch.Tensor] = None,
             addend: Optional[torch.Tensor] = None, colsum: Optional[torch.Tensor] = None,
             tag: str = "big") -> torch.Tensor:
-    """C[..., m, n] = epilogue(alpha * sum_k a[..., m, k] b[..., n, k]) on the tcgen05 GEMM.  One launch on TF32-rounded
+    """C[..., m, n] = epilogue(alpha * sum_k a[..., m, k] b[..., n, k]) on the wgmma GEMM.  One launch on TF32-rounded
     operands, or — in 'tf32x3' mode / for call-site classes the precision policy maps to it — three passes on the hi/lo
     operand splits (fp32-grade products)."""
     if not _three_pass(tag):
@@ -449,7 +466,7 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] = N
                           accumulate=accumulate, split_k=split_k, amax=amax, drop_p=drop_p, seed=seed,
                           round_out=round_out, reduce_z1=reduce_z1, gelu_bwd=gelu_bwd, addend=addend, colsum=colsum)
     _req_cuda(a, b)
-    # ONE launch over K-concatenated operand splits: [A_hi | A_lo | A_hi] . [B_hi | B_hi | B_lo]^T (fp32 accumulation in TMEM
+    # ONE launch over K-concatenated operand splits: [A_hi | A_lo | A_hi] . [B_hi | B_hi | B_lo]^T (fp32 accumulation in registers
     # over the three partial products), so every epilogue / accumulate / split-K option works unchanged
     return _gemm_nt_1(_split_cat(a, 0), _split_cat(b, 1), out=out, alpha=alpha, bias=bias, bias_mode=bias_mode, gelu=gelu,
                       preact=preact, accumulate=accumulate, split_k=split_k, amax=amax, drop_p=drop_p, seed=seed,
@@ -520,7 +537,7 @@ def colsum(x2d: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tenso
     """out[c] += sum_r x2d[r, c] (rows uniformly strided)."""
     if out is None:
         out = _zeros((x2d.shape[1],), x2d.device)
-    L.call("sx_colsum", x2d.data_ptr(), L.SX_F32, x2d.shape[0], x2d.shape[1], x2d.stride(0), out.data_ptr(), _stream())
+    L.call("sx_colsum", x2d.data_ptr(), L.SX_F32, x2d.shape[0], x2d.shape[1], x2d.stride(0), out.data_ptr(), *_part_args(x2d.device), _stream())
     return out
 
 
@@ -627,14 +644,14 @@ class _AttnScores(torch.autograd.Function):
                     out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, tag=ctx.tag)
         if rb_shape is not None and ctx.needs_input_grad[4]:
             drb = _zeros((U1,), q.device)     # sum over batch and keys
-            L.call("sx_rowsum", dS.data_ptr(), B * U1, U2, dS.stride(-2), U1, drb.data_ptr(), _stream())
+            L.call("sx_rowsum", dS.data_ptr(), B * U1, U2, dS.stride(-2), U1, drb.data_ptr(), *_part_args(dS.device), _stream())
             drb = drb.view(rb_shape)
         return dq, dk, None, None, drb, None
 
 
 def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_scores=False, round_out=True):
-    """P = dropout(softmax(min(Q K^T / sqrt(d), clip))) per mode in ONE tcgen05 kernel (csrc/sx_attn.cu): the scores stay
-    in TMEM and the softmax runs on the tcgen05.ld fragments (reference segtran_shared.py:566-567, :569-580, :601, :605).
+    """P = dropout(softmax(min(Q K^T / sqrt(d), clip))) per mode in ONE wgmma kernel (csrc/sx_attn.cu): the scores stay
+    in registers and the softmax runs on the accumulator fragments (reference segtran_shared.py:566-567, :569-580, :601, :605).
     q [Bq,U1,M*d] (Bq = 1 broadcasts), k [B,U2,M*d], both contiguous fp32 (TF32-rounded by their producers).
     -> (P [B,M,U1,U2] view of a row-padded buffer, S or None (raw scaled scores, same layout), lse [B,M,U1],
         rowmax [B,M,U1], stat [2])."""
@@ -661,10 +678,6 @@ def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_sc
     a.lse, a.rowmax, a.stat, a.diag = lse.data_ptr(), rowmax.data_ptr(), stat.data_ptr(), _ptr(diag)
     a.drop_p = drop_p
     a.drop_seed, a.drop_seed_dev = _seed_args(seed)
-    if U2 > 256:                              # partial row statistics of the (row block, key chunk) tiles
-        nfl = B * M * ((U1 + 255) // 256) * ((U2 + 255) // 256) * 1536
-        scratch = torch.empty(nfl, device=q.device, dtype=torch.float32)
-        a.scratch, a.scratch_floats = scratch.data_ptr(), nfl
     L.call("sx_attn_probs_fwd", C.byref(a), _stream())
     return P, S, lse, rowmax, stat
 
@@ -951,7 +964,7 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
         if ctx.needs_input_grad[7]:
             tgt = _grad_target(bo)
             dbo_buf = tgt if tgt is not None else _zeros((M * Fd,), G.device)
-            L.call("sx_colsum_batched", dY.data_ptr(), B, M * U1 * Fd, M, U1 * Fd, U1, Fd, Fd, dbo_buf.data_ptr(), _stream())
+            L.call("sx_colsum_batched", dY.data_ptr(), B, M * U1 * Fd, M, U1 * Fd, U1, Fd, Fd, dbo_buf.data_ptr(), *_part_args(dY.device), _stream())
             dbo = None if tgt is not None else dbo_buf
         if ctx.needs_input_grad[0]:
             dP = _rowpad_empty((B, M, U1, U2), P.device)
@@ -986,7 +999,7 @@ class _SqueezeOutFused(torch.autograd.Function):
     """Y[b,m] = dropout(gelu(P[b,m] V'[b,:,m] + bm)) Wo[m]^T + bo[m]  with  P = dropout(softmax(min(Q K^T/sqrt(d), clip)))
     — CrossAttFeatTrans.forward (segtran_shared.py:566-605) + ExpandedFeatTrans up to MMPrivateOutput's Linear
     (:447, :243-245, :267) as ONE autograd node:
-      forward : sx_attn_probs_fwd (tcgen05 scores -> in-TMEM softmax -> P)  ->  P.V' GEMM (bias/GELU/dropout epilogue)
+      forward : sx_attn_probs_fwd (wgmma scores -> in-register softmax -> P)  ->  P.V' GEMM (bias/GELU/dropout epilogue)
                 -> grouped output Linear;
       backward: dH GEMM (GELU'/dropout epilogue + bias-gradient column sums) -> dP GEMM -> sx_softmax_bwd on the saved raw
                 scores (P recomputed from S and the row log-sum-exp, the row term sum_a P_a dP_a taken from the SAME dP values
@@ -1045,7 +1058,7 @@ class _SqueezeOutFused(torch.autograd.Function):
         if ctx.needs_input_grad[11]:
             tgt = _grad_target(bo)
             dbo_buf = tgt if tgt is not None else _zeros((M * Fd,), G.device)
-            L.call("sx_colsum_batched", dY.data_ptr(), B, M * U1 * Fd, M, U1 * Fd, U1, Fd, Fd, dbo_buf.data_ptr(), _stream())
+            L.call("sx_colsum_batched", dY.data_ptr(), B, M * U1 * Fd, M, U1 * Fd, U1, Fd, Fd, dbo_buf.data_ptr(), *_part_args(dY.device), _stream())
             dbo = None if tgt is not None else dbo_buf
         if ctx.needs_input_grad[2]:
             dvp = torch.empty_like(vp)
@@ -1102,7 +1115,7 @@ class _LayerNorm(torch.autograd.Function):
         dgb, dg = _sink_or_zeros(ctx.leaves[0])
         dbb, db = _sink_or_zeros(ctx.leaves[1])
         L.call("sx_layernorm_bwd", dy.data_ptr(), x.data_ptr(), R, Cd, g.data_ptr(), stats.data_ptr(), dx.data_ptr(),
-               L.SX_F32, ctx.rnd_bwd, dgb.data_ptr(), dbb.data_ptr(), _stream())
+               L.SX_F32, ctx.rnd_bwd, dgb.data_ptr(), dbb.data_ptr(), *_part_args(dy.device), _stream())
         return dx, dg, db, None, None
 
 
@@ -1140,7 +1153,7 @@ class _GroupLinear(torch.autograd.Function):
         if ctx.needs_input_grad[2]:
             tgt = _grad_target(bo)
             db = tgt if tgt is not None else _zeros((M * Fd,), G.device)
-            L.call("sx_colsum_batched", dY.data_ptr(), B, M * N * Fd, M, N * Fd, N, Fd, Fd, db.data_ptr(), _stream())
+            L.call("sx_colsum_batched", dY.data_ptr(), B, M * N * Fd, M, N * Fd, N, Fd, Fd, db.data_ptr(), *_part_args(dY.device), _stream())
             if tgt is not None:
                 db = None
         return dG, dW, db
@@ -1177,7 +1190,7 @@ class _LnSoftAggr(torch.autograd.Function):
         scratch = torch.empty(B * M * N, device=Y.device, dtype=torch.float32)
         L.call("sx_ln_softaggr_bwd", dout.data_ptr(), Y.data_ptr(), B, M, N, Fd, g.data_ptr(), b.data_ptr(),
                ws.data_ptr(), drop_p, *_seed_args(seed), stats.data_ptr(), wts.data_ptr(), dY.data_ptr(), L.SX_F32, _rt(), dgb.data_ptr(),
-               dbb.data_ptr(), dwsb.data_ptr(), dbsb.data_ptr(), scratch.data_ptr(), _stream())
+               dbb.data_ptr(), dwsb.data_ptr(), dbsb.data_ptr(), scratch.data_ptr(), *_part_args(dout.device), _stream())
         return dY, dg, db, dws, dbs, None, None
 
 
@@ -1210,7 +1223,7 @@ class _SoftAggr(torch.autograd.Function):
         R = B * M * N
         dws = _sgemm(dscore, x, 1, Fd, R, (1, 1), (Fd, 1))[0].view(ctx.shapes[0])         # sum_r dscore[r] x[r,:]
         dbs = _zeros((1,), x.device)
-        L.call("sx_rowsum", dscore.data_ptr(), 1, R, R, 1, dbs.data_ptr(), _stream())
+        L.call("sx_rowsum", dscore.data_ptr(), 1, R, R, 1, dbs.data_ptr(), *_part_args(dscore.device), _stream())
         return dx, dws, dbs.view(ctx.shapes[1])
 
 
@@ -1249,7 +1262,7 @@ class _PosCode(torch.autograd.Function):
         dWb, dW = _sink_or_zeros(ctx.leaves[0], like=W)
         dbb, db = _sink_or_zeros(ctx.leaves[1], like=b)
         L.call("sx_pos_lsinu_bwd", pos2d.data_ptr(), pmax.data_ptr(), R, pd, W.data_ptr(), b.data_ptr(), C0,
-               dpe.data_ptr(), scratch.data_ptr(), dWb.data_ptr(), dbb.data_ptr(), _stream())
+               dpe.data_ptr(), scratch.data_ptr(), dWb.data_ptr(), dbb.data_ptr(), *_part_args(pos2d.device), _stream())
         return None, dW, db, None
 
 
@@ -1286,7 +1299,7 @@ class _Prologue(torch.autograd.Function):
         scratch = torch.empty_like(x)
         L.call("sx_prologue_bwd", dh.data_ptr(), x.data_ptr(), B, N, Cd, g.data_ptr(), b.data_ptr(), pe.data_ptr(), C0,
                pe_bstride, posw, _ptr(mask), drop_p, *_seed_args(seed), stats.data_ptr(), dx.data_ptr(), dgb.data_ptr(), dbb.data_ptr(),
-               _ptr(dpe), scratch.data_ptr(), _stream())
+               _ptr(dpe), scratch.data_ptr(), *_part_args(dh.device), _stream())
         return dx, dg, db, dpe, None, None, None, None
 
 
@@ -1500,7 +1513,7 @@ class _HeadContract(torch.autograd.Function):
             dWcb = _zeros((K, Cf), curr.device)
             L.call("sx_head_contract_bwd_weight", dL.data_ptr(), curr.data_ptr(), B, Cf, V, K, dWcb.data_ptr(), _stream())
         dcc = _zeros((K,), curr.device)               # d(const)[k] = sum_{b,v} dL
-        L.call("sx_rowsum", dL.data_ptr(), B * K, V, V, K, dcc.data_ptr(), _stream())
+        L.call("sx_rowsum", dL.data_ptr(), B * K, V, V, K, dcc.data_ptr(), *_part_args(dL.device), _stream())
         if Wb2 is not None:
             # Wcb = Wc Wb ; cc = Wc bb + bc
             dWc = gemm_nt(dWcb, Wb2, round_out=False).view(1, K, Fd)                  # dWcb Wb^T   [K,F]
@@ -1600,7 +1613,7 @@ class _Conv1x1Add(torch.autograd.Function):
         if has_b and ctx.needs_input_grad[2]:
             tgt = _grad_target(b)
             buf = tgt if tgt is not None else _zeros((Cout,), dy.device)
-            L.call("sx_rowsum", dy.data_ptr(), B * Cout, V, V, Cout, buf.data_ptr(), _stream())
+            L.call("sx_rowsum", dy.data_ptr(), B * Cout, V, V, Cout, buf.data_ptr(), *_part_args(dy.device), _stream())
             db = None if tgt is not None else buf
         return dx, dW, db, (dy if has_add else None)
 

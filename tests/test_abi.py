@@ -31,7 +31,7 @@ def test_gemm_args_struct_layout_matches_header():
     import ctypes as C
     from segtran_b200 import _lib
     assert C.sizeof(_lib.sx_operand) == 40
-    assert C.sizeof(_lib.sx_gemm_args) == 248
+    assert C.sizeof(_lib.sx_gemm_args) == 264 and _lib.sx_gemm_args.part.offset == 248
     assert _lib.sx_gemm_args.A.offset == 24 and _lib.sx_gemm_args.C.offset == 104
 
 

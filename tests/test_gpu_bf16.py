@@ -1,5 +1,5 @@
 """The bf16-operand tensor-core mode (ops.set_precision("bf16"), BASELINE.json config 5's precision): every operand
-majorness of the GEMM (CTA-pair and single-CTA kernels) against an fp64 product of the bf16-rounded operands, and the
+majorness of the GEMM against an fp64 product of the bf16-rounded operands, and the
 encoder fixtures forward + backward within the mode's error budget."""
 import pytest
 import torch

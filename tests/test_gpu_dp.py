@@ -1,6 +1,6 @@
 """Data-parallel correctness on real GPUs over NCCL (SURVEY §4 item v, reference train3d.py:671-676): a 2-rank step on a
 split batch must give the single-GPU gradient of the concatenated batch, and after the BertAdam update every rank must
-hold bit-identical parameters.  Needs >= 2 GPUs (skipped otherwise; run with `gpurun --gpus 2`)."""
+hold bit-identical parameters.  Needs >= 2 GPUs (skipped otherwise)."""
 import os
 import socket
 

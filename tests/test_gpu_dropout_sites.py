@@ -2,7 +2,7 @@
 (segtran_shared.py:944 feature dropout in the prologue, :605 attention dropout, :245 MMSharedMid, :273 MMPrivateOutput) keeps
 elements at rate 1-p, scales the kept ones by 1/(1-p), is deterministic in its seed, differs between seeds, shows no row /
 column structure, and the backward pass applies the SAME mask as the forward pass (the masks are never stored).
-The attention site of the fused tcgen05 kernel is covered in test_gpu_attn.py."""
+The attention site of the fused wgmma kernel is covered in test_gpu_attn.py."""
 import pytest
 import torch
 
@@ -74,7 +74,7 @@ def test_softmax_attention_dropout_mask_and_backward_uses_it():
 
 
 def test_gemm_epilogue_dropout_mask_mid_layer():
-    """MMSharedMid: dropout(gelu(x W^T + b)) in the epilogue of the tcgen05 GEMM, mask regenerated in the backward epilogue."""
+    """MMSharedMid: dropout(gelu(x W^T + b)) in the epilogue of the wgmma GEMM, mask regenerated in the backward epilogue."""
     from segtran_b200 import ops
     torch.manual_seed(2)
     x = torch.randn(2, 640, 512, device="cuda", requires_grad=True)

@@ -1,4 +1,4 @@
-"""GPU parity of the B200 SegtranFusionEncoder against the golden fixtures produced by the real reference
+"""GPU parity of the CUDA SegtranFusionEncoder against the golden fixtures produced by the real reference
 (and, transitively, the oracle).  Tolerance: 1e-3 rel on outputs (BASELINE.json north_star), written below."""
 import pytest
 import torch

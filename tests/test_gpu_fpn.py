@@ -1,4 +1,4 @@
-"""GPU parity of the fused FPN pyramid pieces (SURVEY §8 f.1): conv1x1 + bias + add as one tcgen05 GEMM and the two-pass
+"""GPU parity of the fused FPN pyramid pieces (SURVEY §8 f.1): conv1x1 + bias + add as one wgmma GEMM and the two-pass
 GroupNorm, against the stock PyTorch modules in true fp32 (forward and all gradients).  The end-to-end check is
 tests/test_gpu_shells.py, whose Segtran3d / Segtran2d fixtures (produced by the real reference) run through these stages."""
 import pytest

@@ -67,7 +67,7 @@ def test_full_size_stack_forward_and_gradients_match_oracle(cfg):
     # same criterion as the golden-fixture tests).  The absolute term matters for gradients that are differences of large
     # cancelling terms — the bias of the mode-softmax score (exactly zero in exact arithmetic) and the tied squeeze-out
     # Q/K weight are 1e-4 .. 1e-3 in magnitude next to 1e2 .. 1e3 for the others; on exactly these two the fp32-grade 3-pass
-    # mode deviates from the fp32 CPU oracle by the same 2 .. 100 % as the default mode (profiles/r2_grad_noise.txt), i.e.
+    # mode deviates from the fp32 CPU oracle by the same 2 .. 100 % as the default mode, i.e.
     # the fp32 reference value itself is rounding noise at that scale.
     got = dict(enc.named_parameters())
     gscale = max(float(v.grad.abs().max()) for v in p.values() if v.grad is not None)

@@ -72,9 +72,9 @@ def test_gemm_nt_tf32x3_recovers_fp32_products():
 
 
 def test_gemm_kernel_variants_agree():
-    """The CTA-pair kernel (tcgen05 cta_group::2, TMA-store / TMA reduce-add epilogue) and the 1-CTA kernel (register
-    stores / atomics) are two implementations of the same contract: same results on ragged, batched, MN-major, fused-epilogue
-    and split-K / batch-reduced problems."""
+    """The persistent kernel with one tile per CTA and with a grid of a few CTAs that each walk many tiles (operand
+    ring and barrier phases carried across tiles) compute the same contract: same results on ragged, batched,
+    MN-major, fused-epilogue and split-K / batch-reduced problems."""
     import segtran_b200._lib as L
     from segtran_b200 import ops
     a = tf32(torch.randn(2, 3, 300, 200, device="cuda"))
@@ -91,18 +91,15 @@ def test_gemm_kernel_variants_agree():
         return y, h, red, sk
 
     try:
-        L.call("sx_gemm_debug_set", b"cg2", 0)
         ref = run()
-        for cg2, c_tma in ((1, 1), (1, 0)):
-            L.call("sx_gemm_debug_set", b"cg2", cg2)
-            L.call("sx_gemm_debug_set", b"c_tma", c_tma)
+        for ctas in (7, 1):
+            L.call("sx_gemm_debug_set", b"max_ctas", ctas)
             got = run()
             assert torch.equal(got[0] == 0, ref[0] == 0)                  # identical dropout masks
             for g, r in zip(got, ref):
                 close(g.double(), r.double(), 2e-6)
     finally:
-        L.call("sx_gemm_debug_set", b"cg2", -1)
-        L.call("sx_gemm_debug_set", b"c_tma", -1)
+        L.call("sx_gemm_debug_set", b"max_ctas", -1)
 
 
 def test_epilogue_gelu_matches_fp64_erf():

@@ -1,9 +1,8 @@
-"""Pins oracle/segtran_oracle.py: (1) against the committed golden fixtures produced by the real
-reference (oracle/gen_golden.py), (2) against the live reference modules when /root/reference is present."""
+"""Pins oracle/segtran_oracle.py against the committed golden fixtures produced by the real reference
+(oracle/gen_golden.py)."""
 import pytest
 import torch
 
-from oracle import ref_import as R
 from oracle import segtran_oracle as O
 from tests.helpers import load_golden, oracle_encoder, rel_err
 
@@ -106,22 +105,15 @@ def test_seg2d_shell_matches_golden():
     assert rel_err(y, fx["out"]) < TOL
 
 
-@pytest.mark.skipif(not R.available(), reason="reference tree not mounted (GPU box)")
 def test_oracle_matches_live_reference_train_mode_shapes():
-    """Live check incl. a fresh (non-fixture) config; dropout=0 so train() == eval() numerically."""
-    ns = R.load()
-    dims = [32, 32, 16]
-    cfg = R.encoder_config(ns.shared, dims=dims, num_modes=2, num_attractors=5, pos_dim=2, qk_have_bias=True)
-    enc = R.build_encoder(cfg, seed=11).train()
-    torch.manual_seed(12)
-    x = torch.randn(3, 20, 32)
+    """A fresh (non-fixture) config in train mode; dropout=0 so train() == eval() numerically."""
+    fx = load_golden("live_ref")["train_mode"]
+    dims = fx["dims"]
     pos = O.voxels_pos_for_grid((4, 5), (8, 8), 3)
     mask = torch.ones(3, 20, 1, dtype=torch.bool)
-    with R.quiet():
-        y = enc(x, pos, mask, torch.Size((4, 5)))
-    p = {"voxel_fusion." + k: v for k, v in enc.state_dict().items()}
-    y2 = O.fusion_encoder(p, "voxel_fusion.", x, pos, mask, dims, 2)
-    assert rel_err(y2, y) < TOL
+    p = {"voxel_fusion." + k: v for k, v in fx["state_dict"].items()}
+    y2 = O.fusion_encoder(p, "voxel_fusion.", fx["x"], pos, mask, dims, 2)
+    assert rel_err(y2, fx["out"]) < TOL
 
 
 def test_dice_and_indices():
