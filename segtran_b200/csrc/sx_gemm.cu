@@ -3,14 +3,14 @@
 //   C[z][m][n] = epilogue(alpha * sum_k A[z][m][k] * B[z][n][k])
 //
 // Persistent, warp-specialised kernel, one CTA per SM, 128 x 128 output tiles:
-//   warpgroup 0    : TMA producer (one elected thread: cp.async.bulk.tensor 4-D boxes, 128-byte swizzle, 4-stage
-//                    mbarrier ring)
+//   warpgroup 0    : warp 0: TMA producer (one elected thread: cp.async.bulk.tensor 4-D boxes, 128-byte swizzle);
+//                    warps 1-3: transposers (tf32 MN-major operands only, see below)
 //   warpgroups 1-2 : consumers, 64 tile rows each: wgmma.mma_async with the fp32 accumulators in registers, then the
 //                    epilogue (bias / GELU / dropout / TF32 rounding) straight from the accumulator fragments to global
 // Operands may be K-major or MN-major, so forward (x W^T), data-gradient (dy W) and weight-gradient (dy^T x) products
 // all run without transposes in global memory.  bf16 operands reach wgmma in either majorness (its transpose bits);
-// tf32 wgmma reads K-major operands only, so an MN-major tf32 tile is transposed in shared memory by the consumers
-// (conflict-free 16-byte stores into the K-major swizzled layout) before its MMAs.
+// tf32 wgmma reads K-major operands only, so TMA lands an MN-major tf32 tile in a raw ring and the transposer warps
+// rewrite it into the K-major stage the consumers read.  The consumers run the same loop for every majorness.
 // Operand arithmetic: tf32 on fp32 storage (parity-grade) or bf16 storage (fast).
 //
 // Replaces in the reference: nn.Linear / torch.matmul / grouped Conv1d call sites on the hot path,
@@ -24,15 +24,27 @@
 namespace {
 using namespace sxtc;
 
-constexpr int NUM_THREADS = 384;          // warpgroup 0: TMA producer; warpgroups 1-2: MMA + epilogue
-constexpr int STAGES = 4;
+constexpr int NUM_THREADS = 384;          // warpgroup 0: TMA + transposers; warpgroups 1-2: MMA + epilogue
+constexpr int STAGES = 4;                 // K-major operand ring (what wgmma reads)
 constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;     // 32 KB
+constexpr int XPOSE_WARPS = 3;            // warps 1-3 of warpgroup 0
 
+// Shared-memory plan of one instantiation.  A tf32 MN-major operand goes through a raw ring (as TMA lands it) before
+// the transposers write its K-major copy into the stage; everything else lands in the stage directly.
 template <int ES, bool A_MN, bool B_MN>
-constexpr int smem_bytes() {
-  // MN-major tf32 operands: two K-major copies of a stage (double buffered between the consumer warpgroups)
-  return STAGES * STAGE_BYTES + ((ES == 4 && (A_MN || B_MN)) ? 2 * STAGE_BYTES : 0) + 1024 /*align*/ + 256 /*barriers*/;
-}
+struct Plan {
+  static constexpr bool XA = ES == 4 && A_MN, XB = ES == 4 && B_MN;
+  static constexpr bool XPOSE = XA || XB;
+  static constexpr int RAW_BYTES = (XA ? A_STAGE_BYTES : 0) + (XB ? B_STAGE_BYTES : 0);      // per raw slot
+  static constexpr int RAW_SLOTS = !XPOSE ? 0 : (XA && XB ? 3 : 4);
+  static constexpr int DIRECT_BYTES = STAGE_BYTES - RAW_BYTES;   // per stage, loaded by TMA straight into the stage
+  static constexpr int SMEM = STAGES * STAGE_BYTES + RAW_SLOTS * RAW_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(SMEM <= 227 * 1024, "sx_gemm: shared memory plan exceeds 227 KB");
+  // the transposers address B at A's offset + A_STAGE_BYTES in both the raw slot and the stage, and move 256 4 x 4
+  // blocks (4 boxes of 32 x 32) per operand: both hold only for 128 x 128 tf32 operand tiles
+  static_assert(!XPOSE || (A_STAGE_BYTES == 16384 && B_STAGE_BYTES == 16384 && BM == 128 && BN == 128),
+                "sx_gemm: the transposer assumes 128-row, 16 KB tf32 operand tiles");
+};
 
 struct GemmParams {
   int M, N, K, Z0, Z1;
@@ -61,28 +73,41 @@ struct GemmParams {
   int stream_out;        // output larger than half the L2: store with evict-first (st.global.cs), keep operands (evict-last)
 };
 
-// MN-major tf32 rows [r0, r0 + nrows) of a tile as TMA left them (boxes of 32 rows x 32 k, SWIZZLE_128B) -> the K-major
-// SWIZZLE_128B layout wgmma reads (row r: 128 bytes of k, 16-byte chunk c at (c ^ (r & 7))).  Consecutive threads take
-// consecutive rows: the reads of a warp cover one 128-byte span, the 16-byte stores of each quarter-warp 8 distinct chunks.
-__device__ __forceinline__ void xpose_tf32(const uint8_t* src, uint8_t* dst, int r0, int nrows, int tid, int nthr) {
-  for (int i = tid; i < nrows * 8; i += nthr) {
-    const int r = r0 + i % nrows, kc = i / nrows;
-    const uint8_t* s = src + (r >> 5) * 4096 + (r & 3) * 4;
-    float v[4];
+// MN-major tf32 operand tile as TMA left it (4 boxes of 32 k rows x 128 B of MN, SWIZZLE_128B: 16-byte chunk c of k row
+// k at (c ^ (k & 7))) -> the K-major SWIZZLE_128B tile wgmma reads (MN row r: 128 B of k, chunk kc at (kc ^ (r & 7))).
+// Block b moves MN 4c..4c+3 x k 4kc..4kc+3 of box b >> 6 with four 16-byte loads (one per k row) and four 16-byte
+// stores (one per MN row).  c = b & 7 and kc = c ^ ((b >> 3) & 7): within each quarter-warp (fixed b >> 3) both the
+// loaded chunks c ^ (k & 7) and the stored chunks kc ^ (r & 7) are 8 distinct 16-byte bank groups.
+__device__ __forceinline__ void xpose_load(uint32_t src, int b, float4 (&v)[4]) {
+  const int c = b & 7, kc = c ^ ((b >> 3) & 7);
+  const uint32_t s = src + (b >> 6) * 4096;
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int k = 4 * kc + e;
-      v[e] = *reinterpret_cast<const float*>(s + k * 128 + ((((r & 31) >> 2) ^ (k & 7)) << 4));
-    }
-    *reinterpret_cast<float4*>(dst + r * 128 + ((kc ^ (r & 7)) << 4)) = make_float4(v[0], v[1], v[2], v[3]);
+  for (int e = 0; e < 4; ++e) {
+    const int k = 4 * kc + e;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                 : "=f"(v[e].x), "=f"(v[e].y), "=f"(v[e].z), "=f"(v[e].w)
+                 : "r"(s + k * 128 + ((c ^ (k & 7)) << 4)) : "memory");
   }
+}
+__device__ __forceinline__ void xpose_store(uint32_t dst, int b, const float4 (&v)[4]) {
+  const int c = b & 7, kc = c ^ ((b >> 3) & 7);
+  const int r0 = (b >> 6) * 32 + 4 * c;
+  auto st = [&](int i, float x, float y, float z, float w) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};"
+                 ::"r"(dst + (r0 + i) * 128 + ((kc ^ ((r0 + i) & 7)) << 4)), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
+  };
+  st(0, v[0].x, v[1].x, v[2].x, v[3].x);
+  st(1, v[0].y, v[1].y, v[2].y, v[3].y);
+  st(2, v[0].z, v[1].z, v[2].z, v[3].z);
+  st(3, v[0].w, v[1].w, v[2].w, v[3].w);
 }
 
 template <int ES, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  using PL = Plan<ES, A_MN, B_MN>;
   constexpr bool kTF32 = (ES == 4);
-  constexpr bool XA = kTF32 && A_MN, XB = kTF32 && B_MN;   // tiles transposed in shared memory before the MMAs
+  constexpr bool XA = PL::XA, XB = PL::XB;
   constexpr int BK = BKB / ES;                 // elements of K per stage: 64 (bf16) / 32 (tf32)
   constexpr int MN_BOX = BKB / ES;             // contiguous MN elements per MN-major box: 64 / 32
   constexpr int MN_BOX_BYTES = BK * BKB;       // bytes of one MN-major box (BK rows of 128 B)
@@ -90,10 +115,12 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* xbuf = smem + STAGES * STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xbuf + ((XA || XB) ? 2 * STAGE_BYTES : 0));
-  uint64_t* full_bar = bars;                   // [STAGES]  TMA -> consumers
-  uint64_t* empty_bar = bars + STAGES;         // [STAGES]  consumers -> TMA (one arrival per consumer warpgroup)
+  uint8_t* raw = smem + STAGES * STAGE_BYTES;  // [RAW_SLOTS][A (XA) | B (XB)] MN-major tf32 tiles as TMA lands them
+  uint64_t* bars = reinterpret_cast<uint64_t*>(raw + PL::RAW_SLOTS * PL::RAW_BYTES);
+  uint64_t* full_bar = bars;                   // [STAGES]  TMA bytes + transposer arrivals -> consumers
+  uint64_t* empty_bar = bars + STAGES;         // [STAGES]  consumers -> TMA / transposers (one arrival per warpgroup)
+  uint64_t* raw_full = bars + 2 * STAGES;      // [RAW_SLOTS]  TMA -> transposers
+  uint64_t* raw_empty = raw_full + PL::RAW_SLOTS;   // [RAW_SLOTS]  transposers -> TMA
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -103,8 +130,12 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     sx::tma_prefetch_desc(&tmA);
     sx::tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
-      sx::mbar_init(&full_bar[s], 1);
+      sx::mbar_init(&full_bar[s], (PL::DIRECT_BYTES ? 1 : 0) + (PL::XPOSE ? XPOSE_WARPS : 0));
       sx::mbar_init(&empty_bar[s], 2);
+    }
+    for (int s = 0; s < PL::RAW_SLOTS; ++s) {
+      sx::mbar_init(&raw_full[s], 1);
+      sx::mbar_init(&raw_empty[s], XPOSE_WARPS);
     }
     sx::fence_barrier_init();
   }
@@ -117,46 +148,103 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     z0 = t % p.Z0;
     z1 = t / p.Z0;
   };
+  // k-blocks of split ks (the last split may be shorter)
+  auto split_kbs = [&](int ks) { return min(p.num_kb, (ks + 1) * p.kb_per_split) - ks * p.kb_per_split; };
 
   if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");   // the producer hands its registers over
-    // ===================== TMA producer =====================
-    if (warp == 0 && sx::elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      // operand tiles are re-read by every CTA of the same tile row / column: keep them in L2 while a large
-      // output streams through
-      const uint64_t pol = p.stream_out ? sx::kEvictLast : sx::kEvictNormal;
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");   // the producers hand their registers over
+    if (warp == 0) {
+      // ===================== TMA producer =====================
+      if (sx::elect_one()) {
+        int stage = 0, rs = 0;
+        uint32_t phase = 0, rphase = 0;
+        // operand tiles are re-read by every CTA of the same tile row / column: keep them in L2 while a large
+        // output streams through
+        const uint64_t pol = p.stream_out ? sx::kEvictLast : sx::kEvictNormal;
+        for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+          int z0, z1, mb, nb, ks;
+          decode(t, z0, z1, mb, nb, ks);
+          const int kb0 = ks * p.kb_per_split;
+          const int az0 = p.a_uses_z0 ? z0 : 0, bz0 = p.b_uses_z0 ? z0 : 0;
+          const int m0 = mb * BM, n0 = nb * BN;
+          const int nkb = split_kbs(ks);
+          for (int q = 0; q < p.z1_loop * nkb; ++q) {
+            const int kb = kb0 + q % nkb, zc = p.z1_loop > 1 ? q / nkb : z1;
+            const int az1 = p.a_uses_z1 ? zc : 0, bz1 = p.b_uses_z1 ? zc : 0;
+            const int k0 = kb * BK;
+            if constexpr (PL::XPOSE) {
+              sx::mbar_wait(&raw_empty[rs], rphase ^ 1);
+              sx::mbar_expect_tx(&raw_full[rs], PL::RAW_BYTES);
+              uint8_t* ra = raw + rs * PL::RAW_BYTES;
+              uint8_t* rb = ra + (XA ? A_STAGE_BYTES : 0);
+              if constexpr (XA) {
+#pragma unroll
+                for (int j = 0; j < BM / MN_BOX; ++j)
+                  sx::tma_load_4d(ra + j * MN_BOX_BYTES, &tmA, &raw_full[rs], m0 + j * MN_BOX, k0, az0, az1, pol);
+              }
+              if constexpr (XB) {
+#pragma unroll
+                for (int j = 0; j < BN / MN_BOX; ++j)
+                  sx::tma_load_4d(rb + j * MN_BOX_BYTES, &tmB, &raw_full[rs], n0 + j * MN_BOX, k0, bz0, bz1, pol);
+              }
+              if (++rs == PL::RAW_SLOTS) { rs = 0; rphase ^= 1; }
+            }
+            if constexpr (PL::DIRECT_BYTES > 0) {
+              sx::mbar_wait(&empty_bar[stage], phase ^ 1);
+              sx::mbar_expect_tx(&full_bar[stage], PL::DIRECT_BYTES);
+              uint8_t* sa = smem + stage * STAGE_BYTES;
+              uint8_t* sb = sa + A_STAGE_BYTES;
+              if constexpr (!XA) {
+                if constexpr (!A_MN) {
+                  sx::tma_load_4d(sa, &tmA, &full_bar[stage], k0, m0, az0, az1, pol);
+                } else {
+#pragma unroll
+                  for (int j = 0; j < BM / MN_BOX; ++j)
+                    sx::tma_load_4d(sa + j * MN_BOX_BYTES, &tmA, &full_bar[stage], m0 + j * MN_BOX, k0, az0, az1, pol);
+                }
+              }
+              if constexpr (!XB) {
+                if constexpr (!B_MN) {
+                  sx::tma_load_4d(sb, &tmB, &full_bar[stage], k0, n0, bz0, bz1, pol);
+                } else {
+#pragma unroll
+                  for (int j = 0; j < BN / MN_BOX; ++j)
+                    sx::tma_load_4d(sb + j * MN_BOX_BYTES, &tmB, &full_bar[stage], n0 + j * MN_BOX, k0, bz0, bz1, pol);
+                }
+              }
+            }
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    } else if constexpr (PL::XPOSE) {
+      // ===================== transposers: raw MN-major slot -> K-major stage =====================
+      constexpr int NT = XPOSE_WARPS * 32;
+      constexpr int NBLK = (XA && XB ? 2 : 1) * 256;     // 4 x 4 blocks per stage (256 per operand)
+      const int xt = threadIdx.x - 32;
+      int stage = 0, rs = 0;
+      uint32_t phase = 0, rphase = 0;
       for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
         int z0, z1, mb, nb, ks;
         decode(t, z0, z1, mb, nb, ks);
-        const int kb0 = ks * p.kb_per_split;
-        const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
-        const int az0 = p.a_uses_z0 ? z0 : 0, bz0 = p.b_uses_z0 ? z0 : 0;
-        const int m0 = mb * BM, n0 = nb * BN;
-        const int nkb = kb1 - kb0;
-        for (int q = 0; q < p.z1_loop * nkb; ++q) {
-          const int kb = kb0 + q % nkb, zc = p.z1_loop > 1 ? q / nkb : z1;
-          const int az1 = p.a_uses_z1 ? zc : 0, bz1 = p.b_uses_z1 ? zc : 0;
+        const int nq = p.z1_loop * split_kbs(ks);
+        for (int q = 0; q < nq; ++q) {
+          sx::mbar_wait(&raw_full[rs], rphase);
           sx::mbar_wait(&empty_bar[stage], phase ^ 1);
-          sx::mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
-          uint8_t* sa = smem + stage * STAGE_BYTES;
-          uint8_t* sb = sa + A_STAGE_BYTES;
-          const int k0 = kb * BK;
-          if constexpr (!A_MN) {
-            sx::tma_load_4d(sa, &tmA, &full_bar[stage], k0, m0, az0, az1, pol);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / MN_BOX; ++j)
-              sx::tma_load_4d(sa + j * MN_BOX_BYTES, &tmA, &full_bar[stage], m0 + j * MN_BOX, k0, az0, az1, pol);
+          const uint32_t src = sx::smem_u32(raw + rs * PL::RAW_BYTES);
+          const uint32_t dst = sx::smem_u32(smem + stage * STAGE_BYTES + (XA ? 0 : A_STAGE_BYTES));
+          for (int b = xt; b < NBLK; b += NT) {
+            float4 v[4];
+            xpose_load(src + (b >> 8) * A_STAGE_BYTES, b & 255, v);
+            xpose_store(dst + (b >> 8) * A_STAGE_BYTES, b & 255, v);
           }
-          if constexpr (!B_MN) {
-            sx::tma_load_4d(sb, &tmB, &full_bar[stage], k0, n0, bz0, bz1, pol);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / MN_BOX; ++j)
-              sx::tma_load_4d(sb + j * MN_BOX_BYTES, &tmB, &full_bar[stage], n0 + j * MN_BOX, k0, bz0, bz1, pol);
+          sx::fence_proxy_async_smem();        // this thread's stores -> visible to wgmma (async proxy)
+          __syncwarp();
+          if (lane == 0) {
+            sx::mbar_arrive(&full_bar[stage]);
+            sx::mbar_arrive(&raw_empty[rs]);
           }
+          if (++rs == PL::RAW_SLOTS) { rs = 0; rphase ^= 1; }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -164,7 +252,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     return;
   }
 
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 224;" ::: "memory");
   // ===================== consumers: MMA + epilogue =====================
   const int cw = wg - 1;                        // tile rows 64 cw .. 64 cw + 63
   const int wtid = threadIdx.x & 127;           // thread within the warpgroup
@@ -174,7 +262,6 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   float tmax = -3.0e38f;
   int stage = 0;
   uint32_t phase = 0;
-  int xi = 0;
 
   // descriptors of this warpgroup's A rows and of the B tile for k-step kk (operand bases are 1 KB aligned)
   auto desc_a = [&](const uint8_t* base, int kk, bool mn) -> uint64_t {
@@ -253,28 +340,14 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
     int z0, z1, mb, nb, ks;
     decode(t, z0, z1, mb, nb, ks);
-    const int kb0 = ks * p.kb_per_split;
-    const int kb1 = min(p.num_kb, kb0 + p.kb_per_split);
+    const int nq = p.z1_loop * split_kbs(ks);
 
     // ---------------- main loop ----------------
-    int prev = -1;                              // stage whose MMAs may still be in flight (no-transpose path)
-    for (int q = 0; q < p.z1_loop * (kb1 - kb0); ++q) {
+    int prev = -1;                              // stage whose MMAs may still be in flight
+    for (int q = 0; q < nq; ++q) {
       sx::mbar_wait(&full_bar[stage], phase);
       const uint8_t* sa = smem + stage * STAGE_BYTES;
       const uint8_t* sb = sa + A_STAGE_BYTES;
-      if constexpr (XA || XB) {
-        uint8_t* xa = xbuf + xi * STAGE_BYTES;
-        uint8_t* xb = xa + A_STAGE_BYTES;
-        // a K-major copy of the MN-major tile(s); the buffer xi was last read by MMAs that both warpgroups completed
-        // before the previous named barrier
-        if constexpr (XA) xpose_tf32(sa, xa, cw * 64, 64, wtid, 128);
-        if constexpr (XB) xpose_tf32(sb, xb, cw * 64, 64, wtid, 128);
-        sx::fence_proxy_async_smem();
-        if constexpr (XB) asm volatile("bar.sync 1, 256;" ::: "memory");
-        else asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
-        if constexpr (XA) sa = xa;
-        if constexpr (XB) sb = xb;
-      }
       sx::acc_fence(acc);
       sx::wgmma_fence();
 #pragma unroll
@@ -286,28 +359,20 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       sx::wgmma_commit();
       sx::acc_fence(acc);
-      if constexpr (XA || XB) {
-        sx::wgmma_wait<0>();
-        if (wtid == 0) sx::mbar_arrive(&empty_bar[stage]);
-        xi ^= 1;
-      } else {
-        sx::wgmma_wait<1>();                    // the previous stage's MMAs are done: release it
-        if (prev >= 0 && wtid == 0) sx::mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-      }
+      sx::wgmma_wait<1>();                      // the previous stage's MMAs are done: release it
+      if (prev >= 0 && wtid == 0) sx::mbar_arrive(&empty_bar[prev]);
+      prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-    if constexpr (!(XA || XB)) {
-      sx::wgmma_wait<0>();
-      sx::acc_fence(acc);
-      if (prev >= 0 && wtid == 0) sx::mbar_arrive(&empty_bar[prev]);
-    }
+    sx::wgmma_wait<0>();
+    sx::acc_fence(acc);
+    if (prev >= 0 && wtid == 0) sx::mbar_arrive(&empty_bar[prev]);
 
     // ---------------- epilogue: accumulator fragments -> bias / GELU / dropout / rounding -> global ----------------
-    const int row0 = mb * BM + cw * 64 + wq * 16;
     const long long zoff = (long long)z1 * p.c_sz1 + (long long)z0 * p.c_sz0;
     const float* bias = p.bias ? p.bias + (long long)z1 * p.bias_sz1 + (long long)z0 * p.bias_sz0 : nullptr;
     const bool add_bias = (bias != nullptr) && (ks == 0);
+    const int row0 = mb * BM + cw * 64 + wq * 16;
     float bias_m[2] = {0.f, 0.f};                         // [h]
     if (add_bias && p.bias_mode == SX_BIAS_M) {
 #pragma unroll
@@ -475,7 +540,7 @@ long long g_max_ctas = -1;         // cap on the persistent grid (tests drive th
 template <int ES, bool A_MN, bool B_MN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int grid, cudaStream_t st) {
   auto kern = sx_gemm_kernel<ES, A_MN, B_MN>;
-  constexpr int bytes = smem_bytes<ES, A_MN, B_MN>();
+  constexpr int bytes = Plan<ES, A_MN, B_MN>::SMEM;
   SX_CHECK_CUDA(set_max_smem_once(kern, bytes));         // per device (a process may drive several GPUs)
   kern<<<grid, NUM_THREADS, bytes, st>>>(ta, tb, p);
   SX_CHECK_CUDA(cudaGetLastError());

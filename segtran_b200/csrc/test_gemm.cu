@@ -165,14 +165,29 @@ static int run_case(const Case& c, bool verbose) {
   return ok ? 0 : 1;
 }
 
+template <typename T>
+__global__ void fill_rand_kernel(T* p, size_t n, unsigned seed, float scale) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    unsigned h = (unsigned)i * 2654435761u + seed;
+    h ^= h >> 15; h *= 0x2c1b3c6du; h ^= h >> 12; h *= 0x297a2d39u; h ^= h >> 15;
+    p[i] = (T)(((int)(h >> 8) - (1 << 23)) * (scale / (1 << 23)));
+  }
+}
+
+// random operands, not zeros: on a power-capped card zero operands draw less power and give optimistic clocks
 static void perf(int op, int amaj, int bmaj, int M, int N, int K, int Z) {
   const int es = op == SX_OP_TF32 ? 4 : 2;
   void *dA, *dB, *dC;
   cudaMalloc(&dA, (size_t)M * K * Z * es);
   cudaMalloc(&dB, (size_t)N * K * Z * es);
   cudaMalloc(&dC, (size_t)M * N * Z * 4);
-  cudaMemset(dA, 0, (size_t)M * K * Z * es);
-  cudaMemset(dB, 0, (size_t)N * K * Z * es);
+  if (es == 4) {
+    fill_rand_kernel<<<1024, 256>>>((float*)dA, (size_t)M * K * Z, 1u, 1.f);
+    fill_rand_kernel<<<1024, 256>>>((float*)dB, (size_t)N * K * Z, 2u, 1.f);
+  } else {
+    fill_rand_kernel<<<1024, 256>>>((__nv_bfloat16*)dA, (size_t)M * K * Z, 1u, 1.f);
+    fill_rand_kernel<<<1024, 256>>>((__nv_bfloat16*)dB, (size_t)N * K * Z, 2u, 1.f);
+  }
   sx_gemm_args g;
   memset(&g, 0, sizeof(g));
   g.op_dtype = op; g.M = M; g.N = N; g.K = K; g.Z0 = Z; g.Z1 = 1;
@@ -195,14 +210,6 @@ static void perf(int op, int amaj, int bmaj, int M, int N, int K, int Z) {
   printf("PERF %s A%s B%s M=%d N=%d K=%d Z=%d : %.3f ms  %.1f TFLOP/s  (%s)\n", op == SX_OP_TF32 ? "tf32" : "bf16",
          amaj ? "mn" : "k", bmaj ? "mn" : "k", M, N, K, Z, ms, tf, cudaGetErrorString(cudaGetLastError()));
   cudaFree(dA); cudaFree(dB); cudaFree(dC);
-}
-
-__global__ void fill_rand_kernel(float* p, size_t n, unsigned seed, float scale) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    unsigned h = (unsigned)i * 2654435761u + seed;
-    h ^= h >> 15; h *= 0x2c1b3c6du; h ^= h >> 12; h *= 0x297a2d39u; h ^= h >> 15;
-    p[i] = ((int)(h >> 8) - (1 << 23)) * (scale / (1 << 23));
-  }
 }
 
 // epilogue cost decomposition on the fused P.V' shape of the cfg-4 step: 16 x (2744 x 1024 x 1024), A K-major, B MN-major
@@ -324,6 +331,15 @@ int main(int argc, char** argv) {
     perf(T, K_, K_, 2744, 1024, 1024, 16);
     perf(H, K_, K_, 2744, 1024, 1024, 16);
     perf(T, K_, K_, 2744, 1024, 256, 16);
+    // the cfg-4 training step's dominant products in their real operand majorness (M N K Z as sx_gemm sees them)
+    perf(T, K_, MN, 2744, 1024, 1024, 16);     // P.V' (forward) and the data gradients dy.W
+    perf(T, MN, MN, 2744, 1024, 1024, 16);
+    perf(T, MN, MN, 1024, 1024, 2744, 16);     // dV' = P^T.dH
+    perf(T, MN, MN, 1024, 1024, 10976, 1);     // dWo and the other weight gradients dy^T.x
+    perf(T, MN, MN, 4096, 1024, 4096, 1);
+    perf(T, K_, MN, 4096, 1024, 4096, 1);
+    perf(T, K_, MN, 2744, 256, 1024, 16);      // score gradients
+    perf(T, MN, MN, 1024, 256, 2744, 16);
   }
   return fails ? 1 : 0;
 }
