@@ -102,6 +102,21 @@ typedef struct {
 int sx_gemm(const sx_gemm_args* args, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Sliding-window positional biases (SlidingPosBiases2D/3D, segtran_shared.py:1002-1175), never expanded to [N,N]:
+ * the tokens are the cells of a row-major grid grid[0..pd); for a query cell q and a key cell k
+ *     bias(q,k) = w * table[(k_0-q_0+R), ..., (k_{pd-1}-q_{pd-1}+R)]   when |k_i - q_i| <= R in every dimension,
+ *     bias(q,k) = 0                                                       otherwise;
+ * table is [2R+1]^pd fp32 (row-major).  Every entry point that takes an sx_posbias reads it through the one device
+ * helper of csrc/sx_posbias.cuh.  table == NULL means no bias.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {
+  const float* table;
+  int32_t pd, R;                 /* pd in {2, 3}, R >= 1 */
+  int32_t grid[3];
+  float w;                       /* pos_code_weight (--posw) */
+} sx_posbias;
+
+/* ---------------------------------------------------------------------------------------------
  * Fused attention probabilities of the squeeze-out stage (csrc/sx_attn.cu):
  *     P[b][m] = dropout( softmax_keys( min(alpha * Q[b,:,m] K[b,:,m]^T, clip) ) )
  * One persistent wgmma kernel replaces segtran_shared.py:566-567 (Q.K^T / sqrt(d)), :569-580 (max statistics and
@@ -116,6 +131,10 @@ int sx_gemm(const sx_gemm_args* args, void* stream);
  * maximum is below -(clip - 104), [2] (written at the end) the maximum as a plain float — the `amax` of sx_softmax_bwd.  diag (optional, device float[3]): [0] running
  * max, [1] += 1 when the clamp fired (max > clip), [2] += stat[1] in that case (rows where the reference's LOWER
  * clamp could have mattered — the upper clamp is applied exactly; see sx_attn.cu).
+ * posbias (table != NULL; self-attention, U1 == U2 == the grid's cell count): the score becomes
+ * min(alpha * Q K^T, clip) + bias(q,k) inside the softmax (segtran_shared.py:589-592).  S, rowmax, stat[0] and the clamp
+ * decision stay on the raw scores; lse is the log-sum-exp of the biased row; stat[1] counts rows whose raw maximum is
+ * below -(clip - 104) + (bmax - bmin), with bmin / bmax the range of {w * table} and 0.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {
   int32_t B, M, U1, U2, d;
@@ -136,6 +155,7 @@ typedef struct {
   uint32_t _pad;
   uint64_t drop_seed;
   const uint64_t* drop_seed_dev;
+  sx_posbias posbias;            /* table == NULL: no positional bias */
 } sx_attn_probs_args;
 int sx_attn_probs_fwd(const sx_attn_probs_args* args, void* stream);
 
@@ -165,7 +185,9 @@ int sx_pos_lsinu_bwd(const float* pos, const float* posmax, int64_t R, int32_t p
 
 /* Fused prologue of SegtranFusionEncoder.forward (segtran_shared.py:916, :930-934, :944-946):
  *   h = mask * dropout( LN( LN_{g,b}(x) + posw * pe[..., :C] ) ),  x [B,N,C] fp32, pe rows of length C0,
- *   pe_bstride = 0 when the code is shared by the batch; mask [B*N] fp32 or NULL; stats [B*N,4]. */
+ *   pe_bstride = 0 when the code is shared by the batch; mask [B*N] fp32 or NULL; stats [B*N,4].
+ * pe == NULL (pos_code_type 'bias' / 'none', :940): h = mask * dropout( LN_{g,b}(x) ), no second LayerNorm; C0,
+ *   pe_bstride and posw are ignored, stats[r] = {mean, rstd, 0, 1} of x's row, and the backward takes dpe == NULL. */
 int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, const float* g, const float* b, const float* pe,
                     int32_t C0, int64_t pe_bstride, float posw, const float* mask, float drop_p, uint64_t seed, const uint64_t* seed_dev, void* h,
                     int32_t h_dtype, int32_t round_tf32, float* stats, void* stream);
@@ -186,6 +208,20 @@ int sx_softmax_fwd(const float* S, int64_t R, int32_t L, int64_t lds, const floa
 int sx_softmax_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, const float* lse, int64_t R, int32_t L,
                    const float* amax, float clip, float drop_p, uint64_t seed, const uint64_t* seed_dev, int64_t ldp_fwd, void* dS,
                    int32_t ds_dtype, int64_t ldo, int32_t round_tf32, void* stream);
+/* The same with a sliding-window positional bias (segtran_shared.py:578-605): row r is query token r % L of a
+ * self-attention (L == the grid's cell count, posbias->table != NULL):
+ *   S' = clamp_if(S) + bias(q, .);  P = dropout(softmax(S')),  lse = log-sum-exp of S'.
+ * Backward: P is recomputed from the raw S, the bias and lse; dS' = P * (g - sum P g) (g = the dropout-masked dP);
+ * dS = dS' with the clamp mask, and dtable[o] += w * sum over rows of dS'[row, key(q, o)] — the gradient BEFORE the
+ * clamp mask, so clamped elements still feed the table.  dtable [(2R+1)^pd] is accumulated in a fixed order through
+ * `part` (no float atomics). */
+int sx_softmax_posbias_fwd(const float* S, int64_t R, int32_t L, int64_t lds, const float* amax, float clip, float drop_p,
+                           uint64_t seed, const uint64_t* seed_dev, void* P, int32_t p_dtype, int64_t ldp, int32_t round_tf32,
+                           float* lse, float* diag, const sx_posbias* posbias, void* stream);
+int sx_softmax_posbias_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, const float* lse, int64_t R, int32_t L,
+                           const float* amax, float clip, float drop_p, uint64_t seed, const uint64_t* seed_dev, int64_t ldp_fwd,
+                           void* dS, int32_t ds_dtype, int64_t ldo, int32_t round_tf32, const sx_posbias* posbias,
+                           float* dtable, float* part, int64_t part_floats, void* stream);
 
 /* LayerNorm with affine over rows, eps 1e-12 (first_norm_layer, segtran_shared.py:456).  stats [R,2]. */
 int sx_layernorm_fwd(const float* x, int64_t R, int32_t C, const float* g, const float* b, void* y, int32_t y_dtype,

@@ -39,13 +39,17 @@ class sx_gemm_args(C.Structure):
                 ("part", C.c_void_p), ("part_floats", C.c_int64)]
 
 
+class sx_posbias(C.Structure):
+    _fields_ = [("table", C.c_void_p), ("pd", C.c_int32), ("R", C.c_int32), ("grid", C.c_int32 * 3), ("w", C.c_float)]
+
+
 class sx_attn_probs_args(C.Structure):
     _fields_ = [("B", C.c_int32), ("M", C.c_int32), ("U1", C.c_int32), ("U2", C.c_int32), ("d", C.c_int32),
                 ("round_tf32", C.c_int32), ("Q", C.c_void_p), ("q_ld", C.c_int64), ("q_bstride", C.c_int64),
                 ("K", C.c_void_p), ("k_ld", C.c_int64), ("k_bstride", C.c_int64), ("alpha", C.c_float),
                 ("clip", C.c_float), ("P", C.c_void_p), ("S", C.c_void_p), ("ldp", C.c_int64), ("lse", C.c_void_p),
                 ("rowmax", C.c_void_p), ("stat", C.c_void_p), ("diag", C.c_void_p), ("drop_p", C.c_float),
-                ("_pad", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p)]
+                ("_pad", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("posbias", sx_posbias)]
 
 
 _P, _I, _L, _F, _U64, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64, C.c_double
@@ -62,6 +66,9 @@ _PROTOS = {
     "sx_prologue_bwd": [_P, _P, _L, _I, _I, _P, _P, _P, _I, _L, _F, _P, _F, _U64, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P],
     "sx_softmax_fwd": [_P, _L, _I, _L, _P, _F, _F, _U64, _P, _P, _I, _L, _I, _P, _P, _P],
     "sx_softmax_bwd": [_P, _L, _P, _L, _P, _L, _I, _P, _F, _F, _U64, _P, _L, _P, _I, _L, _I, _P],
+    "sx_softmax_posbias_fwd": [_P, _L, _I, _L, _P, _F, _F, _U64, _P, _P, _I, _L, _I, _P, _P, C.POINTER(sx_posbias), _P],
+    "sx_softmax_posbias_bwd": [_P, _L, _P, _L, _P, _L, _I, _P, _F, _F, _U64, _P, _L, _P, _I, _L, _I, C.POINTER(sx_posbias),
+                               _P, _P, _L, _P],
     "sx_layernorm_fwd": [_P, _L, _I, _P, _P, _P, _I, _I, _P, _P],
     "sx_layernorm_bwd": [_P, _P, _L, _I, _P, _P, _P, _I, _I, _P, _P, _P, _L, _P],
     "sx_ln_softaggr_fwd": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _F, _U64, _P, _P, _P, _P, _P],
@@ -130,7 +137,8 @@ def check(rc, what):
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
 _LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
-             "sx_attn_probs_fwd": 2, "sx_colsum": 2, "sx_colsum_batched": 2}
+             "sx_attn_probs_fwd": 2, "sx_colsum": 2, "sx_colsum_batched": 2,
+             "sx_softmax_posbias_bwd": 2}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing
 

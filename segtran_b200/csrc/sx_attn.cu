@@ -22,7 +22,15 @@
 // reference.  The lower clamp can only change a row whose own maximum is below -(clip - 104) while another row of the
 // same call exceeds +clip (fp32 exp underflow makes it a no-op everywhere else); such rows are counted in
 // stat[1] and surfaced by sx_attn_diag as diag[2] so that the host can assert it never happened.
+//
+// Positional biases (sx_posbias, segtran_shared.py:589-592): the HAS_BIAS instantiation adds w*log2(e)*table[o] after the
+// upper clamp, in the statistics pass and in the probabilities pass alike (the same arithmetic, so both see the same
+// value).  The table is staged in shared memory once per CTA; each thread decomposes its two query rows into grid
+// coordinates once per work item and steps the key coordinates along the chunk instead of dividing per element.  The raw
+// scores keep driving S, rowmax, stat[0] and the clamp; the low-row test widens by the bias range (header comment of
+// sx_attn_probs_args).  The unbiased instantiation is the kernel without any of this.
 #include "sx_common.cuh"
+#include "sx_posbias.cuh"
 #include "sx_tc.cuh"
 
 namespace {
@@ -60,8 +68,14 @@ struct AttnParams {
   unsigned long long drop_seed;
   const unsigned long long* drop_seed_dev;
   int round_tf32;
+  const float* pb_table;          // HAS_BIAS only
+  sxpb::Geom pb;
 };
 
+constexpr int PB_OFFSET = STAGES * STAGE_BYTES + 256;        // HAS_BIAS: w*log2(e)*table after the barriers
+constexpr int PB_MAX_FLOATS = 29 * 29 * 29;                   // 3-D R <= 14: the ring + table fit 227 KB
+
+template <bool HAS_BIAS>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -82,6 +96,24 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       sx::mbar_init(&empty_bar[s], 2);
     }
     sx::fence_barrier_init();
+  }
+  float* ptab = nullptr;
+  float* pred = nullptr;
+  if constexpr (HAS_BIAS) {
+    // stage w*log2(e)*table; the range of {w*table, 0} (natural units) for the low-row test, reduced per warp here and
+    // over the warps by every consumer after the barrier
+    ptab = reinterpret_cast<float*>(smem + PB_OFFSET);
+    pred = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 128);   // [12 warps][2]
+    float bmn = 0.f, bmx = 0.f;
+    for (int i = threadIdx.x; i < p.pb.T; i += NUM_THREADS) {
+      const float v = p.pb.w * p.pb_table[i];
+      ptab[i] = v * LOG2E;
+      bmn = fminf(bmn, v);
+      bmx = fmaxf(bmx, v);
+    }
+    bmx = sx::warp_max(bmx);
+    bmn = -sx::warp_max(-bmn);
+    if ((threadIdx.x & 31) == 0) { pred[2 * (threadIdx.x >> 5)] = bmn; pred[2 * (threadIdx.x >> 5) + 1] = bmx; }
   }
   __syncthreads();
 
@@ -135,6 +167,12 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   // this thread's column pair is elements (tc & 2, tc & 2 + 1) of a 4-element hash group: one word per pair
   const uint32_t dmul = sx::drop_mul((tc >> 1) & 1), dkey = sx::drop_key(dseed, (tc >> 1) & 1);
   float acc[64];
+  float brange = 0.f;                      // HAS_BIAS: max - min of {w*table, 0}
+  if constexpr (HAS_BIAS) {
+    float bmn = 0.f, bmx = 0.f;
+    for (int w = 0; w < NUM_THREADS / 32; ++w) { bmn = fminf(bmn, pred[2 * w]); bmx = fmaxf(bmx, pred[2 * w + 1]); }
+    brange = bmx - bmn;
+  }
 
   for (int it = blockIdx.x; it < p.items; it += gridDim.x) {
     int b, m, mb;
@@ -151,29 +189,71 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 
     // running statistics of the row over one chunk (log2 units; quad-uniform after the shuffles)
     auto chunk_stats = [&](int nb) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float cm = -3.0e38f;
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-#pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (nb * BN + 8 * j + tc + e < p.U2) cm = fmaxf(cm, acc[4 * j + 2 * h + e]);
-        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 1));
-        cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 2));
-        cm *= p.alpha2;                                       // alpha2 > 0: the max commutes with the scaling
-        rraw[h] = fmaxf(rraw[h], cm);
-        const float mn = fmaxf(rm[h], fminf(cm, p.clip2));
-        float s = 0.f;
+      if constexpr (HAS_BIAS) {
+        // one pass with a running (max, sum) per row; both rows share the key coordinates of the thread's columns
+        int qc[2][3], kc[3];
+        sxpb::coords(p.pb, grow[0], qc[0]);
+        sxpb::coords(p.pb, grow[1], qc[1]);
+        sxpb::coords(p.pb, nb * BN + tc, kc);
+        float cm[2] = {-3.0e38f, -3.0e38f}, mb[2] = {-3.0e38f, -3.0e38f}, s[2] = {0.f, 0.f};
 #pragma unroll
         for (int j = 0; j < 16; ++j)
 #pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (nb * BN + 8 * j + tc + e < p.U2) s += sx::ex2_approx(fminf(acc[4 * j + 2 * h + e] * p.alpha2, p.clip2) - mn);
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
-        rl[h] = rl[h] * sx::ex2_approx(rm[h] - mn) + s;
-        rm[h] = mn;
+          for (int e = 0; e < 2; ++e) {
+            if (nb * BN + 8 * j + tc + e < p.U2) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int o = sxpb::offset(p.pb, qc[h], kc);
+                const float v = acc[4 * j + 2 * h + e];
+                cm[h] = fmaxf(cm[h], v);
+                const float x = fminf(v * p.alpha2, p.clip2) + (o >= 0 ? ptab[o] : 0.f);
+                const float mn = fmaxf(mb[h], x);
+                s[h] = s[h] * sx::ex2_approx(mb[h] - mn) + sx::ex2_approx(x - mn);
+                mb[h] = mn;
+              }
+            }
+            sxpb::step(p.pb, kc, e ? 7 : 1);
+          }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int o = 1; o <= 2; o <<= 1) {
+            cm[h] = fmaxf(cm[h], __shfl_xor_sync(0xffffffffu, cm[h], o));
+            const float mo = __shfl_xor_sync(0xffffffffu, mb[h], o), so = __shfl_xor_sync(0xffffffffu, s[h], o);
+            const float mn = fmaxf(mb[h], mo);
+            s[h] = s[h] * sx::ex2_approx(mb[h] - mn) + so * sx::ex2_approx(mo - mn);
+            mb[h] = mn;
+          }
+          rraw[h] = fmaxf(rraw[h], cm[h] * p.alpha2);
+          const float mn = fmaxf(rm[h], mb[h]);
+          rl[h] = rl[h] * sx::ex2_approx(rm[h] - mn) + s[h] * sx::ex2_approx(mb[h] - mn);
+          rm[h] = mn;
+        }
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float cm = -3.0e38f;
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (nb * BN + 8 * j + tc + e < p.U2) cm = fmaxf(cm, acc[4 * j + 2 * h + e]);
+          cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 1));
+          cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 2));
+          cm *= p.alpha2;                                       // alpha2 > 0: the max commutes with the scaling
+          rraw[h] = fmaxf(rraw[h], cm);
+          const float mn = fmaxf(rm[h], fminf(cm, p.clip2));
+          float s = 0.f;
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (nb * BN + 8 * j + tc + e < p.U2) s += sx::ex2_approx(fminf(acc[4 * j + 2 * h + e] * p.alpha2, p.clip2) - mn);
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+          rl[h] = rl[h] * sx::ex2_approx(rm[h] - mn) + s;
+          rm[h] = mn;
+        }
       }
     };
     // final (max, sum, raw max) of the rows -> 1/sum; lse / rowmax / global statistics
@@ -186,7 +266,11 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
           if ((lane & 3) == 0) {
             p.lse[rowflat[h]] = (rm[h] + __log2f(rl[h])) * LN2;
             if (p.rowmax) p.rowmax[rowflat[h]] = rraw[h] * LN2;
-            if (rraw[h] * LN2 < -(p.clip - 104.f)) ++lowrows;
+            if constexpr (HAS_BIAS) {
+              if (rraw[h] * LN2 < -(p.clip - 104.f) + brange) ++lowrows;
+            } else {
+              if (rraw[h] * LN2 < -(p.clip - 104.f)) ++lowrows;
+            }
           }
         }
       }
@@ -197,8 +281,22 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       for (int h = 0; h < 2; ++h) {
         if (grow[h] >= p.U1) continue;
         const long long roff = rowflat[h] * p.ldp;
+        int qc[3], kc[3];                  // HAS_BIAS: key coordinates, stepped along the chunk as for_bias does
+        if constexpr (HAS_BIAS) {
+          sxpb::coords(p.pb, grow[h], qc);
+          sxpb::coords(p.pb, nb * BN + tc, kc);
+        }
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
+          float b0 = 0.f, b1 = 0.f;
+          if constexpr (HAS_BIAS) {
+            int o = sxpb::offset(p.pb, qc, kc);
+            if (o >= 0) b0 = ptab[o];
+            sxpb::step(p.pb, kc, 1);
+            o = sxpb::offset(p.pb, qc, kc);
+            if (o >= 0) b1 = ptab[o];
+            sxpb::step(p.pb, kc, 7);
+          }
           const int col = nb * BN + 8 * j + tc;
           if (col >= p.U2) continue;
           const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
@@ -206,8 +304,14 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
             if (col + 1 < p.U2) *reinterpret_cast<float2*>(p.S + roff + col) = make_float2(v0 * p.alpha, v1 * p.alpha);
             else p.S[roff + col] = v0 * p.alpha;
           }
-          float f0 = sx::ex2_approx(fminf(v0 * p.alpha2, p.clip2) - rm[h]) * rcp[h];
-          float f1 = sx::ex2_approx(fminf(v1 * p.alpha2, p.clip2) - rm[h]) * rcp[h];
+          float f0, f1;
+          if constexpr (HAS_BIAS) {
+            f0 = sx::ex2_approx(fminf(v0 * p.alpha2, p.clip2) + b0 - rm[h]) * rcp[h];
+            f1 = sx::ex2_approx(fminf(v1 * p.alpha2, p.clip2) + b1 - rm[h]) * rcp[h];
+          } else {
+            f0 = sx::ex2_approx(fminf(v0 * p.alpha2, p.clip2) - rm[h]) * rcp[h];
+            f1 = sx::ex2_approx(fminf(v1 * p.alpha2, p.clip2) - rm[h]) * rcp[h];
+          }
           if (p.drop_p > 0.f) {
             const uint32_t w = sx::drop_word_k(dmul, dkey, (unsigned long long)((roff + col) >> 2));
             f0 = (w & 0xFFFFu) >= p16 ? f0 * keep_scale : 0.f;
@@ -306,6 +410,15 @@ extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, void* stream) {
   p.drop_p = a->drop_p; p.drop_seed = a->drop_seed;
   p.drop_seed_dev = reinterpret_cast<const unsigned long long*>(a->drop_seed_dev);
   p.round_tf32 = a->round_tf32;
+  const bool has_bias = a->posbias.table != nullptr;
+  if (has_bias) {
+    SX_REQUIRE(a->U1 == a->U2, "sx_attn_probs_fwd: positional biases need self-attention (U1 == U2)");
+    const char* err = sxpb::check(&a->posbias, a->U1);
+    SX_REQUIRE(err == nullptr, "sx_attn_probs_fwd: %s", err);
+    p.pb_table = a->posbias.table;
+    p.pb = sxpb::make_geom(a->posbias);
+    SX_REQUIRE(p.pb.T <= PB_MAX_FLOATS, "sx_attn_probs_fwd: positional-bias table too large");
+  }
 
   // Q [Bq][U1][M*d] and K [B][U2][M*d] as (k, row, mode, batch) tensor maps: the per-mode slices are strided views
   sx_operand oq{}, ok{};
@@ -319,10 +432,16 @@ extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, void* stream) {
   rc = make_map(&tk, ok, 4, a->U2, a->d, a->M, a->B, BN, "K");
   if (rc) return rc;
 
-  SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel, SMEM_BYTES));
   const int grid = p.items < sms ? p.items : sms;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  sx_attn_probs_kernel<<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tq, tk, p);
+  if (has_bias) {
+    constexpr int smem_pb = PB_OFFSET + PB_MAX_FLOATS * 4 + 1024;
+    SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel<true>, smem_pb));
+    sx_attn_probs_kernel<true><<<grid, NUM_THREADS, PB_OFFSET + p.pb.T * 4 + 1024, st>>>(tq, tk, p);
+  } else {
+    SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel<false>, SMEM_BYTES));
+    sx_attn_probs_kernel<false><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tq, tk, p);
+  }
   SX_CHECK_CUDA(cudaGetLastError());
   attn_diag_kernel<<<1, 1, 0, st>>>(a->stat, a->clip, a->diag);
   SX_CHECK_CUDA(cudaGetLastError());

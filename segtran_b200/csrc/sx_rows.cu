@@ -5,6 +5,7 @@
 #include <algorithm>
 
 #include "sx_common.cuh"
+#include "sx_posbias.cuh"
 
 namespace {
 
@@ -332,6 +333,212 @@ __global__ void softmax_bwd_kernel(const float* __restrict__ dP, long long ldd, 
     }
     __syncwarp();
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// prologue without a positional code (pos_code_type 'bias' / 'none', segtran_shared.py:916, :940, :944-946):
+//   h = mask * dropout( LN_{g,b}(x) ),  stats[r] = {mean, rstd, 0, 1}
+// One warp per row.  The backward keeps one dg / db accumulator row per warp (a lane owns the columns c = lane mod 32,
+// so there are no atomics), adds the warps in order and stores the CTA's sums in its slot of `part`.
+// ------------------------------------------------------------------------------------------------
+constexpr int NOPOS_WARPS = 4;
+
+template <typename T>
+__global__ void __launch_bounds__(NOPOS_WARPS * 32)
+prologue_nopos_fwd_kernel(const float* __restrict__ x, long long R, int C, const float* __restrict__ g,
+                          const float* __restrict__ b, const float* __restrict__ mask, float drop_p, unsigned long long seed,
+                          const unsigned long long* __restrict__ seed_dev, T* __restrict__ h, float* __restrict__ stats, int rnd) {
+  seed += seed_dev ? *seed_dev : 0ull;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  for (long long r = (long long)blockIdx.x * NOPOS_WARPS + warp; r < R; r += (long long)gridDim.x * NOPOS_WARPS) {
+    const float* xr = x + r * C;
+    float m1, r1;
+    warp_mean_rstd(xr, C, lane, m1, r1);
+    const float mk = mask ? mask[r] : 1.f;
+    T* hr = h + r * C;
+    for (int c = lane; c < C; c += 32) {
+      float v = ((xr[c] - m1) * r1 * g[c] + b[c]) * mk;
+      if (drop_p > 0.f) v = sx::drop_keep1(seed, (unsigned long long)(r * C + c), sx::drop_p16(drop_p)) ? v * keep_scale : 0.f;
+      stf<T>(hr + c, v, rnd);
+    }
+    if (lane == 0) {
+      stats[r * 4 + 0] = m1; stats[r * 4 + 1] = r1; stats[r * 4 + 2] = 0.f; stats[r * 4 + 3] = 1.f;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(NOPOS_WARPS * 32)
+prologue_nopos_bwd_kernel(const float* __restrict__ dh, const float* __restrict__ x, long long R, int C,
+                          const float* __restrict__ g, const float* __restrict__ mask, float drop_p, unsigned long long seed,
+                          const unsigned long long* __restrict__ seed_dev, const float* __restrict__ stats,
+                          float* __restrict__ dx, float* __restrict__ part) {
+  seed += seed_dev ? *seed_dev : 0ull;
+  extern __shared__ float sm[];                     // [NOPOS_WARPS][2C]: dg | db per warp
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* acc = sm + (long long)warp * 2 * C;
+  for (int c = lane; c < 2 * C; c += 32) acc[c] = 0.f;
+  const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  for (long long r = (long long)blockIdx.x * NOPOS_WARPS + warp; r < R; r += (long long)gridDim.x * NOPOS_WARPS) {
+    const float m1 = stats[r * 4 + 0], r1 = stats[r * 4 + 1];
+    const float mk = mask ? mask[r] : 1.f;
+    const float* xr = x + r * C;
+    const float* dr = dh + r * C;
+    auto dy_at = [&](int c) {
+      float d = dr[c] * mk;
+      if (drop_p > 0.f) d = sx::drop_keep1(seed, (unsigned long long)(r * C + c), sx::drop_p16(drop_p)) ? d * keep_scale : 0.f;
+      return d;
+    };
+    float s1 = 0.f, s2 = 0.f;
+    for (int c = lane; c < C; c += 32) {
+      const float xh = (xr[c] - m1) * r1, dy = dy_at(c);
+      acc[c] += dy * xh;
+      acc[C + c] += dy;
+      const float da = dy * g[c];
+      s1 += da; s2 += da * xh;
+    }
+    s1 = sx::warp_sum(s1) / C; s2 = sx::warp_sum(s2) / C;
+    for (int c = lane; c < C; c += 32) {
+      const float xh = (xr[c] - m1) * r1;
+      dx[r * C + c] = r1 * (dy_at(c) * g[c] - s1 - xh * s2);
+    }
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) {
+    float v = 0.f;
+    for (int w = 0; w < NOPOS_WARPS; ++w) v += sm[(long long)w * 2 * C + c];
+    part[(long long)blockIdx.x * 2 * C + c] = v;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// softmax with a sliding-window positional bias (segtran_shared.py:578-605): one CTA per row, the row staged in shared
+// memory.  The bias is applied by walking the (2R+1)^pd window offsets of the row's query (each offset addresses at
+// most one key), and the backward gathers the row's dS' into the CTA's table accumulator the same way — one row at a
+// time, so the sums need no atomics; the CTA's table then goes to its slot of `part`.
+// ------------------------------------------------------------------------------------------------
+constexpr int PB_THREADS = 256;
+
+__device__ __forceinline__ float block_max(float v, float* red) {
+  v = sx::warp_max(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float m = red[0];
+  for (int w = 1; w < PB_THREADS / 32; ++w) m = fmaxf(m, red[w]);
+  __syncthreads();
+  return m;
+}
+__device__ __forceinline__ float block_sum(float v, float* red) {
+  v = sx::warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+  for (int w = 0; w < PB_THREADS / 32; ++w) s += red[w];
+  __syncthreads();
+  return s;
+}
+
+// row <- clamp_if(S row) + w * bias(q, .)
+__device__ __forceinline__ void posbias_stage_row(const float* __restrict__ sr, int L, bool do_clip, float clip,
+                                                  const float* __restrict__ table, const sxpb::Geom& G, int q, float* row) {
+  for (int c = threadIdx.x; c < L; c += PB_THREADS) {
+    float v = sr[c];
+    if (do_clip) v = fminf(fmaxf(v, -clip), clip);
+    row[c] = v;
+  }
+  __syncthreads();
+  int qc[3];
+  sxpb::coords(G, q, qc);
+  for (int o = threadIdx.x; o < G.T; o += PB_THREADS) {
+    const int k = sxpb::key_of(G, qc, o);
+    if (k >= 0) row[k] += G.w * table[o];
+  }
+  __syncthreads();
+}
+
+template <typename T>
+__global__ void __launch_bounds__(PB_THREADS)
+softmax_posbias_fwd_kernel(const float* __restrict__ S, long long R, int L, long long lds, const float* __restrict__ amax,
+                           float clip, float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
+                           T* __restrict__ P, long long ldp, float* __restrict__ lse, int rnd, float* __restrict__ diag,
+                           const float* __restrict__ table, const sxpb::Geom G) {
+  seed += seed_dev ? *seed_dev : 0ull;
+  extern __shared__ float sm[];
+  float* red = sm;                                  // [32]
+  float* row = sm + 32;                             // [L]
+  const bool do_clip = amax && (*amax > clip);
+  if (diag && amax && blockIdx.x == 0 && threadIdx.x == 0) {
+    diag[0] = fmaxf(diag[0], *amax);
+    if (do_clip) diag[1] += 1.f;
+  }
+  const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  for (long long r = blockIdx.x; r < R; r += gridDim.x) {
+    posbias_stage_row(S + r * lds, L, do_clip, clip, table, G, (int)(r % L), row);
+    float m = -3.0e38f;
+    for (int c = threadIdx.x; c < L; c += PB_THREADS) m = fmaxf(m, row[c]);
+    m = block_max(m, red);
+    float s = 0.f;
+    for (int c = threadIdx.x; c < L; c += PB_THREADS) { const float e = __expf(row[c] - m); row[c] = e; s += e; }
+    s = block_sum(s, red);
+    const float inv = 1.f / s;
+    T* pr = P + r * ldp;
+    for (int c = threadIdx.x; c < L; c += PB_THREADS) {
+      float v = row[c] * inv;
+      if (drop_p > 0.f) v = sx::drop_keep1(seed, (unsigned long long)(r * ldp + c), sx::drop_p16(drop_p)) ? v * keep_scale : 0.f;
+      stf<T>(pr + c, v, rnd);
+    }
+    if (threadIdx.x == 0 && lse) lse[r] = m + __logf(s);
+    __syncthreads();
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(PB_THREADS)
+softmax_posbias_bwd_kernel(const float* __restrict__ dP, long long ldd, const float* __restrict__ S, long long lds,
+                           const float* __restrict__ lse, long long R, int L, const float* __restrict__ amax, float clip,
+                           float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
+                           long long ldp_fwd, T* __restrict__ dS, long long ldo, int rnd, const float* __restrict__ table,
+                           const sxpb::Geom G, float* __restrict__ part) {
+  seed += seed_dev ? *seed_dev : 0ull;
+  extern __shared__ float sm[];
+  float* red = sm;                                  // [32]
+  float* tab = sm + 32;                             // [T] this CTA's table gradient
+  float* prow = tab + G.T;                          // [L] P, recomputed
+  float* grow = prow + L;                           // [L] masked dP, then dS'
+  for (int o = threadIdx.x; o < G.T; o += PB_THREADS) tab[o] = 0.f;
+  const bool do_clip = amax && (*amax > clip);
+  const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  for (long long r = blockIdx.x; r < R; r += gridDim.x) {
+    const int q = (int)(r % L);
+    posbias_stage_row(S + r * lds, L, do_clip, clip, table, G, q, prow);
+    const float l = lse[r];
+    float dot = 0.f;
+    for (int c = threadIdx.x; c < L; c += PB_THREADS) {
+      const float pv = __expf(prow[c] - l);
+      float gv = dP[r * ldd + c];
+      if (drop_p > 0.f)
+        gv = sx::drop_keep1(seed, (unsigned long long)(r * ldp_fwd + c), sx::drop_p16(drop_p)) ? gv * keep_scale : 0.f;
+      prow[c] = pv; grow[c] = gv;
+      dot += pv * gv;
+    }
+    dot = block_sum(dot, red);
+    for (int c = threadIdx.x; c < L; c += PB_THREADS) {
+      const float d = prow[c] * (grow[c] - dot);
+      grow[c] = d;
+      float o = d;
+      if (do_clip) { const float v = S[r * lds + c]; if (v < -clip || v > clip) o = 0.f; }
+      stf<T>(dS + r * ldo + c, o, rnd);
+    }
+    __syncthreads();
+    int qc[3];
+    sxpb::coords(G, q, qc);
+    for (int o = threadIdx.x; o < G.T; o += PB_THREADS) {
+      const int k = sxpb::key_of(G, qc, o);
+      if (k >= 0) tab[o] += grow[k];
+    }
+    __syncthreads();
+  }
+  for (int o = threadIdx.x; o < G.T; o += PB_THREADS) part[(long long)blockIdx.x * G.T + o] = G.w * tab[o];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -894,6 +1101,18 @@ extern "C" int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, 
                                const float* pe, int32_t C0, int64_t pe_bstride, float posw, const float* mask,
                                float drop_p, uint64_t seed, const uint64_t* seed_dev, void* h, int32_t h_dtype, int32_t round_tf32, float* stats,
                                void* stream) {
+  if (!pe) {                                        // no positional code: h = mask * dropout(LN_{g,b}(x))
+    const long long R = (long long)B * N;
+    const int grid = grid_for_rows(R, NOPOS_WARPS, sms_cached());
+    if (h_dtype == SX_F32)
+      prologue_nopos_fwd_kernel<float><<<grid, NOPOS_WARPS * 32, 0, ST(stream)>>>(
+          x, R, C, g, b, mask, drop_p, seed, (const unsigned long long*)seed_dev, (float*)h, stats, round_tf32);
+    else
+      prologue_nopos_fwd_kernel<__nv_bfloat16><<<grid, NOPOS_WARPS * 32, 0, ST(stream)>>>(
+          x, R, C, g, b, mask, drop_p, seed, (const unsigned long long*)seed_dev, (__nv_bfloat16*)h, stats, 0);
+    SX_CHECK_CUDA(cudaGetLastError());
+    return 0;
+  }
   if (h_dtype == SX_F32 && C % 4 == 0 && C <= 2048 && C0 % 4 == 0 && pe_bstride % 4 == 0 && al16(x) && al16(h) && al16(pe) &&
       al16(g) && al16(b)) {
     // CTA-per-row kernel: the row in registers, 16-byte accesses at every width
@@ -928,6 +1147,19 @@ extern "C" int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32
                                const float* b, const float* pe, int32_t C0, int64_t pe_bstride, float posw,
                                const float* mask, float drop_p, uint64_t seed, const uint64_t* seed_dev, const float* stats, float* dx, float* dg,
                                float* db, float* dpe, float* dt_scratch, float* part, int64_t part_floats, void* stream) {
+  if (!pe) {
+    SX_REQUIRE(!dpe, "sx_prologue_bwd: dpe must be NULL without a positional code");
+    const long long R = (long long)B * N;
+    SX_REQUIRE(part && part_floats >= 2ll * C, "sx_prologue_bwd: needs at least %lld floats of scratch", 2ll * C);
+    const int grid = std::min(grid_for_rows(R, NOPOS_WARPS, sms_cached()), part_slots(part_floats, 2ll * C));
+    const size_t smem = (size_t)NOPOS_WARPS * 2 * C * 4;
+    SX_REQUIRE(smem <= 200 * 1024, "sx_prologue_bwd: C=%d too large", C);
+    if (set_smem(prologue_nopos_bwd_kernel, smem)) return -2;
+    prologue_nopos_bwd_kernel<<<grid, NOPOS_WARPS * 32, smem, ST(stream)>>>(
+        dh, x, R, C, g, mask, drop_p, seed, (const unsigned long long*)seed_dev, stats, dx, part);
+    SX_CHECK_CUDA(cudaGetLastError());
+    return part_reduce(part, grid, 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream));
+  }
   if (C % 4 == 0 && C <= 2048 && C0 % 4 == 0 && pe_bstride % 4 == 0 && al16(dh) && al16(x) && al16(dx) && al16(pe) && al16(g) &&
       al16(b) && (!dpe || (dt_scratch && al16(dt_scratch) && al16(dpe)))) {
     // CTA-per-row kernel: x / dh read once, dx (and dt, when the positional-code gradient needs it) written once, dg / db
@@ -1415,4 +1647,59 @@ extern "C" int sx_add(const float* a, const float* b, int64_t n, float* y, void*
   add_kernel<<<grid_for_rows(n, 256 * 4, sms_cached()), 256, 0, ST(stream)>>>(a, b, n, y);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int sx_softmax_posbias_fwd(const float* S, int64_t R, int32_t L, int64_t lds, const float* amax, float clip,
+                                      float drop_p, uint64_t seed, const uint64_t* seed_dev, void* P, int32_t p_dtype,
+                                      int64_t ldp, int32_t round_tf32, float* lse, float* diag, const sx_posbias* posbias,
+                                      void* stream) {
+  const char* err = sxpb::check(posbias, L);
+  SX_REQUIRE(err == nullptr, "sx_softmax_posbias_fwd: %s", err);
+  SX_REQUIRE(R % L == 0, "sx_softmax_posbias_fwd: rows must be whole [L x L] blocks");
+  const sxpb::Geom G = sxpb::make_geom(*posbias);
+  const size_t smem = (size_t)(32 + L) * 4;
+  SX_REQUIRE(smem <= 200 * 1024, "sx_softmax_posbias_fwd: L=%d too large", L);
+  const int grid = (int)std::min<long long>(R, (long long)sms_cached() * 8);
+  if (p_dtype == SX_F32) {
+    if (set_smem(softmax_posbias_fwd_kernel<float>, smem)) return -2;
+    softmax_posbias_fwd_kernel<float><<<grid, PB_THREADS, smem, ST(stream)>>>(
+        S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, (float*)P, ldp, lse, round_tf32, diag,
+        posbias->table, G);
+  } else {
+    if (set_smem(softmax_posbias_fwd_kernel<__nv_bfloat16>, smem)) return -2;
+    softmax_posbias_fwd_kernel<__nv_bfloat16><<<grid, PB_THREADS, smem, ST(stream)>>>(
+        S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, (__nv_bfloat16*)P, ldp, lse, 0, diag,
+        posbias->table, G);
+  }
+  SX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int sx_softmax_posbias_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, const float* lse, int64_t R,
+                                      int32_t L, const float* amax, float clip, float drop_p, uint64_t seed,
+                                      const uint64_t* seed_dev, int64_t ldp_fwd, void* dS, int32_t ds_dtype, int64_t ldo,
+                                      int32_t round_tf32, const sx_posbias* posbias, float* dtable, float* part,
+                                      int64_t part_floats, void* stream) {
+  const char* err = sxpb::check(posbias, L);
+  SX_REQUIRE(err == nullptr, "sx_softmax_posbias_bwd: %s", err);
+  SX_REQUIRE(R % L == 0, "sx_softmax_posbias_bwd: rows must be whole [L x L] blocks");
+  SX_REQUIRE(dtable != nullptr, "sx_softmax_posbias_bwd: null dtable");
+  const sxpb::Geom G = sxpb::make_geom(*posbias);
+  SX_REQUIRE(part && part_floats >= G.T, "sx_softmax_posbias_bwd: needs at least %d floats of scratch", G.T);
+  const size_t smem = (size_t)(32 + G.T + 2 * (size_t)L) * 4;
+  SX_REQUIRE(smem <= 200 * 1024, "sx_softmax_posbias_bwd: L=%d too large", L);
+  const int grid = (int)std::min<long long>(std::min<long long>(R, (long long)sms_cached() * 4), part_slots(part_floats, G.T));
+  if (ds_dtype == SX_F32) {
+    if (set_smem(softmax_posbias_bwd_kernel<float>, smem)) return -2;
+    softmax_posbias_bwd_kernel<float><<<grid, PB_THREADS, smem, ST(stream)>>>(
+        dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, ldp_fwd, (float*)dS, ldo,
+        round_tf32, posbias->table, G, part);
+  } else {
+    if (set_smem(softmax_posbias_bwd_kernel<__nv_bfloat16>, smem)) return -2;
+    softmax_posbias_bwd_kernel<__nv_bfloat16><<<grid, PB_THREADS, smem, ST(stream)>>>(
+        dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, ldp_fwd,
+        (__nv_bfloat16*)dS, ldo, 0, posbias->table, G, part);
+  }
+  SX_CHECK_CUDA(cudaGetLastError());
+  return part_reduce(part, grid, G.T, PartDst{{dtable, nullptr, nullptr, nullptr}, {G.T, 0, 0, 0}}, ST(stream));
 }

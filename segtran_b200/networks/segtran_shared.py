@@ -9,8 +9,9 @@ checkpoints load with ``load_state_dict``), while every forward runs on the sm_9
 Supported configuration = the one the reference's drivers force (train3d.py:174-178, train2d.py:245-249):
 squeezed attention (or plain cross attention), pos_code_type 'lsinu', mid_type 'shared',
 trans_output_type 'private'|'shared', tie_qk 'shared'|'loose'|'none', pool_modes_feat 'softmax', plus
---nosqueeze and --squeezeuseffn.  Ablation-only
-switches (mince, sliding biases, multihead, rand/sinu/none position codes) raise NotImplementedError.
+--nosqueeze and --squeezeuseffn, and the positional-code ablations --pos bias (sliding-window biases inside the
+attention softmax, plain attention only) and --pos none.  The other ablation-only switches (mince, multihead, rand/sinu
+position codes) raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -257,9 +258,9 @@ class ExpandedFeatTrans(nn.Module):
         return ops.ln_softaggr(y, ln.weight, ln.bias, f2s.weight, f2s.bias, drop_p=p,
                                seed=ops.new_dropout_seed(y.device) if p > 0 else 0)
 
-    def forward_from_qk(self, input_feat, q, k, clip, att_p, diag):
+    def forward_from_qk(self, input_feat, q, k, clip, att_p, diag, posbias=None):
         """Fused attention entry: q [Bq,U1,M*d], k [B,U2,M*d] (projected, TF32-rounded) instead of the probabilities —
-        scores, clamp, softmax and attention dropout run inside ops.squeeze_out_fused (csrc/sx_attn.cu)."""
+        scores, clamp, positional bias, softmax and attention dropout run inside ops.squeeze_out_fused (csrc/sx_attn.cu)."""
         mid = self.intermediate
         vp = self._value_bank(input_feat, ops.small_tag(input_feat.shape[1], q.shape[1]))
         p = mid.dropout.p if self.training else 0.0
@@ -267,7 +268,7 @@ class ExpandedFeatTrans(nn.Module):
         dev = vp.device
         y = ops.squeeze_out_fused(q, k, vp, self.num_modes, clip, att_p, ops.new_dropout_seed(dev) if att_p > 0 else 0,
                                   mid.shared_linear.bias, p, ops.new_dropout_seed(dev) if p > 0 else 0, gl.weight, gl.bias,
-                                  diag)
+                                  diag, posbias)
         return self._norm_aggregate(y)
 
     def forward(self, input_feat, attention_probs, in_geoshape=None):
@@ -316,8 +317,12 @@ class CrossAttFeatTrans(nn.Module):
         self.key = nn.Linear(self.in_feat_dim, self.att_size_allmode, bias=config.qk_have_bias)
         self.base_initializer_range = config.base_initializer_range
         if config.pos_code_type == 'bias':
-            _unsupported("pos_code_type='bias'")
-        self.pos_code_weight = 1
+            if config.use_attn_consist_loss:
+                raise NotImplementedError("segtran_b200: --attnconsist with --pos bias is not implemented (the attention "
+                                          "scores this build keeps do not include the positional biases)")
+            self.pos_code_weight = config.pos_code_weight
+        else:
+            self.pos_code_weight = 1
         if config.ablate_multihead:
             _unsupported("ablate_multihead")
         self.out_trans = ExpandedFeatTrans(config, name)
@@ -372,10 +377,20 @@ class CrossAttFeatTrans(nn.Module):
         return self._diag_values()[1]
 
     def forward(self, in_query, in_key=None, pos_biases=None):
-        if pos_biases is not None:
-            _unsupported("positional biases")
+        """pos_biases: an ops.PosBias over the tokens of a self-attention (the reference's [1,1,N,N] bias matrix, kept
+        as its window table); it is added to the scores after the clamp, scaled by pos_code_weight (:589-592)."""
         if in_key is None:
             in_key = in_query
+        pb = None
+        if pos_biases is not None:
+            if not isinstance(pos_biases, ops.PosBias):
+                raise TypeError("CrossAttFeatTrans: pos_biases must be an ops.PosBias (SlidingPosBiases2D/3D output)")
+            if self.keep_attn_scores:
+                raise NotImplementedError("segtran_b200: --attnconsist with --pos bias is not implemented")
+            if in_query.shape[1] != pos_biases.num_tokens or in_key.shape[1] != pos_biases.num_tokens:
+                raise ValueError("CrossAttFeatTrans: positional biases over %s cells need a self-attention over as many "
+                                 "tokens (got %d queries, %d keys)" % (pos_biases.grid, in_query.shape[1], in_key.shape[1]))
+            pb = pos_biases.with_weight(float(self.pos_code_weight))
         M = self.num_modes
         # precision classes (ops.small_tag): the projection of the shorter side is an attractor-row product when that side is
         # at most a quarter of the other one; everything else is a token-row projection
@@ -395,10 +410,14 @@ class CrossAttFeatTrans(nn.Module):
             self.attention_scores = None
             if self.training:
                 self.call_count += 1
-            return self.out_trans.forward_from_qk(in_key, q, k, float(self.attn_clip), p, self._diag)
+            return self.out_trans.forward_from_qk(in_key, q, k, float(self.attn_clip), p, self._diag, pb)
         amax = torch.full((1,), -3.0e38, device=dev)
         s = ops.attn_scores(q, k, M, amax)                                   # [B,M,U1,U2], max tracked on device
-        probs = ops.softmax(s, amax, float(self.attn_clip), p, ops.new_dropout_seed(dev) if p > 0 else 0, self._diag)
+        seed = ops.new_dropout_seed(dev) if p > 0 else 0
+        if pb is not None:
+            probs = ops.softmax_posbias(s, pb, amax, float(self.attn_clip), p, seed, self._diag)
+        else:
+            probs = ops.softmax(s, amax, float(self.attn_clip), p, seed, self._diag)
         self.attention_scores = s if self.keep_attn_scores else None
         if self.training:
             self.call_count += 1
@@ -500,23 +519,109 @@ class LearnedSinuPosEmbedder(nn.Module):
         return pe.view(*shp[:-1], -1)
 
 
+class NoneEmbedder(nn.Module):
+    """pos_code_type 'none': no positional code at all (reference segtran_ablation.py:68-74)."""
+
+    def forward(self, pos_normed):
+        return None
+
+
+class _SlidingPosBiases(nn.Module):
+    """Sliding-window positional biases (reference SlidingPosBiases2D/3D, segtran_shared.py:1002-1175): one learned
+    `biases` table [2R+1]^pd, zero-initialised.  The query at cell q and the key at cell k (row-major cells of the
+    feature grid) get biases[k - q + R] when |k_i - q_i| <= R in every dimension, else 0.
+    The reference expands the table into an [N,N] matrix through persistent int64 index buffers (all_h1s, ...: 1.3 GB
+    at the 3-D default max_pos_size); here forward returns the table and the grid (ops.PosBias), and the attention
+    kernels read the table directly.  Those buffers are not allocated: a reference checkpoint's all_* entries are
+    accepted and dropped on load, and this module's state_dict is the reference's minus them."""
+
+    _INDEX_BUFFERS = ()
+
+    def __init__(self, pos_dim, pos_bias_radius, max_pos_size):
+        super().__init__()
+        if pos_dim != self._POS_DIM:
+            raise ValueError("%s: pos_dim must be %d" % (type(self).__name__, self._POS_DIM))
+        if pos_bias_radius < 1:
+            raise ValueError("%s: pos_bias_radius must be >= 1 (got %d)" % (type(self).__name__, pos_bias_radius))
+        self.pos_dim = pos_dim
+        self.R = pos_bias_radius
+        self.max_pos_size = tuple(int(m) for m in max_pos_size)
+        self.biases = nn.Parameter(torch.zeros([2 * pos_bias_radius + 1] * pos_dim))
+
+    def forward(self, feat_shape, device=None, table=None):
+        """feat_shape: the token grid (its last pos_dim extents) -> ops.PosBias with weight 1 (CrossAttFeatTrans applies
+        pos_code_weight).  table: a stand-in for `biases` (the eval-mode snapshot of SegtranPosEncoder)."""
+        grid = tuple(int(s) for s in tuple(feat_shape)[-self.pos_dim:])
+        if any(g > m for g, m in zip(grid, self.max_pos_size)):
+            raise ValueError("%s: feature grid %s exceeds max_pos_size %s" % (type(self).__name__, grid, self.max_pos_size))
+        return ops.PosBias(self.biases if table is None else table, self.R, grid, 1.0)
+
+    def _load_from_state_dict(self, state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
+        for name in self._INDEX_BUFFERS:
+            state_dict.pop(prefix + name, None)
+        super()._load_from_state_dict(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs)
+
+
+class SlidingPosBiases2D(_SlidingPosBiases):
+    _POS_DIM = 2
+    _INDEX_BUFFERS = ('all_h1s', 'all_w1s', 'all_h2s', 'all_w2s')
+
+    def __init__(self, pos_dim, pos_bias_radius=7, max_pos_size=(100, 100)):
+        super().__init__(pos_dim, pos_bias_radius, max_pos_size)
+
+
+class SlidingPosBiases3D(_SlidingPosBiases):
+    _POS_DIM = 3
+    _INDEX_BUFFERS = ('all_h1s', 'all_w1s', 'all_d1s', 'all_h2s', 'all_w2s', 'all_d2s')
+
+    def __init__(self, pos_dim, pos_bias_radius=7, max_pos_size=(20, 20, 20)):
+        super().__init__(pos_dim, pos_bias_radius, max_pos_size)
+
+
 class SegtranPosEncoder(nn.Module):
-    """pos / pos.max() -> learnable sinusoid code; cached in eval mode (reference :1177-1238)."""
+    """pos / pos.max() -> learnable sinusoid code ('lsinu'), sliding-window biases ('bias') or nothing ('none'); cached
+    in eval mode (reference :1177-1238)."""
 
     def __init__(self, config):
         super().__init__()
         self.feat_dim = config.trans_in_dim
         self.pos_embed_dim = self.feat_dim
         self.pos_code_type = config.pos_code_type
-        if self.pos_code_type != 'lsinu':
+        if self.pos_code_type == 'lsinu':
+            self.pos_coder = LearnedSinuPosEmbedder(config.pos_dim, self.pos_embed_dim, omega=1, affine=False)
+        elif self.pos_code_type == 'none':
+            self.pos_coder = NoneEmbedder()
+        elif self.pos_code_type == 'bias':
+            cls = {2: SlidingPosBiases2D, 3: SlidingPosBiases3D}.get(config.pos_dim)
+            if cls is None:
+                raise ValueError("SegtranPosEncoder: positional biases need pos_dim 2 or 3 (got %r)" % config.pos_dim)
+            self.pos_coder = cls(config.pos_dim, config.pos_bias_radius, config.max_pos_size)
+        else:
             _unsupported("pos_code_type=%r" % self.pos_code_type)
-        self.pos_coder = LearnedSinuPosEmbedder(config.pos_dim, self.pos_embed_dim, omega=1, affine=False)
         self.cached_pos_code = None
         self.cached_feat_shape = None
 
     def forward(self, orig_feat_shape, voxels_pos):
-        """voxels_pos [B,N,pd] -> code [N,C0] when the batch shares one set of positions (stride-0 batch dim or
-        B == 1), else [B,N,C0].  The global max of the whole tensor normalises the positions (:1231)."""
+        """'lsinu': voxels_pos [B,N,pd] -> code [N,C0] when the batch shares one set of positions (stride-0 batch dim or
+        B == 1), else [B,N,C0].  The global max of the whole tensor normalises the positions (:1231).
+        'bias': -> ops.PosBias over the grid orig_feat_shape.  A forward that can differentiate (training, or eval with
+        grad enabled) reads the live table, so `biases` gets its gradient, and caches a snapshot of the values it read.
+        An eval pass under no_grad on the same feature shape reuses that snapshot; a new shape snapshots the table afresh
+        (:1209-1215).  So inference right after training sees the table of the last training forward, as the reference's
+        cached [N,N] matrix does; like the lsinu cache, a code that would carry a graph is rebuilt rather than
+        re-used.  'none': -> None."""
+        if self.pos_code_type == 'none':
+            return None
+        if self.pos_code_type == 'bias':
+            key = tuple(int(s) for s in orig_feat_shape)
+            if self.training or (torch.is_grad_enabled() and self.pos_coder.biases.requires_grad):
+                self.cached_pos_code = self.pos_coder(key, table=self.pos_coder.biases.detach().clone())
+                self.cached_feat_shape = key
+                return self.pos_coder(key)
+            if self.cached_pos_code is None or self.cached_feat_shape != key:
+                self.cached_pos_code = self.pos_coder(key, table=self.pos_coder.biases.detach().clone())
+                self.cached_feat_shape = key
+            return self.cached_pos_code
         key = tuple(voxels_pos.shape)              # shape-keyed like the reference's cache (:1219)
         if not self.training and self.cached_pos_code is not None and self.cached_feat_shape == key and \
                 not (torch.is_grad_enabled() and self.cached_pos_code.requires_grad):
@@ -547,11 +652,15 @@ class SegtranFusionEncoder(nn.Module):
         self.use_mince_transformer = config.use_mince_transformer
         if self.use_mince_transformer:
             _unsupported("the mince transformer")
-        if self.pos_code_type == 'bias':
+        if self.use_squeezed_transformer and self.pos_code_type == 'bias':
             print("Squeezed transformer cannot use Positional Biases.")
             print("Please specify '--nosqueeze' to disable squeezed transformer.")
             exit(0)
-        self.pos_code_weight = config.pos_code_weight
+        if self.pos_code_type == 'bias' and config.use_attn_consist_loss:
+            raise NotImplementedError("segtran_b200: --attnconsist with --pos bias is not implemented (the attention "
+                                      "scores this build keeps do not include the positional biases)")
+        # with sliding-window biases the code is not added to the features (:847-850)
+        self.pos_code_weight = config.pos_code_weight if self.pos_code_type != 'bias' else 0
         self.num_scales = 0
         self.pos_code_layer = SegtranPosEncoder(config)
         layer_cls = SqueezedAttFeatTrans if self.use_squeezed_transformer else CrossAttFeatTrans
@@ -587,10 +696,13 @@ class SegtranFusionEncoder(nn.Module):
             pe = self.pos_code_layer(orig_feat_shape, voxels_pos)
             ln = self.vfeat_norm_layers[i]
             p = self.dropout.p if (self.training and i == 0) else 0.0
-            h = ops.prologue(x, ln.weight, ln.bias, pe, float(self.pos_code_weight), mask, p,
+            # 'bias' / 'none': no code on the features and no comb_norm_layers LayerNorm (:929-940); the biases (shared
+            # by every layer) go into the attention scores instead
+            feat_pe = pe if self.pos_code_type == 'lsinu' else None
+            h = ops.prologue(x, ln.weight, ln.bias, feat_pe, float(self.pos_code_weight), mask, p,
                              ops.new_dropout_seed(x.device) if p > 0 else 0)
             ops.grad_ready(h, layer.parameters())                   # backward past `h`: this layer's weights are final
-            x = layer(h, pos_biases=None)
+            x = layer(h, pos_biases=pe if self.pos_code_type == 'bias' else None)
             self.layers_vfeat.append(x)
             if self.use_attn_consist_loss:
                 if self.use_squeezed_transformer:

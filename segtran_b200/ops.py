@@ -649,10 +649,54 @@ class _AttnScores(torch.autograd.Function):
         return dq, dk, None, None, drb, None
 
 
-def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_scores=False, round_out=True):
+class PosBias:
+    """Sliding-window positional bias of a self-attention (SlidingPosBiases2D/3D, segtran_shared.py:1002-1175) without
+    the [N,N] matrix: token n is cell n of the row-major grid `grid` (2 or 3 extents), and the score of query q and key k
+    gains w * table[k - q + R] (per dimension) when k lies within R cells of q in every dimension, 0 otherwise.
+    table [2R+1]^pd is the learned parameter (or an eval-mode snapshot of it); w is pos_code_weight."""
+    __slots__ = ("table", "R", "grid", "w")
+
+    def __init__(self, table, R, grid, w=1.0):
+        grid = tuple(int(g) for g in grid)
+        if len(grid) not in (2, 3) or table.dim() != len(grid) or any(s != 2 * R + 1 for s in table.shape):
+            raise L.SxError("PosBias: table %s does not match radius %d over grid %s" % (tuple(table.shape), R, grid))
+        self.table, self.R, self.grid, self.w = table, int(R), grid, float(w)
+
+    def with_weight(self, w):
+        return PosBias(self.table, self.R, self.grid, w)
+
+    @property
+    def num_tokens(self):
+        n = 1
+        for g in self.grid:
+            n *= g
+        return n
+
+
+def _posbias_desc(table, R, grid, w) -> L.sx_posbias:
+    d = L.sx_posbias()
+    d.table = table.data_ptr()
+    d.pd, d.R = len(grid), R
+    for i, g in enumerate(grid):
+        d.grid[i] = g
+    d.w = w
+    return d
+
+
+def _posbias_table(pb):
+    t = pb.table
+    if t.dtype != torch.float32 or not t.is_contiguous():
+        raise L.SxError("positional-bias table must be contiguous fp32")
+    _req_cuda(t)
+    return t
+
+
+def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_scores=False, round_out=True, posbias=None):
     """P = dropout(softmax(min(Q K^T / sqrt(d), clip))) per mode in ONE wgmma kernel (csrc/sx_attn.cu): the scores stay
     in registers and the softmax runs on the accumulator fragments (reference segtran_shared.py:566-567, :569-580, :601, :605).
     q [Bq,U1,M*d] (Bq = 1 broadcasts), k [B,U2,M*d], both contiguous fp32 (TF32-rounded by their producers).
+    posbias (PosBias, self-attention only): adds the sliding-window bias inside the softmax, after the clamp; S, rowmax
+    and the clamp statistics stay on the raw scores (its table gradient comes from softmax_posbias_backward).
     -> (P [B,M,U1,U2] view of a row-padded buffer, S or None (raw scaled scores, same layout), lse [B,M,U1],
         rowmax [B,M,U1], stat [2])."""
     _req_cuda(q, k)
@@ -678,6 +722,8 @@ def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_sc
     a.lse, a.rowmax, a.stat, a.diag = lse.data_ptr(), rowmax.data_ptr(), stat.data_ptr(), _ptr(diag)
     a.drop_p = drop_p
     a.drop_seed, a.drop_seed_dev = _seed_args(seed)
+    if posbias is not None:
+        a.posbias = _posbias_desc(_posbias_table(posbias), posbias.R, posbias.grid, posbias.w)
     L.call("sx_attn_probs_fwd", C.byref(a), _stream())
     return P, S, lse, rowmax, stat
 
@@ -774,6 +820,54 @@ class _Softmax(torch.autograd.Function):
         L.call("sx_softmax_bwd", dP.data_ptr(), dP.stride(-2), S.data_ptr(), S.stride(-2), lse.data_ptr(), R, Lr,
                _ptr(amax), clip, drop_p, *_seed_args(seed), ldp, dS.data_ptr(), L.SX_F32, dS.stride(-2), _rt(), _stream())
         return dS, None, None, None, None, None
+
+
+def softmax_posbias_backward(dP, ldd, S, lds, lse, R, Lr, amax, clip, drop_p, seed, ldp_fwd, dS, ldo, table, pb_geom,
+                             table_needs_grad):
+    """dS (with the clamp mask) and the table gradient of the biased softmax.  The table gradient goes straight into the
+    table's .grad when direct accumulation is on (returns None then), else into a new tensor that is returned."""
+    R_, grid, w = pb_geom
+    tgt = _grad_target(table) if table_needs_grad else None
+    buf = tgt if tgt is not None else _zeros((table.numel(),), table.device)
+    desc = _posbias_desc(table, R_, grid, w)
+    L.call("sx_softmax_posbias_bwd", dP.data_ptr(), ldd, S.data_ptr(), lds, lse.data_ptr(), R, Lr, _ptr(amax), clip, drop_p,
+           *_seed_args(seed), ldp_fwd, dS.data_ptr(), L.SX_F32, ldo, _rt(), C.byref(desc), buf.data_ptr(),
+           *_part_args(dS.device), _stream())
+    if tgt is not None or not table_needs_grad:
+        return None
+    return buf.view(table.shape)
+
+
+class _SoftmaxPosBias(torch.autograd.Function):
+    """P = dropout(softmax(clamp_if(S) + w * bias))  (segtran_shared.py:578-605 with pos_biases); S is the raw [B,M,N,N]
+    score tensor of a self-attention over the bias grid.  Backward: dS and the table gradient."""
+
+    @staticmethod
+    def forward(ctx, S, amax, clip, drop_p, seed, diag, table, pb_geom):
+        S = _rowpad(S)
+        Lr, ld = S.shape[-1], S.stride(-2)
+        R = S.numel() // Lr
+        P = _rowpad_empty(S.shape, S.device)
+        lse = torch.empty(R, device=S.device, dtype=torch.float32)
+        desc = _posbias_desc(table, *pb_geom)
+        L.call("sx_softmax_posbias_fwd", S.data_ptr(), R, Lr, ld, _ptr(amax), clip, drop_p, *_seed_args(seed), P.data_ptr(),
+               L.SX_F32, P.stride(-2), _rt(), lse.data_ptr(), _ptr(diag), C.byref(desc), _stream())
+        ctx.save_for_backward(S, lse, amax, table)
+        ctx.meta = (clip, drop_p, seed, P.stride(-2), pb_geom)
+        ctx.leaf = table
+        return P
+
+    @staticmethod
+    def backward(ctx, dP):
+        S, lse, amax, table = ctx.saved_tensors
+        clip, drop_p, seed, ldp, pb_geom = ctx.meta
+        dP = _rowpad(dP)
+        Lr = S.shape[-1]
+        R = S.numel() // Lr
+        dS = _rowpad_empty(S.shape, S.device)
+        dT = softmax_posbias_backward(dP, dP.stride(-2), S, S.stride(-2), lse, R, Lr, amax, clip, drop_p, seed, ldp, dS,
+                                      dS.stride(-2), ctx.leaf, pb_geom, ctx.needs_input_grad[6])
+        return dS, None, None, None, None, None, dT, None
 
 
 class _AttnPV(torch.autograd.Function):
@@ -1009,14 +1103,15 @@ class _SqueezeOutFused(torch.autograd.Function):
     (input-gradient error 1.3e-2 at cfg 1 / cfg 4 against 6e-4 for this form), so it is not used."""
 
     @staticmethod
-    def forward(ctx, q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag):
+    def forward(ctx, q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag, table=None, pb_geom=None):
         B, U2 = k.shape[0], k.shape[1]
         U1 = q.shape[1]
         Fd = vp.shape[-1] // M
         q = q.contiguous()
         k = k.contiguous()
         need_bwd = any(ctx.needs_input_grad)
-        P, S, lse, _rowmax, stat = attn_probs_fused(q, k, M, clip, att_p, att_seed, diag, need_scores=need_bwd)
+        pb = PosBias(table, pb_geom[0], pb_geom[1], pb_geom[2]) if table is not None else None
+        P, S, lse, _rowmax, stat = attn_probs_fused(q, k, M, clip, att_p, att_seed, diag, need_scores=need_bwd, posbias=pb)
         vv = vp.view(B, U2, M, Fd).permute(0, 2, 3, 1)
         G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
         H = torch.empty_like(G)
@@ -1028,6 +1123,7 @@ class _SqueezeOutFused(torch.autograd.Function):
         ctx.meta = (M, Fd, float(clip), att_p, hid_p, bm is not None, Wo.shape)
         ctx.seeds = (att_seed, hid_seed)
         ctx.leaves = (bm, Wo, bo)
+        ctx.pb = (table, pb_geom)
         return Y
 
     @staticmethod
@@ -1036,6 +1132,8 @@ class _SqueezeOutFused(torch.autograd.Function):
         M, Fd, clip, att_p, hid_p, has_bm, wshape = ctx.meta
         att_seed, hid_seed = ctx.seeds
         bm, Wo, bo = ctx.leaves
+        table, pb_geom = ctx.pb
+        dT = None
         B, _, U1, U2 = P.shape
         Bq, d = q.shape[0], q.shape[-1] // M
         dY = dY.contiguous()
@@ -1064,13 +1162,17 @@ class _SqueezeOutFused(torch.autograd.Function):
             dvp = torch.empty_like(vp)
             gemm_nt(P.transpose(-1, -2), dH.transpose(-1, -2), out=dvp.view(B, U2, M, Fd).permute(0, 2, 1, 3),
                     round_out=False)
-        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (table is not None and ctx.needs_input_grad[13]):
             dP = torch.empty_strided(P.size(), P.stride(), device=P.device, dtype=torch.float32)
             gemm_nt(dH, vp.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False)
             dS = torch.empty_strided(P.size(), P.stride(), device=P.device, dtype=torch.float32)
             ld = P.stride(-2)
-            L.call("sx_softmax_bwd", dP.data_ptr(), ld, S.data_ptr(), ld, lse.data_ptr(), B * M * U1, U2,
-                   stat[2:].data_ptr(), clip, att_p, *_seed_args(att_seed), ld, dS.data_ptr(), L.SX_F32, ld, _rt(), _stream())
+            if table is not None:
+                dT = softmax_posbias_backward(dP, ld, S, ld, lse, B * M * U1, U2, stat[2:], clip, att_p, att_seed, ld, dS,
+                                              ld, table, pb_geom, ctx.needs_input_grad[13])
+            else:
+                L.call("sx_softmax_bwd", dP.data_ptr(), ld, S.data_ptr(), ld, lse.data_ptr(), B * M * U1, U2,
+                       stat[2:].data_ptr(), clip, att_p, *_seed_args(att_seed), ld, dS.data_ptr(), L.SX_F32, ld, _rt(), _stream())
             scale = 1.0 / math.sqrt(d)
             if ctx.needs_input_grad[0]:
                 bcast = Bq == 1 and B > 1
@@ -1081,11 +1183,18 @@ class _SqueezeOutFused(torch.autograd.Function):
                 dk = torch.empty_like(k)
                 gemm_nt(dS.transpose(-1, -2), q.view(Bq, U1, M, d).permute(0, 2, 3, 1),
                         out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False)
-        return dq, dk, dvp, None, None, None, None, dbm, None, None, dW, dbo, None
+        return dq, dk, dvp, None, None, None, None, dbm, None, None, dW, dbo, None, dT, None
 
 
-def squeeze_out_fused(q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag):
-    return _SqueezeOutFused.apply(q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag)
+def _pb_args(posbias):
+    if posbias is None:
+        return None, None
+    return _posbias_table(posbias), (posbias.R, posbias.grid, posbias.w)
+
+
+def squeeze_out_fused(q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag, posbias=None):
+    """posbias (PosBias): sliding-window positional bias inside the softmax; its table receives a gradient."""
+    return _SqueezeOutFused.apply(q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag, *_pb_args(posbias))
 
 
 class _LayerNorm(torch.autograd.Function):
@@ -1267,18 +1376,20 @@ class _PosCode(torch.autograd.Function):
 
 
 class _Prologue(torch.autograd.Function):
-    """h = mask * dropout(LN(LN_{g,b}(x) + posw * pe[:, :C]))   (segtran_shared.py:916, :930-934, :944-946)."""
+    """h = mask * dropout(LN(LN_{g,b}(x) + posw * pe[:, :C]))   (segtran_shared.py:916, :930-934, :944-946);
+    pe None (no positional code, :940): h = mask * dropout(LN_{g,b}(x))."""
 
     @staticmethod
     def forward(ctx, x, g, b, pe, posw, mask, drop_p, seed):
         x = x.contiguous()
         B, N, Cd = x.shape
-        pe = pe.contiguous()                       # [N, C0] shared by the batch, or [B, N, C0]
-        C0 = pe.shape[-1]
-        pe_bstride = 0 if pe.dim() == 2 else N * C0
+        if pe is not None:
+            pe = pe.contiguous()                   # [N, C0] shared by the batch, or [B, N, C0]
+        C0 = pe.shape[-1] if pe is not None else 0
+        pe_bstride = 0 if pe is None or pe.dim() == 2 else N * C0
         h = torch.empty_like(x)
         stats = torch.empty((B * N, 4), device=x.device, dtype=torch.float32)
-        L.call("sx_prologue_fwd", x.data_ptr(), B, N, Cd, g.data_ptr(), b.data_ptr(), pe.data_ptr(), C0, pe_bstride,
+        L.call("sx_prologue_fwd", x.data_ptr(), B, N, Cd, g.data_ptr(), b.data_ptr(), _ptr(pe), C0, pe_bstride,
                posw, _ptr(mask), drop_p, *_seed_args(seed), h.data_ptr(), L.SX_F32, _rt(), stats.data_ptr(), _stream())
         ctx.save_for_backward(x, g, b, pe, mask, stats)
         ctx.meta = (posw, drop_p, seed, pe_bstride)
@@ -1290,16 +1401,18 @@ class _Prologue(torch.autograd.Function):
         x, g, b, pe, mask, stats = ctx.saved_tensors
         posw, drop_p, seed, pe_bstride = ctx.meta
         B, N, Cd = x.shape
-        C0 = pe.shape[-1]
+        C0 = pe.shape[-1] if pe is not None else 0
         dh = dh.contiguous()
         dx = torch.empty_like(x)
         dgb, dg = _sink_or_zeros(ctx.leaves[0])
         dbb, db = _sink_or_zeros(ctx.leaves[1])
-        dpe = _zeros_like(pe) if ctx.needs_input_grad[3] else None
-        scratch = torch.empty_like(x)
-        L.call("sx_prologue_bwd", dh.data_ptr(), x.data_ptr(), B, N, Cd, g.data_ptr(), b.data_ptr(), pe.data_ptr(), C0,
+        dpe = _zeros_like(pe) if pe is not None and ctx.needs_input_grad[3] else None
+        scratch = torch.empty_like(x) if pe is not None else None
+        L.call("sx_prologue_bwd", dh.data_ptr(), x.data_ptr(), B, N, Cd, g.data_ptr(), b.data_ptr(), _ptr(pe), C0,
                pe_bstride, posw, _ptr(mask), drop_p, *_seed_args(seed), stats.data_ptr(), dx.data_ptr(), dgb.data_ptr(), dbb.data_ptr(),
-               _ptr(dpe), scratch.data_ptr(), *_part_args(dh.device), _stream())
+               _ptr(dpe), _ptr(scratch), *_part_args(dh.device), _stream())
+        if pe is None:
+            L.launch_count -= 1             # without a code: row kernel + part_reduce, one fewer than _LAUNCHES counts
         return dx, dg, db, dpe, None, None, None, None
 
 
@@ -1351,6 +1464,14 @@ def attn_scores(q, k, M, amax=None, row_bias=None, tag="big"):
 def softmax(S, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None):
     """diag: optional device float[2] updated in place: [0] = max(diag[0], *amax), [1] += (*amax > clip)."""
     return _Softmax.apply(S, amax, clip, drop_p, seed, diag)
+
+
+def softmax_posbias(S, posbias, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None):
+    """softmax() with the sliding-window positional bias added after the clamp; S [B,M,N,N] with N = posbias.num_tokens."""
+    if S.shape[-1] != posbias.num_tokens or S.shape[-2] != posbias.num_tokens:
+        raise L.SxError("softmax_posbias: scores %s do not match the %s bias grid" % (tuple(S.shape), posbias.grid))
+    table, geom = _pb_args(posbias)
+    return _SoftmaxPosBias.apply(S, amax, clip, drop_p, seed, diag, table, geom)
 
 
 def attn_pv(P, v, M, tag="big", round_out=True):
