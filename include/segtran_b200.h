@@ -336,6 +336,26 @@ int sx_resize_axis_fwd(const float* x, int64_t outer, int32_t Lin, int32_t Lout,
                        int32_t accumulate, void* stream);
 int sx_resize_axis_bwd(const float* dy, int64_t outer, int32_t Lin, int32_t Lout, int64_t inner, float* dx,
                        void* stream);
+/* Token-grid resampling of the mince transformer (segtran_shared.py:45-66): linear / bilinear / trilinear interpolation
+ * (align_corners=False) of token-major rows on a row-major grid, all axes in one launch.  A 2-D grid passes a leading
+ * axis of extent 1 with ratio 1.  ratio[a]: source cells per output cell, as PyTorch computes it: 1/scale_factor when
+ * F.interpolate is given a scale factor, Lin/Lout when it is given a size; 1/ratio <= 24.
+ * Element (b, g, cell, c) of x / dx is at [b*bs_in + g*gs_in + cell*ld_in + c], of y / dy at
+ * [b*bs_out + g*gs_out + cell*ld_out + c]; c < w is the channel window (pass its first column as the pointer).
+ * fwd: y = resample(x) for c < w, columns [w, w_pad) of y are written as 0; round_tf32 rounds y for a GEMM consumer.
+ * bwd: the adjoint in gather form (every input cell sums, in a fixed order, the output cells that read it; no atomics):
+ *   dx = (dx +) resample^T(dy) for c < w; columns [w, w_pad) of dx are written as 0 unless accumulating. */
+typedef struct {
+  int32_t lin[3];
+  int32_t lout[3];
+  float ratio[3];
+} sx_resample_grid;
+int sx_resize_tokens_fwd(const float* x, int64_t bs_in, int64_t gs_in, int64_t ld_in, float* y, int64_t bs_out,
+                         int64_t gs_out, int64_t ld_out, int32_t B, int32_t G, int32_t w, int32_t w_pad,
+                         const sx_resample_grid* grid, int32_t round_tf32, void* stream);
+int sx_resize_tokens_bwd(const float* dy, int64_t bs_out, int64_t gs_out, int64_t ld_out, float* dx, int64_t bs_in,
+                         int64_t gs_in, int64_t ld_in, int32_t B, int32_t G, int32_t w, int32_t w_pad,
+                         const sx_resample_grid* grid, int32_t accumulate, void* stream);
 /* tiny strided fp32 GEMM on CUDA cores (class-dimension products of the collapsed head):
  *   C[z](m,n) (+)= alpha * sum_k A[z](m,k) B[z](k,n), element strides given explicitly */
 int sx_sgemm_small(const float* A, const float* B, float* C, int32_t M, int32_t N, int32_t K, int64_t sam, int64_t sak,

@@ -52,6 +52,10 @@ class sx_attn_probs_args(C.Structure):
                 ("_pad", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("posbias", sx_posbias)]
 
 
+class sx_resample_grid(C.Structure):
+    _fields_ = [("lin", C.c_int32 * 3), ("lout", C.c_int32 * 3), ("ratio", C.c_float * 3)]
+
+
 _P, _I, _L, _F, _U64, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64, C.c_double
 
 # name -> argtypes (every function returns int; 0 = success)
@@ -97,6 +101,8 @@ _PROTOS = {
     "sx_token_scores_bwd": [_P, _P, _I, _I, _I, _I, _P, _P],
     "sx_resize_axis_fwd": [_P, _L, _I, _I, _L, _P, _I, _P],
     "sx_resize_axis_bwd": [_P, _L, _I, _I, _L, _P, _P],
+    "sx_resize_tokens_fwd": [_P, _L, _L, _L, _P, _L, _L, _L, _I, _I, _I, _I, C.POINTER(sx_resample_grid), _I, _P],
+    "sx_resize_tokens_bwd": [_P, _L, _L, _L, _P, _L, _L, _L, _I, _I, _I, _I, C.POINTER(sx_resample_grid), _I, _P],
     "sx_groupnorm_fwd": [_P, _I, _I, _L, _I, _P, _P, _F, _P, _P, _P, _I, _P],
     "sx_groupnorm_bwd": [_P, _P, _I, _I, _L, _I, _P, _P, _P, _P, _P, _P, _P, _P],
     "sx_seg_loss_fwd": [_P, _P, _I, _I, _L, _P, _P, _F, _P, _P, _P, _P],

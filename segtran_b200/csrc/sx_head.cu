@@ -16,6 +16,7 @@
 #include <cstdlib>
 
 #include "sx_common.cuh"
+#include "sx_resample.cuh"
 
 namespace {
 
@@ -134,14 +135,7 @@ head_contract_bwd_weight_kernel(const float* __restrict__ dL, const float* __res
 }
 
 // ---- 1-D linear resize along one axis of x viewed as [outer, Lin, inner] -> [outer, Lout, inner] ----
-__device__ __forceinline__ void src_index(int j, float scale, int Lin, int& i0, int& i1, float& w1) {
-  float s = ((float)j + 0.5f) * scale - 0.5f;       // area_pixel_compute_source_index, align_corners=False
-  if (s < 0.f) s = 0.f;
-  i0 = (int)s;
-  if (i0 > Lin - 1) i0 = Lin - 1;
-  i1 = i0 + ((i0 < Lin - 1) ? 1 : 0);
-  w1 = s - (float)i0;
-}
+// (ratio Lin/Lout: F.interpolate with a target size; sx::src_index is in sx_resample.cuh)
 
 template <typename I>
 __global__ void resize_axis_fwd_kernel(const float* __restrict__ x, long long outer_, int Lin, int Lout, long long inner_,
@@ -156,7 +150,7 @@ __global__ void resize_axis_fwd_kernel(const float* __restrict__ x, long long ou
     const I o = t / (I)Lout;
     int i0, i1;
     float w1;
-    src_index(j, scale, Lin, i0, i1, w1);
+    sx::src_index(j, scale, Lin, i0, i1, w1);
     const float* base = x + o * Lin * inner + in;
     const float v = (1.f - w1) * base[(long long)i0 * inner] + w1 * base[(long long)i1 * inner];
     y[idx] = accumulate ? y[idx] + v : v;
@@ -187,7 +181,7 @@ __global__ void resize_axis_bwd_kernel(const float* __restrict__ dy, long long o
     for (int j = jlo; j <= jhi; ++j) {
       int i0, i1;
       float w1;
-      src_index(j, scale, Lin, i0, i1, w1);
+      sx::src_index(j, scale, Lin, i0, i1, w1);
       float w = 0.f;
       if (i0 == i) w += 1.f - w1;
       if (i1 == i) w += w1;
@@ -208,7 +202,7 @@ __global__ void resize_axis_fwd_v4_kernel(const float4* __restrict__ x, unsigned
     const unsigned o = t / (unsigned)Lout;
     int i0, i1;
     float w1;
-    src_index(j, scale, Lin, i0, i1, w1);
+    sx::src_index(j, scale, Lin, i0, i1, w1);
     const float4* base = x + (size_t)o * Lin * inner4 + in;
     const float4 a = __ldg(base + (size_t)i0 * inner4), b = __ldg(base + (size_t)i1 * inner4);
     const float w0 = 1.f - w1;
@@ -237,7 +231,7 @@ __global__ void resize_axis_bwd_v4_kernel(const float4* __restrict__ dy, unsigne
     for (int j = jlo; j <= jhi; ++j) {
       int i0, i1;
       float w1;
-      src_index(j, scale, Lin, i0, i1, w1);
+      sx::src_index(j, scale, Lin, i0, i1, w1);
       float w = 0.f;
       if (i0 == i) w += 1.f - w1;
       if (i1 == i) w += w1;
@@ -264,7 +258,7 @@ __global__ void resize_last_fwd_kernel(const float* __restrict__ x, unsigned row
     for (int u = 0; u < 4; ++u) {
       int i0, i1;
       float w1;
-      src_index(j0 + u, scale, Lin, i0, i1, w1);
+      sx::src_index(j0 + u, scale, Lin, i0, i1, w1);
       o[u] = (1.f - w1) * __ldg(base + i0) + w1 * __ldg(base + i1);
     }
     float4* dst = reinterpret_cast<float4*>(y + (size_t)r * Lout + j0);
@@ -296,7 +290,7 @@ __global__ void resize_last_bwd_kernel(const float* __restrict__ dy, unsigned ro
       for (int j = jlo; j <= jhi; ++j) {
         int i0, i1;
         float w1;
-        src_index(j, scale, Lin, i0, i1, w1);
+        sx::src_index(j, scale, Lin, i0, i1, w1);
         float w = 0.f;
         if (i0 == i) w += 1.f - w1;
         if (i1 == i) w += w1;

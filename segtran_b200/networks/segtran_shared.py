@@ -9,8 +9,9 @@ checkpoints load with ``load_state_dict``), while every forward runs on the sm_9
 Supported configuration = the one the reference's drivers force (train3d.py:174-178, train2d.py:245-249):
 squeezed attention (or plain cross attention), pos_code_type 'lsinu', mid_type 'shared',
 trans_output_type 'private'|'shared', tie_qk 'shared'|'loose'|'none', pool_modes_feat 'softmax', plus
---nosqueeze and --squeezeuseffn, and the positional-code ablations --pos bias (sliding-window biases inside the
-attention softmax, plain attention only) and --pos none.  The other ablation-only switches (mince, multihead, rand/sinu
+--nosqueeze and --squeezeuseffn, the positional-code ablations --pos bias (sliding-window biases inside the
+attention softmax, plain attention only) and --pos none, and the mince transformer (--mince with --nosqueeze: plain
+attention on several downsampled copies of the token grid).  The other ablation-only switches (multihead, rand/sinu
 position codes) raise NotImplementedError.
 """
 from __future__ import annotations
@@ -39,6 +40,51 @@ def gen_all_indices(shape, device):
     """Coordinates of every cell of a grid, [*shape, len(shape)] (reference segtran_shared.py:28-36)."""
     axes = [torch.arange(int(s), device=device) for s in shape]
     return torch.stack(torch.meshgrid(*axes, indexing='ij'), dim=len(axes))
+
+
+def multi_resize_shape(shape, scales):
+    """The token grid of every mince scale: int(g / scale) cells per axis (reference segtran_shared.py:38-43)."""
+    return [torch.Size([int(g / scale) for g in shape]) for scale in scales]
+
+
+def mince_grids(shape, scales):
+    """multi_resize_shape, checked against what F.interpolate(scale_factor=1/scale) produces (floor(g * (1/scale)) cells,
+    which the reference's reshapes rely on): a scale that empties an axis or where the two disagree raises ValueError."""
+    grid = tuple(int(g) for g in shape)
+    if len(grid) not in (2, 3):
+        raise ValueError("mince transformer: a 2-D or 3-D token grid is needed (got %s)" % (grid,))
+    out = []
+    for scale, shp in zip(scales, multi_resize_shape(grid, scales)):
+        for g, n in zip(grid, shp):
+            if n < 1:
+                raise ValueError("mince transformer: scale %s leaves an empty axis of the grid %s" % (scale, grid))
+            if n != math.floor(g * (1.0 / scale)):
+                raise ValueError("mince transformer: scale %s gives int(%d / %s) = %d cells but F.interpolate makes %d"
+                                 % (scale, g, scale, n, math.floor(g * (1.0 / scale))))
+        out.append(tuple(int(n) for n in shp))
+    return out
+
+
+def fracs_to_indices(feat_dim, mince_channel_props):
+    """Channel boundaries of the mince scales (reference segtran_shared.py:68-87): the proportions (fractions or
+    unnormalised weights) are normalised; scale i < last gets int(frac_i * feat_dim) channels, the last one the rest.
+    -> (boundaries [S+1], widths [S])."""
+    fracs = np.array(mince_channel_props, dtype=float)
+    fracs /= fracs.sum()
+    n = len(fracs)
+    idx = [0] * (n + 1)
+    for i in range(n - 1):
+        idx[i + 1] = idx[i] + int(fracs[i] * feat_dim)
+    idx[-1] = feat_dim
+    return idx, [idx[i + 1] - idx[i] for i in range(n)]
+
+
+def _check_mince_config(config):
+    if config.mince_scales is None or config.mince_channel_props is None:
+        raise ValueError("mince transformer: mince_scales and mince_channel_props must be given")
+    if len(config.mince_channel_props) != len(config.mince_scales):
+        raise ValueError("mince transformer: %d scales but %d channel proportions"
+                         % (len(config.mince_scales), len(config.mince_channel_props)))
 
 
 
@@ -107,6 +153,13 @@ class SegtranConfig:
             print("'%s' orig in-feat: %d, in-feat: %d, out-feat: %d, in-scheme: %s, out-scheme: %s, translayer_dims: %s"
                   % (config_name, self.orig_in_feat_dim, self.trans_in_dim, self.trans_out_dim, self.in_fpn_scheme,
                      self.out_fpn_scheme, self.translayer_dims))
+
+
+def _prod(shape):
+    n = 1
+    for g in shape:
+        n *= int(g)
+    return n
 
 
 def _unsupported(what):
@@ -202,8 +255,15 @@ class ExpandedFeatTrans(nn.Module):
         if self.has_input_skip:
             _unsupported("has_input_skip")
         if config.use_mince_transformer and config.mince_scales is not None:
-            _unsupported("the mince transformer")
-        self.num_scales = 0
+            # (:344-354) P.V per scale on the channel windows of --minceprops, upsampled and concatenated
+            _check_mince_config(config)
+            self.mince_scales = list(config.mince_scales)
+            self.num_scales = len(self.mince_scales)
+            self.mince_channel_props = config.mince_channel_props
+            self.mince_channel_indices, _ = fracs_to_indices(self.feat_dim, self.mince_channel_props)
+        else:
+            self.num_scales = 0
+            self.mince_scales = None
         self.first_linear = nn.Linear(self.in_feat_dim, self.feat_dim_allmode, bias=config.v_has_bias)
         self.first_norm_layer = nn.LayerNorm(self.feat_dim, eps=1e-12, elementwise_affine=True)
         self.base_initializer_range = config.base_initializer_range
@@ -271,9 +331,38 @@ class ExpandedFeatTrans(nn.Module):
                                   diag, posbias)
         return self._norm_aggregate(y)
 
+    def _mince_fuse(self, input_feat, probs, grid):
+        """(:413-443) U [B,M,N,F]: V = first_linear(x) in full; per scale s its channel window [Lv_s, Rv_s) of every mode
+        is downsampled onto the scale's grid (zero-padded to a multiple of 4 columns), multiplied by P_s and upsampled
+        back into its window of U."""
+        M, Fd = self.num_modes, self.feat_dim
+        grids = mince_grids(grid, self.mince_scales)
+        if len(probs) != self.num_scales:
+            raise ValueError("ExpandedFeatTrans: %d attention probabilities for %d mince scales" % (len(probs), self.num_scales))
+        idx = self.mince_channel_indices
+        wins = [(idx[s], idx[s + 1]) for s in range(self.num_scales)]
+        if any(b <= a for a, b in wins):
+            raise ValueError("ExpandedFeatTrans: an empty mince channel window %s of %d channels" % (wins, Fd))
+        v = ops.linear(input_feat, self.first_linear.weight, self.first_linear.bias, round_out=False)    # [B,N,M*F]
+        ratios = [(ops.down_ratio(sc),) * len(grid) for sc in self.mince_scales]
+        vs = ops.resize_tokens(v, M, grid, grids, ratios, wins)                  # [B,N_s,M*pad4(w_s)] each
+        us = [ops.attn_pv(p, vv, M, round_out=False) for p, vv in zip(probs, vs)]     # [B,M,N_s,pad4(w_s)]
+        return ops.resize_tokens_into(us, grid, grids, wins, Fd)                 # [B,M,N,F]
+
     def forward(self, input_feat, attention_probs, in_geoshape=None):
-        """input_feat [B,U2,C]; attention_probs [B,M,U1,U2] -> [B,U1,F]."""
+        """input_feat [B,U2,C]; attention_probs [B,M,U1,U2] -> [B,U1,F].  With mince scales: attention_probs is the list
+        of per-scale probabilities and in_geoshape the token grid."""
         M = self.num_modes
+        if self.num_scales > 0:
+            if in_geoshape is None:
+                raise ValueError("ExpandedFeatTrans: the mince transformer needs the token grid (in_geoshape)")
+            u = self._mince_fuse(input_feat, attention_probs, tuple(int(g) for g in in_geoshape))
+            if not self.has_FFN:
+                z = u[:, 0] if M == 1 else self.feat_softaggr(u)
+                return ops.layer_norm(z, self.first_norm_layer.weight, self.first_norm_layer.bias)
+            # the channel windows sit between P.V and the mid Linear: the unfolded branch below
+            g = self.intermediate(u)
+            return self._norm_aggregate(self.output(g, u))
         folded = self.supports_fused_attention()
         if not folded:
             v = ops.linear(input_feat, self.first_linear.weight, self.first_linear.bias)     # [B,U2,M*F]
@@ -431,9 +520,133 @@ class CrossAttFeatTrans(nn.Module):
 
 
 class CrossMinceAttFeatTrans(nn.Module):
+    """Mince attention (reference :612-785): per scale s, the Q/K channel window [L_s, R_s) of every mode (the modes'
+    d = in_feat_dim / M channels split equally between the scales) is downsampled onto the scale's grid (scale_factor
+    1/scale_s), S_s = Q_s K_s^T / sqrt(d) with the FULL d, conditionally clamped on this scale's own maximum, plus
+    pos_code_weight * the scale's positional biases, softmax and attention dropout; then ExpandedFeatTrans combines the
+    scales (:404-447).  Not a CrossAttFeatTrans: SegtranInitWeights leaves query and key untied and gives the key no
+    identity bias."""
+
     def __init__(self, config, name):
         super().__init__()
-        _unsupported("the mince transformer")
+        self.config, self.name = config, name
+        self.num_modes, self.in_feat_dim, self.feat_dim = config.num_modes, config.in_feat_dim, config.feat_dim
+        self.attention_mode_dim = self.in_feat_dim // self.num_modes
+        self.att_size_allmode = self.num_modes * self.attention_mode_dim
+        self.query = nn.Linear(self.in_feat_dim, self.att_size_allmode, bias=config.qk_have_bias)
+        self.key = nn.Linear(self.in_feat_dim, self.att_size_allmode, bias=config.qk_have_bias)
+        if not config.use_mince_transformer:
+            raise ValueError("CrossMinceAttFeatTrans needs use_mince_transformer")
+        _check_mince_config(config)
+        self.mince_scales = list(config.mince_scales)
+        self.num_scales = len(self.mince_scales)
+        self.mince_qk_channel_indices, _ = fracs_to_indices(self.attention_mode_dim, [1] * self.num_scales)
+        if any(self.mince_qk_channel_indices[s + 1] <= self.mince_qk_channel_indices[s] for s in range(self.num_scales)):
+            raise ValueError("CrossMinceAttFeatTrans: %d channels per mode cannot be split between %d scales"
+                             % (self.attention_mode_dim, self.num_scales))
+        self.base_initializer_range = config.base_initializer_range
+        self.pos_code_weight = config.pos_code_weight if config.pos_code_type == 'bias' else 1
+        if config.ablate_multihead:
+            _unsupported("ablate_multihead")
+        if config.use_attn_consist_loss:
+            raise NotImplementedError("segtran_b200: --attnconsist with --mince is not implemented (the reference "
+                                      "crashes on the per-scale list of attention scores)")
+        self.out_trans = ExpandedFeatTrans(config, name)
+        self.att_dropout = nn.Dropout(config.attention_probs_dropout_prob)
+        self.keep_attn_scores = False
+        self.tie_qk_scheme = config.tie_qk_scheme
+        self.attn_clip = config.attn_clip
+        self.attn_diag_cycles = config.__dict__.get('attn_diag_cycles', 500)
+        self.call_count = 0
+        self.attention_scores = None
+        self._diag = None            # per scale, device [3]: running max of the scores, clamped calls, ambiguous rows
+
+    tie_qk = CrossAttFeatTrans.tie_qk
+    add_identity_bias = CrossAttFeatTrans.add_identity_bias
+
+    # ---- per-scale diagnostics, synchronised lazily (the reference does .item() syncs per scale, :738-755) ----
+    def _diag_lists(self):
+        if self._diag is None:
+            return [0.0] * self.num_scales, [0] * self.num_scales, [0] * self.num_scales
+        vals = [d.tolist() for d in self._diag]
+        return [max(v[0], 0.0) for v in vals], [int(v[1]) for v in vals], [int(v[2]) for v in vals]
+
+    @property
+    def max_attn(self):
+        return self._diag_lists()[0]
+
+    @property
+    def clamp_count(self):
+        return self._diag_lists()[1]
+
+    @property
+    def lower_clamp_ambiguous_rows(self):
+        """Rows where the reference's lower clamp could have changed the result, summed over the scales (expected 0)."""
+        return sum(self._diag_lists()[2])
+
+    def forward(self, in_query, query_geoshape, in_key=None, key_geoshape=None, pos_biases=None):
+        """in_query [B,N,C] on the token grid query_geoshape; pos_biases: None or one ops.PosBias (or None) per scale, each
+        over that scale's grid."""
+        if in_key is None:
+            in_key, key_geoshape = in_query, query_geoshape
+        grid = tuple(int(g) for g in query_geoshape)
+        if key_geoshape is None or tuple(int(g) for g in key_geoshape) != grid:
+            raise ValueError("CrossMinceAttFeatTrans: query and key grids must agree (got %s and %s)"
+                             % (grid, None if key_geoshape is None else tuple(key_geoshape)))
+        grids = mince_grids(grid, self.mince_scales)
+        N = _prod(grid)
+        if in_query.shape[1] != N or in_key.shape[1] != N:
+            raise ValueError("CrossMinceAttFeatTrans: %d / %d tokens on a grid of %d cells"
+                             % (in_query.shape[1], in_key.shape[1], N))
+        pbs = [None] * self.num_scales
+        if pos_biases is not None:
+            if len(pos_biases) != self.num_scales:
+                raise ValueError("CrossMinceAttFeatTrans: %d positional biases for %d scales"
+                                 % (len(pos_biases), self.num_scales))
+            for s, pb in enumerate(pos_biases):
+                if pb is None:
+                    continue
+                if not isinstance(pb, ops.PosBias):
+                    raise TypeError("CrossMinceAttFeatTrans: pos_biases entries must be ops.PosBias or None")
+                if pb.grid != grids[s]:
+                    raise ValueError("CrossMinceAttFeatTrans: positional biases over %s at scale %s, whose grid is %s"
+                                     % (pb.grid, self.mince_scales[s], grids[s]))
+                pbs[s] = pb.with_weight(float(self.pos_code_weight))
+        M, d = self.num_modes, self.attention_mode_dim
+        q = ops.linear(in_query, self.query.weight, self.query.bias, tag="proj", round_out=False)
+        k = ops.linear(in_key, self.key.weight, self.key.bias, tag="proj", round_out=False)
+        idx = self.mince_qk_channel_indices
+        wins = [(idx[s], idx[s + 1]) for s in range(self.num_scales)]
+        ratios = [(ops.down_ratio(sc),) * len(grid) for sc in self.mince_scales]
+        qs = ops.resize_tokens(q, M, grid, grids, ratios, wins)        # [B,N_s,M*pad4(w_s)], TF32-rounded
+        ks = ops.resize_tokens(k, M, grid, grids, ratios, wins)
+        dev = q.device
+        if self._diag is None or self._diag[0].device != dev:
+            self._diag = [torch.tensor([-3.0e38, 0.0, 0.0], device=dev) for _ in range(self.num_scales)]
+        p = self.att_dropout.p if self.training else 0.0
+        alpha = 1.0 / math.sqrt(d)                                     # (:736) the full per-mode width
+        self.call_count += 1
+        diag_call = self.training and self.call_count % self.attn_diag_cycles == 0     # prints avg-attn: needs S
+        fused = ops.attn_fusion_enabled() and not diag_call and q.is_cuda
+        probs = []
+        for s in range(self.num_scales):
+            seed = ops.new_dropout_seed(dev) if p > 0 else 0
+            if fused:
+                probs.append(ops.attn_probs(qs[s], ks[s], M, alpha, float(self.attn_clip), p, seed, self._diag[s], pbs[s]))
+                continue
+            amax = torch.full((1,), -3.0e38, device=dev)
+            sc = ops.attn_scores(qs[s], ks[s], M, amax, alpha=alpha)   # [B,M,N_s,N_s], max tracked on device
+            if pbs[s] is not None:
+                probs.append(ops.softmax_posbias(sc, pbs[s], amax, float(self.attn_clip), p, seed, self._diag[s]))
+            else:
+                probs.append(ops.softmax(sc, amax, float(self.attn_clip), p, seed, self._diag[s]))
+            if diag_call:
+                with torch.no_grad():
+                    avg = float(sc.sum() / (sc > 0).sum().clamp_min(1))
+                mx, cc, _ = self._diag_lists()
+                print("{} attn max: {:.2f}, avg: {:.2f}, clamp-count: {}".format(self.mince_scales[s], mx[s], avg, cc[s]))
+                self._diag[s] = torch.tensor([-3.0e38, 0.0, 0.0], device=dev)
+        return self.out_trans(in_key, probs, grid)
 
 
 class SqueezedAttFeatTrans(nn.Module):
@@ -650,8 +863,10 @@ class SegtranFusionEncoder(nn.Module):
         self.dropout = nn.Dropout(config.hidden_dropout_prob)
         self.use_squeezed_transformer = config.use_squeezed_transformer
         self.use_mince_transformer = config.use_mince_transformer
-        if self.use_mince_transformer:
-            _unsupported("the mince transformer")
+        if self.use_squeezed_transformer and self.use_mince_transformer:
+            print("Squeezed transformer cannot be used with Mince transformer.")
+            print("Please specify '--nosqueeze' to disable squeezed transformer.")
+            exit(0)
         if self.use_squeezed_transformer and self.pos_code_type == 'bias':
             print("Squeezed transformer cannot use Positional Biases.")
             print("Please specify '--nosqueeze' to disable squeezed transformer.")
@@ -661,9 +876,24 @@ class SegtranFusionEncoder(nn.Module):
                                       "scores this build keeps do not include the positional biases)")
         # with sliding-window biases the code is not added to the features (:847-850)
         self.pos_code_weight = config.pos_code_weight if self.pos_code_type != 'bias' else 0
-        self.num_scales = 0
-        self.pos_code_layer = SegtranPosEncoder(config)
-        layer_cls = SqueezedAttFeatTrans if self.use_squeezed_transformer else CrossAttFeatTrans
+        if self.use_mince_transformer:
+            _check_mince_config(config)
+            if config.use_attn_consist_loss:
+                raise NotImplementedError("segtran_b200: --attnconsist with --mince is not implemented (the reference "
+                                          "crashes on the per-scale list of attention scores)")
+            self.num_scales = len(config.mince_scales)
+            self.mince_scales = list(config.mince_scales)
+        else:
+            self.num_scales = 0
+        if self.num_scales > 0 and self.pos_code_type in ('bias', 'none'):
+            # (:852-861) one positional encoder per scale, each over that scale's grid
+            self.pos_code_layers = nn.ModuleList([SegtranPosEncoder(config) for _ in range(self.num_scales)])
+        else:
+            self.pos_code_layer = SegtranPosEncoder(config)
+        if self.use_squeezed_transformer:
+            layer_cls = SqueezedAttFeatTrans
+        else:
+            layer_cls = CrossMinceAttFeatTrans if self.use_mince_transformer else CrossAttFeatTrans
         layers = []
         for i in range(self.num_translayers):
             cfg_i = copy.copy(config)
@@ -692,8 +922,13 @@ class SegtranFusionEncoder(nn.Module):
         x = vfeat if vfeat.dtype == torch.float32 else vfeat.float()
         if self.training and x.is_cuda:
             ops.advance_seed(x.device)           # one new dropout stream per training step (device side, graph safe)
+        per_scale = self.num_scales > 0 and self.pos_code_type in ('bias', 'none')
         for i, layer in enumerate(self.translayers):
-            pe = self.pos_code_layer(orig_feat_shape, voxels_pos)
+            if per_scale:
+                grids = mince_grids(orig_feat_shape, self.mince_scales)
+                pe = [self.pos_code_layers[s](grids[s], voxels_pos) for s in range(self.num_scales)]
+            else:
+                pe = self.pos_code_layer(orig_feat_shape, voxels_pos)
             ln = self.vfeat_norm_layers[i]
             p = self.dropout.p if (self.training and i == 0) else 0.0
             # 'bias' / 'none': no code on the features and no comb_norm_layers LayerNorm (:929-940); the biases (shared
@@ -702,7 +937,10 @@ class SegtranFusionEncoder(nn.Module):
             h = ops.prologue(x, ln.weight, ln.bias, feat_pe, float(self.pos_code_weight), mask, p,
                              ops.new_dropout_seed(x.device) if p > 0 else 0)
             ops.grad_ready(h, layer.parameters())                   # backward past `h`: this layer's weights are final
-            x = layer(h, pos_biases=pe if self.pos_code_type == 'bias' else None)
+            if self.num_scales > 0:
+                x = layer(h, orig_feat_shape, pos_biases=pe if self.pos_code_type == 'bias' else None)
+            else:
+                x = layer(h, pos_biases=pe if self.pos_code_type == 'bias' else None)
             self.layers_vfeat.append(x)
             if self.use_attn_consist_loss:
                 if self.use_squeezed_transformer:

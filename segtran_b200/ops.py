@@ -10,6 +10,7 @@ import ctypes as C
 import math
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -607,11 +608,11 @@ class _AttnScores(torch.autograd.Function):
     SqueezedAttFeatTrans): it is added after the scaling, so it must already be scaled."""
 
     @staticmethod
-    def forward(ctx, q, k, M, amax, row_bias, tag):
+    def forward(ctx, q, k, M, amax, row_bias, tag, alpha=None):
         Bq, U1, Cq = q.shape
         B, U2 = k.shape[0], k.shape[1]
         d = Cq // M
-        scale = 1.0 / math.sqrt(d)
+        scale = 1.0 / math.sqrt(d) if alpha is None else float(alpha)
         qv = q.view(Bq, U1, M, d).permute(0, 2, 1, 3)         # [Bq,M,U1,d] strided view, d contiguous
         kv = k.view(B, U2, M, d).permute(0, 2, 1, 3)
         S = _rowpad_empty((B, M, U1, U2), q.device)
@@ -631,22 +632,32 @@ class _AttnScores(torch.autograd.Function):
         Bq, U1, Cq = q.shape
         B, U2 = k.shape[0], k.shape[1]
         dS = _rowpad(dS)
-        dq = dk = drb = None
-        if ctx.needs_input_grad[0]:
-            # dQ[b,m] (U1 x d) = scale * dS[b,m] (U1 x U2) . K[b,m] (U2 x d)
-            bcast = Bq == 1 and B > 1
-            dq = _zeros_like(q) if bcast else torch.empty_like(q)
-            gemm_nt(dS, k.view(B, U2, M, d).permute(0, 2, 3, 1), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3),
-                    alpha=scale, round_out=False, reduce_z1=bcast, split_k=1, tag=ctx.tag)
-        if ctx.needs_input_grad[1]:
-            dk = torch.empty_like(k)
-            gemm_nt(dS.transpose(-1, -2), q.view(Bq, U1, M, d).permute(0, 2, 3, 1),
-                    out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, tag=ctx.tag)
+        dq, dk = _score_grads(dS, q, k, M, scale, ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.tag)
+        drb = None
         if rb_shape is not None and ctx.needs_input_grad[4]:
             drb = _zeros((U1,), q.device)     # sum over batch and keys
             L.call("sx_rowsum", dS.data_ptr(), B * U1, U2, dS.stride(-2), U1, drb.data_ptr(), *_part_args(dS.device), _stream())
             drb = drb.view(rb_shape)
-        return dq, dk, None, None, drb, None
+        return dq, dk, None, None, drb, None, None
+
+
+def _score_grads(dS, q, k, M, scale, need_q, need_k, tag="big"):
+    """Gradients of S = scale * Q K^T per mode: dQ = scale dS K, dK = scale dS^T Q (q may have batch 1: broadcast)."""
+    Bq, U1, Cq = q.shape
+    B, U2 = k.shape[0], k.shape[1]
+    d = Cq // M
+    dq = dk = None
+    if need_q:
+        # dQ[b,m] (U1 x d) = scale * dS[b,m] (U1 x U2) . K[b,m] (U2 x d)
+        bcast = Bq == 1 and B > 1
+        dq = _zeros_like(q) if bcast else torch.empty_like(q)
+        gemm_nt(dS, k.view(B, U2, M, d).permute(0, 2, 3, 1), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3),
+                alpha=scale, round_out=False, reduce_z1=bcast, split_k=1, tag=tag)
+    if need_k:
+        dk = torch.empty_like(k)
+        gemm_nt(dS.transpose(-1, -2), q.view(Bq, U1, M, d).permute(0, 2, 3, 1),
+                out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, tag=tag)
+    return dq, dk
 
 
 class PosBias:
@@ -691,12 +702,15 @@ def _posbias_table(pb):
     return t
 
 
-def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_scores=False, round_out=True, posbias=None):
+def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_scores=False, round_out=True, posbias=None,
+                     alpha=None):
     """P = dropout(softmax(min(Q K^T / sqrt(d), clip))) per mode in ONE wgmma kernel (csrc/sx_attn.cu): the scores stay
     in registers and the softmax runs on the accumulator fragments (reference segtran_shared.py:566-567, :569-580, :601, :605).
     q [Bq,U1,M*d] (Bq = 1 broadcasts), k [B,U2,M*d], both contiguous fp32 (TF32-rounded by their producers).
     posbias (PosBias, self-attention only): adds the sliding-window bias inside the softmax, after the clamp; S, rowmax
     and the clamp statistics stay on the raw scores (its table gradient comes from softmax_posbias_backward).
+    alpha: the score scale (default 1/sqrt(d) of the per-mode width; the mince transformer scales zero-padded channel
+    windows by the full width).
     -> (P [B,M,U1,U2] view of a row-padded buffer, S or None (raw scaled scores, same layout), lse [B,M,U1],
         rowmax [B,M,U1], stat [2])."""
     _req_cuda(q, k)
@@ -717,7 +731,7 @@ def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_sc
     a.round_tf32 = 1 if (round_out and _PRECISION == "tf32") else 0
     a.Q, a.q_ld, a.q_bstride = q.data_ptr(), Cq, (0 if Bq == 1 else U1 * Cq)
     a.K, a.k_ld, a.k_bstride = k.data_ptr(), Ck, U2 * Ck
-    a.alpha, a.clip = 1.0 / math.sqrt(d), float(clip)
+    a.alpha, a.clip = (1.0 / math.sqrt(d) if alpha is None else float(alpha)), float(clip)
     a.P, a.S, a.ldp = P.data_ptr(), _ptr(S), P.stride(-2)
     a.lse, a.rowmax, a.stat, a.diag = lse.data_ptr(), rowmax.data_ptr(), stat.data_ptr(), _ptr(diag)
     a.drop_p = drop_p
@@ -1457,8 +1471,9 @@ def dot(x, w):
     return _Dot.apply(x, w.contiguous())
 
 
-def attn_scores(q, k, M, amax=None, row_bias=None, tag="big"):
-    return _AttnScores.apply(q, k, M, amax, row_bias, tag)
+def attn_scores(q, k, M, amax=None, row_bias=None, tag="big", alpha=None):
+    """alpha: score scale (default 1/sqrt(d) of the per-mode width)."""
+    return _AttnScores.apply(q, k, M, amax, row_bias, tag, alpha)
 
 
 def softmax(S, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None):
@@ -1573,6 +1588,194 @@ class _Resize(torch.autograd.Function):
 
 def resize_linear(x, size):
     return _Resize.apply(x, tuple(int(s) for s in size))
+
+
+# ------------------------------------------------------------------------------------------------
+# token-grid resampling (mince transformer, segtran_shared.py:45-66): csrc/sx_resample.cu
+# ------------------------------------------------------------------------------------------------
+def _f32(v) -> float:
+    return float(np.float32(v))
+
+
+def down_ratio(scale) -> float:
+    """Source cells per output cell of F.interpolate(scale_factor=1/scale): 1/scale_factor, rounded to fp32 as PyTorch's
+    kernels do (so a 7-cell axis at scale 2 becomes 3 cells read at stride 2.0)."""
+    return _f32(1.0 / (1.0 / float(scale)))
+
+
+def size_ratio(lin, lout) -> float:
+    """Source cells per output cell of F.interpolate(size=...): Lin/Lout in fp32."""
+    return float(np.float32(lin) / np.float32(lout))
+
+
+def _resample_grid(lin, lout, ratios) -> L.sx_resample_grid:
+    if len(lin) not in (1, 2, 3) or len(lout) != len(lin) or len(ratios) != len(lin):
+        raise L.SxError("resize_tokens: 1-D to 3-D grids expected (got %s -> %s)" % (tuple(lin), tuple(lout)))
+    pad = 3 - len(lin)
+    g = L.sx_resample_grid()
+    for a in range(3):
+        u = a - pad
+        g.lin[a], g.lout[a], g.ratio[a] = (int(lin[u]), int(lout[u]), float(ratios[u])) if u >= 0 else (1, 1, 1.0)
+    return g
+
+
+def _cells(grid) -> int:
+    n = 1
+    for v in grid:
+        n *= int(v)
+    return n
+
+
+def _tok_layout(t: torch.Tensor, G: int):
+    """(batch, group, row) strides of a contiguous token-major [B, N, G*D] tensor, and D."""
+    B, N, C = t.shape
+    return (N * C, C // G, C), C // G
+
+
+def _mode_layout(t: torch.Tensor):
+    """(batch, group, row) strides of a contiguous mode-major [B, G, N, W] tensor."""
+    B, G, N, W = t.shape
+    return (G * N * W, N * W, W)
+
+
+def _resize_fwd(x, xs, y, ys, B, G, w, w_pad, grid, rnd):
+    L.call("sx_resize_tokens_fwd", x, *xs, y, *ys, B, G, w, w_pad, C.byref(grid), rnd, _stream())
+
+
+def _resize_bwd(dy, ys, dx, xs, B, G, w, w_pad, grid, acc):
+    L.call("sx_resize_tokens_bwd", dy, *ys, dx, *xs, B, G, w, w_pad, C.byref(grid), acc, _stream())
+
+
+class _ResizeTokensDown(torch.autograd.Function):
+    """Per window s: y_s [B, N_s, G*w_pad_s] = resample of the channel window [c0_s, c1_s) of every group of the token-major
+    x [B, N, G*D] from `grid` to grids_out[s] (ratios[s]); columns [w_s, w_pad_s) of each group are zeros.
+    Backward: the windows of dx are written one by one (no zero-fill when they tile [0, D))."""
+
+    @staticmethod
+    def forward(ctx, x, G, grid, grids_out, ratios, windows, w_pads, round_out):
+        _req_cuda(x)
+        x = x.contiguous()
+        B = x.shape[0]
+        xs, D = _tok_layout(x, G)
+        outs = []
+        for g_out, r, (c0, c1), wp in zip(grids_out, ratios, windows, w_pads):
+            y = torch.empty((B, _cells(g_out), G * wp), device=x.device, dtype=torch.float32)
+            _resize_fwd(x.data_ptr() + 4 * c0, xs, y.data_ptr(), _tok_layout(y, G)[0], B, G, c1 - c0, wp,
+                        _resample_grid(grid, g_out, r), _rt() if round_out else 0)
+            outs.append(y)
+        ctx.meta = (x.shape, G, tuple(grid), [tuple(g) for g in grids_out], ratios, windows, w_pads)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *dys):
+        shape, G, grid, grids_out, ratios, windows, w_pads = ctx.meta
+        B, N, Cx = shape
+        D = Cx // G
+        tiled = sorted(windows)[0][0] == 0 and sorted(windows)[-1][1] == D and \
+            all(a[1] == b[0] for a, b in zip(sorted(windows), sorted(windows)[1:]))
+        dx = (torch.empty if tiled else torch.zeros)(shape, device=dys[0].device, dtype=torch.float32)
+        xs = (N * Cx, D, Cx)
+        for dy, g_out, r, (c0, c1), wp in zip(dys, grids_out, ratios, windows, w_pads):
+            dy = dy.contiguous()
+            _resize_bwd(dy.data_ptr(), _tok_layout(dy, G)[0], dx.data_ptr() + 4 * c0, xs, B, G, c1 - c0, c1 - c0,
+                        _resample_grid(grid, g_out, r), 0)
+        return dx, None, None, None, None, None, None, None
+
+
+def resize_tokens(x, G, grid, grids_out, ratios, windows, w_pads=None, round_out=True):
+    """Linear / bilinear / trilinear resampling (align_corners=False) of channel windows of token-major rows.
+    x [B, N, G*D] (N = cells of the row-major `grid`); windows [(c0, c1), ...] of each group's D channels; grids_out and
+    ratios (per axis, see down_ratio / size_ratio) per window.  -> tuple of [B, N_s, G*w_pad_s] (w_pad_s defaults to
+    c1-c0 rounded up to 4; padding columns are zero), TF32-rounded for a GEMM consumer unless round_out=False."""
+    if w_pads is None:      # 16-byte GEMM operand strides: 4 fp32 columns, 8 when the products run on bf16 copies
+        w_pads = [((c1 - c0 + 7) // 8 * 8) if _PRECISION == "bf16" else _pad4(c1 - c0) for c0, c1 in windows]
+    return _ResizeTokensDown.apply(x, int(G), tuple(int(v) for v in grid), [tuple(int(v) for v in g) for g in grids_out],
+                                   [tuple(float(r) for r in rs) for rs in ratios], [(int(a), int(b)) for a, b in windows],
+                                   [int(w) for w in w_pads], bool(round_out))
+
+
+class _ResizeTokensUpInto(torch.autograd.Function):
+    """U [B, G, N, F] with its channel window [c0_s, c1_s) = resample of us[s][..., :c1_s-c0_s] ([B, G, N_s, W_s],
+    mode-major) from grids_in[s] to `grid` (ratios[s]); the windows tile [0, F), so every element of U is written once.
+    Backward: each dus[s] reads its window of dU (padding columns [c1_s-c0_s, W_s) zero)."""
+
+    @staticmethod
+    def forward(ctx, grid, grids_in, ratios, windows, Fd, round_out, *us):
+        B, G = us[0].shape[0], us[0].shape[1]
+        N = _cells(grid)
+        U = torch.empty((B, G, N, Fd), device=us[0].device, dtype=torch.float32)
+        Us = _mode_layout(U)
+        for u, g_in, r, (c0, c1) in zip(us, grids_in, ratios, windows):
+            u = u.contiguous()
+            _resize_fwd(u.data_ptr(), _mode_layout(u), U.data_ptr() + 4 * c0, Us, B, G, c1 - c0, c1 - c0,
+                        _resample_grid(g_in, grid, r), _rt() if round_out else 0)
+        ctx.meta = (tuple(grid), grids_in, ratios, windows, [tuple(u.shape) for u in us])
+        return U
+
+    @staticmethod
+    def backward(ctx, dU):
+        grid, grids_in, ratios, windows, ushapes = ctx.meta
+        dU = dU.contiguous()
+        B, G = dU.shape[0], dU.shape[1]
+        dUs = _mode_layout(dU)
+        dus = []
+        for g_in, r, (c0, c1), ush in zip(grids_in, ratios, windows, ushapes):
+            du = torch.empty(ush, device=dU.device, dtype=torch.float32)
+            _resize_bwd(dU.data_ptr() + 4 * c0, dUs, du.data_ptr(), _mode_layout(du), B, G, c1 - c0, ush[-1],
+                        _resample_grid(g_in, grid, r), 0)
+            dus.append(du)
+        return (None, None, None, None, None, None) + tuple(dus)
+
+
+def resize_tokens_into(us, grid, grids_in, windows, Fd, round_out=True):
+    """Upsample each us[s] [B, G, N_s, W_s] (mode-major, e.g. P_s.V_s) to the full `grid` with F.interpolate(size=grid)
+    semantics, writing channel window windows[s] of ONE [B, G, N, Fd] tensor (the concatenation over the windows)."""
+    ratios = [tuple(size_ratio(a, b) for a, b in zip(g_in, grid)) for g_in in grids_in]
+    return _ResizeTokensUpInto.apply(tuple(int(v) for v in grid), [tuple(int(v) for v in g) for g in grids_in], ratios,
+                                     [(int(a), int(b)) for a, b in windows], int(Fd), bool(round_out), *us)
+
+
+class _AttnProbs(torch.autograd.Function):
+    """P = dropout(softmax(clamp_if(alpha Q K^T) [+ w bias])) per mode as one node over the fused kernel
+    (attn_probs_fused): backward = softmax backward on the saved raw scores (sx_softmax_bwd / softmax_posbias_backward,
+    with the table gradient) -> dQ, dK products."""
+
+    @staticmethod
+    def forward(ctx, q, k, M, alpha, clip, drop_p, seed, diag, table, pb_geom):
+        pb = PosBias(table, *pb_geom) if table is not None else None
+        need_bwd = any(ctx.needs_input_grad)
+        P, S, lse, _rowmax, stat = attn_probs_fused(q, k, M, clip, drop_p, seed, diag, need_scores=need_bwd, posbias=pb,
+                                                    alpha=alpha)
+        ctx.save_for_backward(q, k, S, lse, stat)
+        ctx.meta = (M, alpha, clip, drop_p, P.stride(-2), pb_geom)
+        ctx.seed = seed
+        ctx.leaf = table
+        return P
+
+    @staticmethod
+    def backward(ctx, dP):
+        q, k, S, lse, stat = ctx.saved_tensors
+        M, alpha, clip, drop_p, ldp, pb_geom = ctx.meta
+        table = ctx.leaf
+        B, _, U1, U2 = S.shape
+        dP = _rowpad(dP)
+        dS = _rowpad_empty(S.shape, S.device)
+        dT = None
+        if table is not None:
+            dT = softmax_posbias_backward(dP, dP.stride(-2), S, S.stride(-2), lse, B * M * U1, U2, stat[2:], clip, drop_p,
+                                          ctx.seed, ldp, dS, dS.stride(-2), table, pb_geom, ctx.needs_input_grad[8])
+        else:
+            L.call("sx_softmax_bwd", dP.data_ptr(), dP.stride(-2), S.data_ptr(), S.stride(-2), lse.data_ptr(), B * M * U1, U2,
+                   stat[2:].data_ptr(), clip, drop_p, *_seed_args(ctx.seed), ldp, dS.data_ptr(), L.SX_F32, dS.stride(-2),
+                   _rt(), _stream())
+        dq, dk = _score_grads(dS, q, k, M, alpha, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        return dq, dk, None, None, None, None, None, None, dT, None
+
+
+def attn_probs(q, k, M, alpha, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None):
+    """Differentiable fused attention probabilities (see _AttnProbs); q, k [B, U, M*d] contiguous, TF32-rounded."""
+    return _AttnProbs.apply(q.contiguous(), k.contiguous(), M, float(alpha), float(clip), drop_p, seed, diag,
+                            *_pb_args(posbias))
 
 
 def _sgemm(A, B, M, N, K, sa, sb, out=None, alpha=1.0, accumulate=False, Z=1, zs=(0, 0, 0)):
