@@ -159,6 +159,68 @@ typedef struct {
 } sx_attn_probs_args;
 int sx_attn_probs_fwd(const sx_attn_probs_args* args, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Attention-consistency loss of one layer (csrc/sx_consist.cu; train3d.py:426-449 and train2d.py:668-723), without
+ * the [B,N,N] affinity matrix X or the [B,N,N] class-consistency matrix ever reaching memory:
+ *   c_ij = min(max(sum_k F[b,k,i] F[b,k,j], 0), 1)           F [B][K][N] fp32 (the downsampled mask), K <= 16
+ *   SX_CONSIST_BCE    : loss = mean over B*N*N of BCEWithLogits(X, c)       (train3d.py)
+ *   SX_CONSIST_MARGIN : mu_b = mean of X_b; element (b,i,j) is inconsistent when (x < mu_b && c != 0) or
+ *                       (x > mu_b - 0.1 && c == 0); loss = sum |x - mu_b| over the inconsistent elements of all batches
+ *                       divided by their count (NaN when there are none, as in the reference)       (train2d.py)
+ * Pair input (X = Xo . Xi, squeezed layers): Xo [B][N][A] and Xt = Xi^T [B][N][A], both K-major (row pitch and batch
+ *   stride multiples of 4 floats), TF32 values; A may be the width of K-concatenated hi/lo operand splits
+ *   (sx_split_tf32_cat, roles 0 and 1), which makes the product 3-pass.  X is produced tile by tile by a persistent
+ *   wgmma kernel and consumed on the accumulator fragments.
+ * Dense input (Xo == NULL): X [B][N][N] with row pitch x_ld and batch stride x_bstride.
+ * mu (MARGIN only): device [B], the per-batch means of X, computed by the caller.
+ * R (optional): the unscaled residual sigmoid(x) - c (BCE) or sign(x - mu)*[inconsistent] (MARGIN), [B][N][ldr],
+ *   rounded to TF32 when round_r; the backward products dXo = R Xi^T and dXi = Xo^T R are sx_gemm calls.
+ * out (device float [2 + B], written): [0] the layer's loss, [1] d loss / d x per unit residual (1/(B N^2), or 1/count,
+ *   0 when count == 0), [2 + b] (MARGIN) the gradient through mu_b per element of batch b and unit residual,
+ *   -(sum of sign(x - mu_b) over the inconsistent elements of batch b) / N^2.
+ * cap (optional, device float[2]): cap[0] += out[0]; cap[1] = t > 1 ? 1/t : 1 with t = cap_scale * cap[0] — the
+ *   factor of train2d.py's `if loss > 1: loss /= loss.item()` after the last layer, without a host read.
+ * The per-CTA sums go through `part` and are added in a fixed order: two runs give the same bits.
+ * ------------------------------------------------------------------------------------------- */
+enum { SX_CONSIST_BCE = 0, SX_CONSIST_MARGIN = 1 };
+typedef struct {
+  int32_t B, N, A, K;
+  int32_t variant;
+  int32_t round_r;
+  const float* Xo;
+  int64_t xo_ld, xo_bstride;
+  const float* Xt;
+  int64_t xt_ld, xt_bstride;
+  const float* X;
+  int64_t x_ld, x_bstride;
+  const float* F;
+  const float* mu;
+  float* R;
+  int64_t ldr;
+  float* out;
+  float* cap;
+  float cap_scale;
+  int32_t _pad;
+  float* part;
+  int64_t part_floats;
+} sx_consist_args;
+int sx_attn_consist_fwd(const sx_consist_args* args, void* stream);
+/* Gradient of one layer's loss with respect to one input, from the raw backward product G (R Xi^T, Xo^T R, or R itself
+ * for a dense input), in place or out of place: for batch b, row r, column c of [B][rows][cols]
+ *   dst = s * (G + m_b * v),  s = (*gout) * out[1],  m_b = out[2 + b] (MARGIN; 0 for BCE),
+ *   v = vrow[b*rows + r] if vrow, else vcol[b*cols + c] if vcol, else 1
+ * (the rank-1 term of the gradient through mu: vrow / vcol are Xo's column sums / Xi's row sums per batch). */
+int sx_attn_consist_bwd(const sx_consist_args* args, const float* gout, const float* G, int32_t rows, int32_t cols,
+                        int64_t ldg, int64_t g_bstride, const float* vrow, const float* vcol, float* dst, int64_t ldd,
+                        int64_t d_bstride, void* stream);
+
+/* The attention scores a layer keeps for the loss above (segtran_shared.py:578-598): the reference keeps them after its
+ * conditional clamp.  S [R,L] (row pitch lds), amax = device max of S.
+ *   dY == NULL: out = (*amax > clip) ? clamp(S, -clip, clip) : S
+ *   otherwise : out = (*amax > clip && |S| > clip) ? 0 : dY       (the clamp's gradient) */
+int sx_clamp_if(const float* S, int64_t R, int32_t L, int64_t lds, const float* amax, float clip, const float* dY,
+                int64_t ldy, float* out, int64_t ldo, void* stream);
+
 /* Dropout seeds: every dropout-capable entry takes `seed` (by value) and `seed_dev` (device pointer or NULL); the
  * effective seed is seed + *seed_dev, read on the device in stream order, so a captured CUDA graph draws a new mask
  * on every replay.  sx_seed_derive writes out[0] = base[0] + add (the per-call seed an op keeps for its backward);

@@ -17,6 +17,7 @@ SX_MAJOR_K, SX_MAJOR_MN = 0, 1
 SX_BIAS_NONE, SX_BIAS_N, SX_BIAS_M = 0, 1, 2
 SX_ACT_NONE, SX_ACT_GELU, SX_ACT_GELU_BWD = 0, 1, 2
 SX_SCHED_WARMUP_LINEAR, SX_SCHED_WARMUP_CONSTANT = 0, 1
+SX_CONSIST_BCE, SX_CONSIST_MARGIN = 0, 1
 
 
 class SxError(RuntimeError):
@@ -52,6 +53,15 @@ class sx_attn_probs_args(C.Structure):
                 ("_pad", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("posbias", sx_posbias)]
 
 
+class sx_consist_args(C.Structure):
+    _fields_ = [("B", C.c_int32), ("N", C.c_int32), ("A", C.c_int32), ("K", C.c_int32), ("variant", C.c_int32),
+                ("round_r", C.c_int32), ("Xo", C.c_void_p), ("xo_ld", C.c_int64), ("xo_bstride", C.c_int64),
+                ("Xt", C.c_void_p), ("xt_ld", C.c_int64), ("xt_bstride", C.c_int64), ("X", C.c_void_p),
+                ("x_ld", C.c_int64), ("x_bstride", C.c_int64), ("F", C.c_void_p), ("mu", C.c_void_p), ("R", C.c_void_p),
+                ("ldr", C.c_int64), ("out", C.c_void_p), ("cap", C.c_void_p), ("cap_scale", C.c_float),
+                ("_pad", C.c_int32), ("part", C.c_void_p), ("part_floats", C.c_int64)]
+
+
 class sx_resample_grid(C.Structure):
     _fields_ = [("lin", C.c_int32 * 3), ("lout", C.c_int32 * 3), ("ratio", C.c_float * 3)]
 
@@ -63,6 +73,9 @@ _PROTOS = {
     "sx_gemm": [C.POINTER(sx_gemm_args), _P],
     "sx_gemm_debug_set": [C.c_char_p, _L],
     "sx_attn_probs_fwd": [C.POINTER(sx_attn_probs_args), _P],
+    "sx_attn_consist_fwd": [C.POINTER(sx_consist_args), _P],
+    "sx_attn_consist_bwd": [C.POINTER(sx_consist_args), _P, _P, _I, _I, _L, _L, _P, _P, _P, _L, _L, _P],
+    "sx_clamp_if": [_P, _L, _I, _L, _P, _F, _P, _L, _P, _L, _P],
     "sx_reduce_max": [_P, _L, _P, _P],
     "sx_pos_lsinu_fwd": [_P, _P, _L, _I, _P, _P, _I, _P, _P],
     "sx_pos_lsinu_bwd": [_P, _P, _L, _I, _P, _P, _I, _P, _P, _P, _P, _P, _L, _P],
@@ -144,7 +157,7 @@ def check(rc, what):
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
 _LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
              "sx_attn_probs_fwd": 2, "sx_colsum": 2, "sx_colsum_batched": 2,
-             "sx_softmax_posbias_bwd": 2}
+             "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing
 

@@ -507,7 +507,8 @@ class CrossAttFeatTrans(nn.Module):
             probs = ops.softmax_posbias(s, pb, amax, float(self.attn_clip), p, seed, self._diag)
         else:
             probs = ops.softmax(s, amax, float(self.attn_clip), p, seed, self._diag)
-        self.attention_scores = s if self.keep_attn_scores else None
+        # kept after the conditional clamp, as the reference keeps them (:578-598)
+        self.attention_scores = ops.clamp_if(s, amax, float(self.attn_clip)) if self.keep_attn_scores else None
         if self.training:
             self.call_count += 1
             if self.call_count % self.attn_diag_cycles == 0:
@@ -690,7 +691,7 @@ class SqueezedAttFeatTrans(nn.Module):
         s = ops.attn_scores(qw, in_feat, 1, amax, rb, tag="insq")                      # [B,1,A,N]
         p = t.att_dropout.p if t.training else 0.0
         probs = ops.softmax(s, amax, float(t.attn_clip), p, ops.new_dropout_seed(dev) if p > 0 else 0, t._diag)
-        t.attention_scores = s if t.keep_attn_scores else None
+        t.attention_scores = ops.clamp_if(s, amax, float(t.attn_clip)) if t.keep_attn_scores else None
         if t.training:
             t.call_count += 1
         u = ops.attn_pv(probs, in_feat, 1, tag="insq", round_out=not x3)               # P1 h            [B,1,A,C]

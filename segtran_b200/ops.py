@@ -2047,3 +2047,177 @@ def seg_head(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, d_pool_k=1, perm
         out = transpose(Lo.reshape(B * K, Dd, H * W)).view(B, K, H, W, Dd)
         return out
     return resize_linear(Lo, tuple(out_size))
+
+
+# ------------------------------------------------------------------------------------------------
+# attention-consistency loss (train3d.py:426-449, train2d.py:668-723): csrc/sx_consist.cu
+# ------------------------------------------------------------------------------------------------
+CONSIST_BCE, CONSIST_MARGIN = L.SX_CONSIST_BCE, L.SX_CONSIST_MARGIN
+
+
+def _consist_pack(x3: torch.Tensor, transpose_in: bool, rnd: int) -> torch.Tensor:
+    """[B,R,C] -> K-major [B,N,pad4(A)] copy of the pair operand (N, A) = (R, C), or (C, R) when transpose_in; the pad
+    columns are zero (the column sums of the margin variant run over them); TF32-rounded when rnd."""
+    B = x3.shape[0]
+    N, A = (x3.shape[2], x3.shape[1]) if transpose_in else (x3.shape[1], x3.shape[2])
+    Ap = _pad4(A)
+    if Ap == A and x3.is_contiguous():
+        out = torch.empty((B, N, A), device=x3.device, dtype=torch.float32)
+        if transpose_in:
+            L.call("sx_transpose", x3.data_ptr(), B, A, N, out.data_ptr(), _stream())
+            src = out
+        else:
+            src = x3
+    else:
+        out = torch.zeros((B, N, Ap), device=x3.device, dtype=torch.float32)
+        out[..., :A].copy_(x3.transpose(1, 2) if transpose_in else x3)
+        src = out
+    if rnd or src is not out:
+        L.call("sx_convert", src.data_ptr(), L.SX_F32, out.numel(), out.data_ptr(), L.SX_F32, rnd, _stream())
+    return out
+
+
+def _consist_colsums(P: torch.Tensor, A: int) -> torch.Tensor:
+    """[B,N,Ap] -> [B,A] column sums per batch, in a fixed order."""
+    B, N, Ap = P.shape
+    cs = _zeros((B, Ap), P.device)
+    L.call("sx_colsum_batched", P.data_ptr(), 1, 0, B, N * Ap, N, Ap, Ap, cs.data_ptr(), *_part_args(P.device), _stream())
+    return cs if Ap == A else cs[:, :A].contiguous()
+
+
+class _AttnConsist(torch.autograd.Function):
+    """One layer's attention-consistency loss.  Pair entry (Xo [B,1,N,A], Xi [B,1,A,N]): X = Xo Xi is formed tile by tile
+    on the tensor cores (precision class "big") and never stored; dense entry X [B,1,N,N].  F [B,K,N] is the flattened
+    downsampled mask.  cap: optional device float[2] that accumulates the layers' losses and the 2-D cap factor."""
+
+    @staticmethod
+    def forward(ctx, Xo, Xi, X, F, variant, cap, cap_scale):
+        _req_cuda(Xo, Xi, X, F, cap)
+        B, K, N = F.shape
+        dev = F.device
+        need = any(ctx.needs_input_grad[:3])
+        a = L.sx_consist_args()
+        a.B, a.N, a.K, a.variant = B, N, K, variant
+        F = F.contiguous()
+        a.F = F.data_ptr()
+        out = torch.empty(2 + B, device=dev, dtype=torch.float32)
+        a.out = out.data_ptr()
+        a.cap, a.cap_scale = _ptr(cap), float(cap_scale)
+        a.part, a.part_floats = _part_args(dev)
+        margin = variant == CONSIST_MARGIN
+        nn2 = 1.0 / (float(N) * N)
+        saved = []
+        if X is None:
+            A = Xo.shape[-1]
+            three = _three_pass("big")
+            XoP = _consist_pack(Xo.reshape(B, N, A), False, 0 if three else 1)
+            XtP = _consist_pack(Xi.reshape(B, A, N), True, 0 if three else 1)
+            cs_o = cs_t = None
+            if margin:                   # mu_b = (1^T Xo_b)(Xi_b 1) / N^2: no pass over X
+                cs_o, cs_t = _consist_colsums(XoP, A), _consist_colsums(XtP, A)
+                mu = _sgemm(cs_o, cs_t, 1, 1, A, (A, 1), (1, 1), alpha=nn2, Z=B, zs=(A, A, 1)).view(B)
+                a.mu = mu.data_ptr()
+            ko, kt = (_split_cat(XoP[..., :A], 0)[0], _split_cat(XtP[..., :A], 1)[0]) if three else (XoP, XtP)
+            a.A = ko.shape[-1] if three else A
+            a.Xo, a.xo_ld, a.xo_bstride = ko.data_ptr(), ko.stride(1), ko.stride(0)
+            a.Xt, a.xt_ld, a.xt_bstride = kt.data_ptr(), kt.stride(1), kt.stride(0)
+            a.round_r = _rt()
+            saved = [XoP, XtP, cs_o, cs_t]
+            ctx.shapes = (Xo.shape, Xi.shape, A)
+        else:
+            X3 = X.reshape(B, N, N)
+            if X3.stride(2) != 1 or X3.stride(0) != N * X3.stride(1):
+                X3 = X3.contiguous()
+            if margin:                   # mu_b: one ordered reduction over the rows of X_b
+                rs = _zeros((B * N,), dev)
+                L.call("sx_rowsum", X3.data_ptr(), B * N, N, X3.stride(1), B * N, rs.data_ptr(), *_part_args(dev), _stream())
+                mu = _zeros((B,), dev)
+                L.call("sx_rowsum", rs.data_ptr(), B, N, N, B, mu.data_ptr(), *_part_args(dev), _stream())
+                L.call("sx_scale", mu.data_ptr(), B, None, nn2, mu.data_ptr(), _stream())
+                a.mu = mu.data_ptr()
+            a.X, a.x_ld, a.x_bstride = X3.data_ptr(), X3.stride(1), X3.stride(0)
+            ctx.shapes = (X.shape,)
+        R = None
+        if need:
+            R = _rowpad_empty((B, N, N), dev)
+            a.R, a.ldr = R.data_ptr(), R.stride(1)
+        L.call("sx_attn_consist_fwd", C.byref(a), _stream())
+        ctx.save_for_backward(out, R, *[t for t in saved if t is not None])
+        ctx.meta = (B, N, variant, X is None, margin)
+        return out[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        out, R, *rest = ctx.saved_tensors
+        B, N, variant, pair, margin = ctx.meta
+        a = L.sx_consist_args()
+        a.B, a.N, a.variant, a.out = B, N, variant, out.data_ptr()
+        g = g.contiguous()
+        dXo = dXi = dX = None
+
+        def finish(G, rows, cols, vrow, vcol):             # in place: G <- s * (G + m_b v)
+            L.call("sx_attn_consist_bwd", C.byref(a), g.data_ptr(), G.data_ptr(), rows, cols, G.stride(-2),
+                   G.stride(-3), _ptr(vrow), _ptr(vcol), G.data_ptr(), G.stride(-2), G.stride(-3), _stream())
+            return G
+
+        if pair:
+            XoP, XtP = rest[0], rest[1]
+            cs_o, cs_t = (rest[2], rest[3]) if margin else (None, None)
+            xo_shape, xi_shape, A = ctx.shapes
+            if ctx.needs_input_grad[0]:              # dXo_b = R_b Xi_b^T
+                G = gemm_nt(R, XtP[..., :A].transpose(1, 2), round_out=False)[0]
+                dXo = finish(G, N, A, None, cs_t).view(xo_shape)
+            if ctx.needs_input_grad[1]:              # dXi_b = Xo_b^T R_b
+                G = gemm_nt(XoP[..., :A].transpose(1, 2), R.transpose(1, 2), round_out=False)[0]
+                dXi = finish(G, A, N, cs_o, None).view(xi_shape)
+        elif ctx.needs_input_grad[2]:
+            (x_shape,) = ctx.shapes
+            dX = torch.empty((B, N, N), device=R.device, dtype=torch.float32)
+            L.call("sx_attn_consist_bwd", C.byref(a), g.data_ptr(), R.data_ptr(), N, N, R.stride(1), R.stride(0), None,
+                   None, dX.data_ptr(), N, N * N, _stream())
+            dX = dX.view(x_shape)
+        return dXo, dXi, dX, None, None, None, None
+
+
+class _ClampIf(torch.autograd.Function):
+    """The scores a layer keeps for the attention-consistency loss (segtran_shared.py:578-598): clamp(S, -clip, clip) when
+    the call's maximum (*amax, on the device) exceeds clip, S otherwise; the clamp mask in the backward."""
+
+    @staticmethod
+    def forward(ctx, S, amax, clip):
+        R, Lr = S.numel() // S.shape[-1], S.shape[-1]
+        if not _rows_ok(S):
+            S = _rowpad(S)
+        out = _rowpad_empty(S.shape, S.device)
+        L.call("sx_clamp_if", S.data_ptr(), R, Lr, S.stride(-2), amax.data_ptr(), float(clip), None, 0, out.data_ptr(),
+               out.stride(-2), _stream())
+        ctx.save_for_backward(S, amax)
+        ctx.clip = float(clip)
+        return out
+
+    @staticmethod
+    def backward(ctx, dY):
+        S, amax = ctx.saved_tensors
+        R, Lr = S.numel() // S.shape[-1], S.shape[-1]
+        dY = dY if dY.is_contiguous() else _rowpad(dY)
+        ldy = Lr if dY.is_contiguous() else dY.stride(-2)
+        dS = _rowpad_empty(S.shape, S.device)
+        L.call("sx_clamp_if", S.data_ptr(), R, Lr, S.stride(-2), amax.data_ptr(), ctx.clip, dY.data_ptr(), ldy,
+               dS.data_ptr(), dS.stride(-2), _stream())
+        return dS, None, None
+
+
+def clamp_if(S, amax, clip):
+    return _ClampIf.apply(S, amax, clip)
+
+
+def attn_consist(entry, F, variant, cap=None, cap_scale=1.0):
+    """Attention-consistency loss of one layer entry of `layers_attn_scores` as a 0-dim device tensor.
+    entry: [in_ator_scores [B,1,A,N], ator_out_scores [B,1,N,A]] (squeezed layer, X = ator_out . in_ator) or the
+    dense [B,1,N,N] scores (--nosqueeze); F [B,K,N] fp32 (K <= 16); variant CONSIST_BCE (train3d.py) or CONSIST_MARGIN
+    (train2d.py).  cap (device float[2]): cap[0] += the loss, cap[1] <- the factor 1/t if t = cap_scale*cap[0] > 1, else 1
+    — train2d.py's cap on the layer mean, read on the device by the caller."""
+    if isinstance(entry, (list, tuple)):
+        Xi, Xo = entry
+        return _AttnConsist.apply(Xo, Xi, None, F, int(variant), cap, cap_scale)
+    return _AttnConsist.apply(None, None, entry, F, int(variant), cap, cap_scale)

@@ -2,6 +2,7 @@
 as device-resident kernels behind the same call shapes the reference training loop uses.
 
   seg_loss(logits, mask, pos_weight, class_weights, dice_w)   train3d.py:731-756 + utils/losses.py:47-60
+  attn_consist_loss3d / attn_consist_loss2d                    train3d.py:426-449 / train2d.py:668-723 (--attnconsist)
   FlatBertAdam(param_groups, ..., bucket=GradBucket)           optimization.py:43-164 + train3d.py:760-761 (--gradclip)
 
 Nothing here synchronises with the host: the loss, the clip coefficients, the scheduled learning rates and the step
@@ -59,6 +60,57 @@ def seg_loss(logits: torch.Tensor, mask: torch.Tensor, pos_weight: Optional[torc
     One pass over the logits for the sums, one for the gradient; ce and dice are returned for logging."""
     o = _SegLoss.apply(logits, mask, pos_weight, class_weights, dice_w)
     return o[0], o[1].detach(), o[2].detach()
+
+
+def _attn_consist_loss(layers_attn_scores, orig_feat_shape, mask, only_first_layer, variant):
+    grid = tuple(int(s) for s in orig_feat_shape)
+    if variant == ops.CONSIST_BCE:
+        if mask.dim() != 5 or len(grid) != 3:
+            raise ValueError("attn_consist_loss3d: mask [B,C,H,W,D] and a 3-D orig_feat_shape expected")
+        mask = mask.permute(0, 1, 4, 2, 3)                 # (train3d.py:429) [B,C,D,H,W], resized to orig_feat_shape
+    elif mask.dim() != 4 or len(grid) != 2:
+        raise ValueError("attn_consist_loss2d: mask [B,C,H,W] and a 2-D orig_feat_shape expected")
+    B, K = mask.shape[:2]
+    N = 1
+    for s in grid:
+        N *= s
+    n = 1 if only_first_layer else len(layers_attn_scores)
+    entries = list(layers_attn_scores[:n])
+    for e in entries:
+        t = e[1] if isinstance(e, (list, tuple)) else e        # ator_out_scores [B,1,N,A] / dense [B,1,N,N]
+        if t.shape[0] != B:
+            raise ValueError("attn_consist_loss: the mask has batch %d, the attention scores %d" % (B, t.shape[0]))
+        if t.shape[-2] != N or (not isinstance(e, (list, tuple)) and t.shape[-1] != N):
+            raise ValueError("attn_consist_loss: %d tokens in the attention scores, orig_feat_shape %s has %d"
+                             % (t.shape[-2], grid, N))
+    if K > 16:
+        raise ValueError("attn_consist_loss: %d mask channels (at most 16 supported)" % K)
+    with torch.no_grad():                                  # linear resize, align_corners=False, one pass per axis
+        F = ops.resize_linear(mask.to(torch.float32), grid).reshape(B, K, N).contiguous()
+    cap = torch.zeros(2, device=F.device, dtype=torch.float32) if variant == ops.CONSIST_MARGIN else None
+    total = None
+    for e in entries:
+        l = ops.attn_consist(e, F, variant, cap, 1.0 / n)
+        total = l if total is None else ops.add(total, l)
+    loss = ops.scale(total, 1.0 / n)
+    if cap is not None:                                    # `if loss > 1: loss /= loss.item()`, factor kept on the device
+        loss = ops.dot(loss, cap[1:2]).reshape(())
+    return loss
+
+
+def attn_consist_loss3d(layers_attn_scores, orig_feat_shape, mask, only_first_layer=True):
+    """train3d.py:426-449 as a drop-in: mean BCE-with-logits of each layer's token affinity X (ator_out . in_ator for a
+    squeezed layer, the [B,1,N,N] scores otherwise) against clip(F^T F, 0, 1) of the mask resized to orig_feat_shape,
+    averaged over the first layer or all of them.  mask [B,C,H,W,D]; orig_feat_shape (D2,H2,W2)-ordered as the reference
+    resizes it.  A 0-dim device tensor; X and the target matrix are never stored."""
+    return _attn_consist_loss(layers_attn_scores, orig_feat_shape, mask, only_first_layer, ops.CONSIST_BCE)
+
+
+def attn_consist_loss2d(layers_attn_scores, orig_feat_shape, mask, only_first_layer=False):
+    """train2d.py:668-723 as a drop-in: per layer, the mean |x - mu_b| over the pairs whose affinity sits on the wrong side
+    of the batch mean mu_b (same-class pairs below it, other pairs above mu_b - 0.1); averaged over the layers and capped
+    at 1 (the reference's `loss /= loss.item()` becomes a device-side factor).  mask [B,C,H,W]."""
+    return _attn_consist_loss(layers_attn_scores, orig_feat_shape, mask, only_first_layer, ops.CONSIST_MARGIN)
 
 
 # ------------------------------------------------------------------------------------------------------------------
