@@ -353,6 +353,41 @@ int sx_token_scores(const float* vf, const float* W, int32_t B, int32_t N, int32
 /* and its data gradient: dvf[b,n,f] = sum_k dt[b,k,n] W[k,f]   (F % 4 == 0) */
 int sx_token_scores_bwd(const float* dt, const float* W, int32_t B, int32_t N, int32_t F, int32_t K, float* dvf,
                         void* stream);
+/* Out-FPN dropout head (--outdrop; segtran3d.py:372-396, :488-490; segtran2d.py:304-311, :427), which cannot be
+ * collapsed: the dropout mask is per channel.  The dropped map X [B,F',D',HW] is never written:
+ *   Ls[b,k,d',hw] = bc[k] + sum_f Wc[k,f] keep(b,f,d',hw) X[b,f,d',hw] / (1-p)
+ * with X formed on the fly from src [B,Fs,Ds,HW] by the depth map `dmap`:
+ *   SX_HEAD_DMAP_NONE   X = src                                    (F' = Fs, D' = Ds; 2-D heads pass Ds = 1)
+ *   SX_HEAD_DMAP_INTERP X = linear resize of src along depth to D' = Dk*Ds (F.interpolate, align_corners=False)
+ *   SX_HEAD_DMAP_UNFOLD X[b,f,j*Ds+i,hw] = src[b,f*Dk+j,i,hw]      (out_fpn_upsampleD's reshape; F' = Fs/Dk, D' = Dk*Ds)
+ * keep(e) = the counter-based dropout hash of the flat index e of the element in [B,F',D',HW] layout with the effective
+ * seed seed + *seed_dev (CUDA-graph safe), p in [0, 1).  Wc [K][F'], bc [K] (optional); any K (classes are processed
+ * in chunks of 4).  Ls / dLs: [B][K][D'][HW].
+ * fwd writes Ls.  bwd writes dsrc [B,Fs,Ds,HW] (or adds to it when accumulate) in gather form and ADDS
+ * dWc[k,f] = sum keep dLs X / (1-p) into dWc through ordered per-CTA slots of `part`; the class-bias gradient is the
+ * row sum of dLs (sx_rowsum).  No float atomics: two runs give the same bits. */
+enum { SX_HEAD_DMAP_NONE = 0, SX_HEAD_DMAP_INTERP = 1, SX_HEAD_DMAP_UNFOLD = 2 };
+typedef struct {
+  const float* src;
+  int32_t B, Fs, Ds;
+  int32_t Fo;                    /* F' */
+  int64_t HW;
+  int32_t Dk;                    /* D_pool_K */
+  int32_t dmap;                  /* SX_HEAD_DMAP_* */
+  int32_t K;
+  int32_t _pad;
+  const float* Wc;
+  const float* bc;
+  float p;
+  uint32_t _pad2;
+  uint64_t seed;
+  const uint64_t* seed_dev;
+  float* part;
+  int64_t part_floats;
+} sx_head_dropout_args;
+int sx_head_dropout_fwd(const sx_head_dropout_args* args, float* Ls, void* stream);
+int sx_head_dropout_bwd(const sx_head_dropout_args* args, const float* dLs, float* dsrc, int32_t accumulate, float* dWc,
+                        void* stream);
 /* -------------------------------------------------------------------------------------------
  * FPN pyramid stage (SURVEY.md section 8 row f.1; segtran3d.py:299-313, :347-359, segtran2d.py:244-300):
  *   curr <- GroupNorm_G( conv1x1(curr) + bias + upsample(higher) )

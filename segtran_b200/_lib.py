@@ -18,6 +18,7 @@ SX_BIAS_NONE, SX_BIAS_N, SX_BIAS_M = 0, 1, 2
 SX_ACT_NONE, SX_ACT_GELU, SX_ACT_GELU_BWD = 0, 1, 2
 SX_SCHED_WARMUP_LINEAR, SX_SCHED_WARMUP_CONSTANT = 0, 1
 SX_CONSIST_BCE, SX_CONSIST_MARGIN = 0, 1
+SX_HEAD_DMAP_NONE, SX_HEAD_DMAP_INTERP, SX_HEAD_DMAP_UNFOLD = 0, 1, 2
 
 
 class SxError(RuntimeError):
@@ -60,6 +61,13 @@ class sx_consist_args(C.Structure):
                 ("x_ld", C.c_int64), ("x_bstride", C.c_int64), ("F", C.c_void_p), ("mu", C.c_void_p), ("R", C.c_void_p),
                 ("ldr", C.c_int64), ("out", C.c_void_p), ("cap", C.c_void_p), ("cap_scale", C.c_float),
                 ("_pad", C.c_int32), ("part", C.c_void_p), ("part_floats", C.c_int64)]
+
+
+class sx_head_dropout_args(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("B", C.c_int32), ("Fs", C.c_int32), ("Ds", C.c_int32), ("Fo", C.c_int32),
+                ("HW", C.c_int64), ("Dk", C.c_int32), ("dmap", C.c_int32), ("K", C.c_int32), ("_pad", C.c_int32),
+                ("Wc", C.c_void_p), ("bc", C.c_void_p), ("p", C.c_float), ("_pad2", C.c_uint32), ("seed", C.c_uint64),
+                ("seed_dev", C.c_void_p), ("part", C.c_void_p), ("part_floats", C.c_int64)]
 
 
 class sx_resample_grid(C.Structure):
@@ -110,6 +118,8 @@ _PROTOS = {
     "sx_head_contract_fwd": [_P, _P, _P, _I, _I, _L, _I, _P, _I, _P],
     "sx_head_contract_bwd_data": [_P, _P, _I, _I, _L, _I, _P, _P],
     "sx_head_contract_bwd_weight": [_P, _P, _I, _I, _L, _I, _P, _P],
+    "sx_head_dropout_fwd": [C.POINTER(sx_head_dropout_args), _P, _P],
+    "sx_head_dropout_bwd": [C.POINTER(sx_head_dropout_args), _P, _P, _I, _P, _P],
     "sx_token_scores": [_P, _P, _I, _I, _I, _I, _P, _P],
     "sx_token_scores_bwd": [_P, _P, _I, _I, _I, _I, _P, _P],
     "sx_resize_axis_fwd": [_P, _L, _I, _I, _L, _P, _I, _P],
@@ -157,7 +167,7 @@ def check(rc, what):
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
 _LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
              "sx_attn_probs_fwd": 2, "sx_colsum": 2, "sx_colsum_batched": 2,
-             "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2}
+             "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2, "sx_head_dropout_bwd": 2}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing
 

@@ -1,7 +1,8 @@
 """Segtran2d shell on the H100 hot path — same module surface as the reference's code/networks/segtran2d.py.
 
 Backbone (ResNet / EfficientNet) and the in-/out-FPN pyramids stay stock PyTorch/cuDNN (out of the hot path);
-token flatten, the Squeeze-and-Expansion stack and the pixel-wise head (collapsed form) run on segtran_b200 kernels.
+token flatten, the Squeeze-and-Expansion stack and the pixel-wise head (collapsed form; with --outdrop in training, the
+dropout head of csrc/sx_head_drop.cu) run on segtran_b200 kernels.
 The backbone is the reference's own class when this package is dropped into the reference tree
 (``resnet`` / ``efficientnet.model`` importable), or any module passed as ``backbone=``.
 """
@@ -230,10 +231,11 @@ class Segtran2d(SegtranInitWeights):
             lv = self.voxel_fusion.layers_vfeat[i]
             self.feature_maps.append(lv.detach().view(B0, H2, W2, self.translayer_dims[i + 1]).permute(0, 3, 1, 2))
         self.orig_feat_shape = grid
-        if self.out_fpn_do_dropout and self.training:
-            raise NotImplementedError("segtran_b200: out_fpn_do_dropout breaks the linear head collapse")
         bridge = self.out_fpn_bridgeconv
         Wb, bb = (bridge.weight, bridge.bias) if isinstance(bridge, nn.Conv2d) else (None, None)
+        if self.out_fpn_do_dropout and self.training:         # per-channel mask: the dropout head (sx_head_drop.cu)
+            return ops.seg_head_dropout(curr_feat, fused, tuple(grid), Wb, bb, self.out_conv.weight, self.out_conv.bias,
+                                        (H, W), self.out_fpn_dropout.p)
         return ops.seg_head(curr_feat, fused, tuple(grid), Wb, bb, self.out_conv.weight, self.out_conv.bias, (H, W))
 
     def forward(self, batch):

@@ -7,7 +7,9 @@ What runs where
     with ``extract_features`` passed as ``backbone=``.
   * token flatten, Squeeze-and-Expansion stack, scatter and the voxel-wise head: segtran_b200 kernels.
     The head uses the collapsed form (csrc/sx_head.cu): ``out_fpn_bridgeconv3d`` and ``out_conv3d`` keep their
-    own parameters (checkpoint compatible) but are applied as one class-dimension contraction.
+    own parameters (checkpoint compatible) but are applied as one class-dimension contraction.  ``--upd conv``
+    (``out_fpn_upsampleD``) is linear too and is folded into the class conv in weight space.  ``--outdrop`` in training
+    runs the dropout head (csrc/sx_head_drop.cu), which never writes the dropped full-resolution map.
 """
 from __future__ import annotations
 
@@ -111,8 +113,8 @@ class Segtran3d(SegtranInitWeights):
         self.D_pool_K = config.D_pool_K
         self.out_fpn_upsampleD_scheme = config.out_fpn_upsampleD_scheme
         self.input_scale = config.input_scale
-        if self.out_fpn_upsampleD_scheme not in ('interp', 'none'):
-            raise NotImplementedError("segtran_b200: out_fpn_upsampleD_scheme='conv' is not implemented")
+        if self.out_fpn_upsampleD_scheme not in ('interp', 'none', 'conv'):
+            raise NotImplementedError("out_fpn_upsampleD_scheme=%r" % self.out_fpn_upsampleD_scheme)
 
         if self.eff_in_channels != 3:
             if self.inchan_to3_scheme == 'avgto3' and self.eff_in_channels in (2, 4):
@@ -165,7 +167,12 @@ class Segtran3d(SegtranInitWeights):
         self.out_fpn23_conv3d = nn.Conv3d(d[2], d[3], 1)
         self.out_fpn34_conv3d = nn.Conv3d(d[3], d[4], 1)
         self.out_fpn_bridgeconv3d = nn.Conv3d(d[last_out], self.trans_out_dim, 1)
-        self.out_feat_dim = self.out_fpn_out_dim
+        if self.out_fpn_upsampleD_scheme == 'conv':
+            # created here, before the norms, as the reference does: seeded construction draws the same weights
+            self.out_feat_dim = self.out_fpn_out_dim // self.D_pool_K
+            self.out_fpn_upsampleD = nn.Conv3d(self.out_fpn_out_dim, self.out_feat_dim * self.D_pool_K, 1)
+        else:
+            self.out_feat_dim = self.out_fpn_out_dim
         if self.out_fpn_use_bn:
             self.out_bn2b, self.out_bn3b, self.out_bn4b = nn.BatchNorm3d(d[2]), nn.BatchNorm3d(d[3]), nn.BatchNorm3d(d[4])
             self.out_fpn_norms = [None, None, self.out_bn2b, self.out_bn3b, self.out_bn4b]
@@ -261,11 +268,26 @@ class Segtran3d(SegtranInitWeights):
             self._pos_cache_key, self._pos_cache = key, idx
         voxels_pos = self._pos_cache.unsqueeze(0).expand(B, -1, -1)  # one set of positions, shared by the batch
         fused = self.voxel_fusion(vfeat, voxels_pos, None if vmask is None else vmask.unsqueeze(2), grid)
-        ops.grad_ready(fused, list(self.out_fpn_bridgeconv3d.parameters()) + list(self.out_conv3d.parameters()))   # backward past the head
+        head_params = list(self.out_fpn_bridgeconv3d.parameters()) + list(self.out_conv3d.parameters())
+        if self.out_fpn_upsampleD_scheme == 'conv':
+            head_params += list(self.out_fpn_upsampleD.parameters())
+        ops.grad_ready(fused, head_params)                            # backward past the head
         self.layers_attn_scores = self.voxel_fusion.layers_attn_scores
         self.orig_feat_shape = grid
+        bridge, cls = self.out_fpn_bridgeconv3d, self.out_conv3d
+        # the depth upsampling runs only when D_pool_K > 1 (reference segtran3d.py:372)
+        unfold = self.D_pool_K > 1 and self.out_fpn_upsampleD_scheme == 'conv'
         if self.out_fpn_do_dropout and self.training:
-            raise NotImplementedError("segtran_b200: out_fpn_do_dropout breaks the linear head collapse")
+            ud = self.out_fpn_upsampleD if unfold else None
+            return ops.seg_head_dropout(curr_feat, fused, tuple(grid), bridge.weight, bridge.bias, cls.weight, cls.bias,
+                                        out_size, self.out_fpn_dropout.p, d_pool_k=self.D_pool_K,
+                                        upsample_d=self.out_fpn_upsampleD_scheme,
+                                        Wu=None if ud is None else ud.weight, bu=None if ud is None else ud.bias)
+        if unfold:
+            ud = self.out_fpn_upsampleD
+            Wf, bf = ops.fold_unfold(cls.weight, cls.bias, ud.weight, ud.bias, self.D_pool_K)
+            return ops.seg_head(curr_feat, fused, tuple(grid), bridge.weight, bridge.bias, Wf, bf, out_size,
+                                d_unfold=self.D_pool_K)
         dk = self.D_pool_K if (self.D_pool_K > 1 and self.out_fpn_upsampleD_scheme == 'interp') else 1
         return ops.seg_head(curr_feat, fused, tuple(grid), self.out_fpn_bridgeconv3d.weight,
                             self.out_fpn_bridgeconv3d.bias, self.out_conv3d.weight, self.out_conv3d.bias, out_size,

@@ -2027,26 +2027,184 @@ def fpn_stage(cur, higher, conv, norm, scheme="AN"):
     return _Add.apply(group_norm(y, norm.weight, norm.bias, norm.num_groups, norm.eps), hi)
 
 
-def seg_head(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, d_pool_k=1, permute_dhw_to_hwd=False):
+HEAD_MAXK = 8        # classes per pass of the head-contraction entry points (csrc/sx_head.cu MAXK)
+
+
+def _head_out(Lo, out_size):
+    """Class scores at the head resolution [B,K,*sp] -> logits: 3-D (D',H1,W1) -> trilinear to (D,H,W), permuted to
+    (H,W,D) (segtran3d.py:488-496); 2-D -> bilinear to out_size (segtran2d.py:435-436)."""
+    if Lo.dim() == 5:
+        B, K = Lo.shape[:2]
+        H, W, D = out_size
+        Lo = resize_linear(Lo, (D, H, W))                  # same maps as interpolating the (H,W,D)-permuted tensor
+        Dd = Lo.shape[2]
+        return transpose(Lo.reshape(B * K, Dd, H * W)).view(B, K, H, W, Dd)
+    return resize_linear(Lo, tuple(out_size))
+
+
+def _sgemm_s(A, B, C, M, N, K, sa, sb, sc, Z=1, zs=(0, 0, 0), accumulate=False):
+    """sx_sgemm_small with explicit strides on every operand, output included: sa=(sam,sak), sb=(sbk,sbn), sc=(scm,scn),
+    zs = batch strides of (A, B, C)."""
+    L.call("sx_sgemm_small", A.data_ptr(), B.data_ptr(), C.data_ptr(), M, N, K, sa[0], sa[1], sb[0], sb[1], sc[0], sc[1],
+           Z, zs[0], zs[1], zs[2], 1.0, 1 if accumulate else 0, _stream())
+    return C
+
+
+class _FoldUnfold(torch.autograd.Function):
+    """The depth-unfolding conv of --upd conv (out_fpn_upsampleD, segtran3d.py:207-213, :373-379) folded into the class
+    conv in weight space.  Wu [F'*Dk, F], bu [F'*Dk], Wc [K, F'], bc [K]; source channel f*Dk + j of Wu's output lands at
+    output depth j*D1 + i, so class row (k, j) of the folded head is
+        Wf[k*Dk + j, :] = sum_f Wc[k,f] Wu[f*Dk + j, :]        bf[k*Dk + j] = bc[k] + sum_f Wc[k,f] bu[f*Dk + j]"""
+
+    @staticmethod
+    def forward(ctx, Wc, bc, Wu, bu, Dk):
+        K, Fo = Wc.shape
+        Fd = Wu.shape[1]
+        Wc = Wc.contiguous()
+        Wu = Wu.reshape(Fo * Dk, Fd).contiguous()
+        bu = bu.contiguous()
+        Wf = torch.empty((K, Dk, Fd), device=Wc.device, dtype=torch.float32)
+        _sgemm_s(Wc, Wu, Wf, K, Fd, Fo, (Fo, 1), (Dk * Fd, 1), (Dk * Fd, 1), Z=Dk, zs=(0, Fd, Fd))
+        bf = bc.detach().reshape(K, 1).expand(K, Dk).contiguous()
+        _sgemm_s(Wc, bu, bf, K, Dk, Fo, (Fo, 1), (Dk, 1), (Dk, 1), accumulate=True)
+        ctx.save_for_backward(Wc, Wu, bu)
+        ctx.Dk = Dk
+        return Wf.view(K * Dk, Fd), bf.view(K * Dk)
+
+    @staticmethod
+    def backward(ctx, gW, gb):
+        Wc, Wu, bu = ctx.saved_tensors
+        Dk = ctx.Dk
+        K, Fo = Wc.shape
+        Fd = Wu.shape[1]
+        dev = Wc.device
+        gW = torch.zeros((K * Dk, Fd), device=dev) if gW is None else gW.contiguous()
+        gb = torch.zeros((K * Dk,), device=dev) if gb is None else gb.contiguous()
+        dWc = torch.empty((K, Fo), device=dev, dtype=torch.float32)
+        _sgemm_s(gW, Wu, dWc, K, Fo, Dk * Fd, (Dk * Fd, 1), (1, Dk * Fd), (Fo, 1))          # gW . Wu^T per (j, c)
+        _sgemm_s(gb, bu, dWc, K, Fo, Dk, (Dk, 1), (1, Dk), (Fo, 1), accumulate=True)
+        dbc = _zeros((K,), dev)
+        L.call("sx_rowsum", gb.data_ptr(), K, Dk, Dk, K, dbc.data_ptr(), *_part_args(dev), _stream())
+        dWu = torch.empty((Fo * Dk, Fd), device=dev, dtype=torch.float32)
+        _sgemm_s(Wc, gW, dWu, Fo, Fd, K, (1, Fo), (Dk * Fd, 1), (Dk * Fd, 1), Z=Dk, zs=(0, Fd, Fd))
+        dbu = torch.empty((Fo * Dk,), device=dev, dtype=torch.float32)
+        _sgemm_s(Wc, gb, dbu, Fo, Dk, K, (1, Fo), (Dk, 1), (Dk, 1))
+        return dWc, dbc, dWu, dbu, None
+
+
+def fold_unfold(Wc, bc, Wu, bu, d_pool_k):
+    """(Wc [K,F',1..], bc, Wu [F'*Dk,F,1..], bu) -> the folded class conv ([K*Dk, F], [K*Dk]) of --upd conv."""
+    K = Wc.shape[0]
+    return _FoldUnfold.apply(Wc.reshape(K, -1), bc, Wu.reshape(Wu.shape[0], -1), bu, int(d_pool_k))
+
+
+def seg_head(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, d_pool_k=1, permute_dhw_to_hwd=False, d_unfold=1):
     """Collapsed voxel-wise head.  curr [B,Cf,*sp1]; vfeat_fused [B,N,F] tokens on `grid`;
     3-D: sp1=(D1,H1,W1), depth x d_pool_k, permute to (H,W,D), trilinear to out_size=(H,W,D)  (segtran3d.py:364-496)
-    2-D: sp1=(H1,W1), bilinear to out_size=(H,W)                                              (segtran2d.py:304-436)"""
+    2-D: sp1=(H1,W1), bilinear to out_size=(H,W)                                              (segtran2d.py:304-436)
+    d_unfold > 1 (--upd conv, Wc / bc from fold_unfold): class row k*d_unfold + j fills output depths j*D1 .. j*D1+D1-1
+    of class k.  More than HEAD_MAXK class rows run in chunks of HEAD_MAXK."""
     B, N, Fd = vfeat_fused.shape
     K = Wc.shape[0]
     Wc2 = Wc.reshape(K, Fd)
     sp1 = tuple(curr.shape[2:])
-    tv = _TokenClassScores.apply(vfeat_fused, Wc2).view(B, K, *grid)
-    tvup = resize_linear(tv, sp1).reshape(B, K, -1)
-    Lo = _HeadContract.apply(curr, Wb, bb, Wc2, bc, tvup)
+    if K <= HEAD_MAXK:
+        tv = _TokenClassScores.apply(vfeat_fused, Wc2).view(B, K, *grid)
+        tvup = resize_linear(tv, sp1).reshape(B, K, -1)
+        Lo = _HeadContract.apply(curr, Wb, bb, Wc2, bc, tvup)
+    else:
+        parts = []
+        for k0 in range(0, K, HEAD_MAXK):
+            Wk = Wc2[k0:k0 + HEAD_MAXK]
+            kc = Wk.shape[0]
+            tv = _TokenClassScores.apply(vfeat_fused, Wk).view(B, kc, *grid)
+            tvup = resize_linear(tv, sp1).reshape(B, kc, -1)
+            parts.append(_HeadContract.apply(curr, Wb, bb, Wk, None if bc is None else bc[k0:k0 + HEAD_MAXK], tvup))
+        Lo = torch.cat(parts, 1)
     if len(sp1) == 3:
-        if d_pool_k > 1:
+        if d_unfold > 1:
+            Lo = Lo.view(B, K // d_unfold, d_unfold * sp1[0], sp1[1], sp1[2])
+        elif d_pool_k > 1:
             Lo = resize_linear(Lo, (sp1[0] * d_pool_k, sp1[1], sp1[2]))
-        H, W, D = out_size
-        Lo = resize_linear(Lo, (D, H, W))                  # same maps as interpolating the (H,W,D)-permuted tensor
-        Dd = Lo.shape[2]
-        out = transpose(Lo.reshape(B * K, Dd, H * W)).view(B, K, H, W, Dd)
-        return out
-    return resize_linear(Lo, tuple(out_size))
+    return _head_out(Lo, out_size)
+
+
+class _HeadDropout(torch.autograd.Function):
+    """Class scores of the dropped out-FPN map (csrc/sx_head_drop.cu), the map itself never written:
+        Ls[b,k,d',hw] = bc[k] + sum_f Wc[k,f] keep(b,f,d',hw) X[b,f,d',hw] / (1-p)
+    src [B,Fs,Ds,HW] is the map before the depth upsampling (Y, or Y2 = out_fpn_upsampleD(Y) for --upd conv); X is src
+    through the depth map (none / interp x Dk / unfold).  The mask is regenerated in backward from the saved seed."""
+
+    @staticmethod
+    def forward(ctx, src, Wc, bc, p, seed, dmap, Dk):
+        src = src.contiguous()
+        Wc = Wc.contiguous()
+        B, Fs, Ds, HW = src.shape
+        K, Fo = Wc.shape
+        Do = Ds if dmap == L.SX_HEAD_DMAP_NONE else Ds * Dk
+        sv, sp = _seed_args(seed)
+        a = L.sx_head_dropout_args()
+        a.src, a.B, a.Fs, a.Ds, a.Fo, a.HW, a.Dk, a.dmap, a.K = src.data_ptr(), B, Fs, Ds, Fo, HW, Dk, dmap, K
+        a.Wc, a.bc, a.p, a.seed, a.seed_dev = Wc.data_ptr(), _ptr(bc), float(p), sv, sp
+        a.part, a.part_floats = _part_args(src.device)
+        Ls = torch.empty((B, K, Do, HW), device=src.device, dtype=torch.float32)
+        L.call("sx_head_dropout_fwd", C.byref(a), Ls.data_ptr(), _stream())
+        ctx.save_for_backward(src, Wc)
+        ctx.meta = (float(p), seed, dmap, Dk, bc is not None)
+        return Ls
+
+    @staticmethod
+    def backward(ctx, dLs):
+        src, Wc = ctx.saved_tensors
+        p, seed, dmap, Dk, has_bc = ctx.meta
+        B, Fs, Ds, HW = src.shape
+        K, Fo = Wc.shape
+        dLs = dLs.contiguous()
+        dev = src.device
+        sv, sp = _seed_args(seed)
+        a = L.sx_head_dropout_args()
+        a.src, a.B, a.Fs, a.Ds, a.Fo, a.HW, a.Dk, a.dmap, a.K = src.data_ptr(), B, Fs, Ds, Fo, HW, Dk, dmap, K
+        a.Wc, a.bc, a.p, a.seed, a.seed_dev = Wc.data_ptr(), None, p, sv, sp
+        a.part, a.part_floats = _part_args(dev)
+        dsrc = torch.empty_like(src)
+        dWc = _zeros((K, Fo), dev)
+        L.call("sx_head_dropout_bwd", C.byref(a), dLs.data_ptr(), dsrc.data_ptr(), 0, dWc.data_ptr(), _stream())
+        dbc = None
+        if has_bc:
+            dbc = _zeros((K,), dev)
+            V = dLs.shape[2] * HW
+            L.call("sx_rowsum", dLs.data_ptr(), B * K, V, V, K, dbc.data_ptr(), *_part_args(dev), _stream())
+        return dsrc, dWc, dbc, None, None, None, None
+
+
+def seg_head_dropout(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, p, d_pool_k=1, upsample_d="interp", Wu=None,
+                     bu=None, seed=None):
+    """Voxel-wise head with dropout on the out-FPN map (training with --outdrop; segtran3d.py:364-396, :488-496,
+    segtran2d.py:304-311, :427-436).  The map before the depth upsampling, Y = Wb curr + bb + up(vfeat), is built with
+    conv1x1_add and resize_linear (and Y2 = Wu Y + bu for --upd conv, Wu not None); the dropped, depth-upsampled map
+    only ever exists inside _HeadDropout.  seed: None draws a per-call device seed (a new mask on every call and every
+    CUDA-graph replay); an int or an int64 device tensor fixes it."""
+    _req_cuda(curr, vfeat_fused)
+    B, N, Fd = vfeat_fused.shape
+    K = Wc.shape[0]
+    sp1 = tuple(curr.shape[2:])
+    up = resize_linear(transpose(vfeat_fused).view(B, Fd, *grid), sp1)
+    Y = conv1x1_add(curr, Wb, bb, addend=up) if Wb is not None else add(curr.contiguous(), up)
+    Dk = int(d_pool_k)
+    if Wu is not None:
+        Y = conv1x1_add(Y, Wu, bu)
+        dmap = L.SX_HEAD_DMAP_UNFOLD
+    elif len(sp1) == 3 and Dk > 1 and upsample_d == "interp":
+        dmap = L.SX_HEAD_DMAP_INTERP
+    else:
+        dmap, Dk = L.SX_HEAD_DMAP_NONE, 1
+    if seed is None:
+        seed = new_dropout_seed(curr.device)
+    Ds = sp1[0] if len(sp1) == 3 else 1
+    HW = sp1[-1] * sp1[-2]
+    src = Y.reshape(B, Y.shape[1], Ds, HW)
+    Ls = _HeadDropout.apply(src, Wc.reshape(K, -1), bc, float(p), seed, dmap, Dk)
+    return _head_out(Ls.view(B, K, Ls.shape[2], *sp1[-2:]) if len(sp1) == 3 else Ls.view(B, K, *sp1), out_size)
 
 
 # ------------------------------------------------------------------------------------------------
