@@ -334,8 +334,10 @@ int sx_colsum_batched(const float* X, int32_t Z1, int64_t stride_z1, int32_t Z0,
 int sx_add(const float* a, const float* b, int64_t n, float* y, void* stream);
 /* out[r % out_mod] += sum_c X[r,c]  (class-bias gradient of the head: rows = (batch, class)) */
 int sx_rowsum(const float* X, int64_t R, int64_t C, int64_t ld, int32_t out_mod, float* out, float* part, int64_t part_floats, void* stream);
-/* batched transpose [Z,R,C] -> [Z,C,R] fp32: token flatten / scatter (segtran3d.py:328-330, :478-480) */
-int sx_transpose(const float* in, int64_t Z, int32_t R, int32_t C, float* out, void* stream);
+/* batched transpose [Z,R,C] -> [Z,C,R] fp32 with output row pitch ldo >= R (floats; columns R..ldo-1 are not written):
+   token flatten / scatter (segtran3d.py:328-330, :478-480, ldo = R) and the K-major GEMM operand copies (ldo = R rounded
+   up to a multiple of 4, the 16-byte row pitch TMA needs) */
+int sx_transpose(const float* in, int64_t Z, int32_t R, int32_t C, int32_t ldo, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Segmentation head, collapsed form (segtran3d.py:364-367, :381-386, :488-496; segtran2d.py:304-306,

@@ -109,7 +109,7 @@ _PROTOS = {
     "sx_split_tf32": [_P, _L, _P, _P, _P],
     "sx_split_tf32_cat": [_P, _I, _I, _I, _I, _L, _L, _L, _L, _I, _I, _P, _P],
     "sx_colsum": [_P, _I, _L, _I, _L, _P, _P, _L, _P],
-    "sx_transpose": [_P, _L, _I, _I, _P, _P],
+    "sx_transpose": [_P, _L, _I, _I, _I, _P, _P],
     "sx_colsum_batched": [_P, _I, _L, _I, _L, _L, _I, _L, _P, _P, _L, _P],
     "sx_dot": [_P, _P, _L, _P, _P],
     "sx_add": [_P, _P, _L, _P, _P],

@@ -958,12 +958,13 @@ colsum_v4_kernel(const float* __restrict__ X, int Z1, long long sz1, long long s
   }
 }
 
-// batched 2-D transpose: in [Z, R, C] -> out [Z, C, R]   (flatten / scatter, segtran3d.py:328-330, :478-480)
-__global__ void transpose_kernel(const float* __restrict__ in, int R, int C, float* __restrict__ out) {
+// batched 2-D transpose: in [Z, R, C] -> out [Z, C, R] with row pitch ldo   (flatten / scatter, segtran3d.py:328-330,
+// :478-480; K-major GEMM operand copies)
+__global__ void transpose_kernel(const float* __restrict__ in, int R, int C, int ldo, float* __restrict__ out) {
   __shared__ float tile[32][33];
   const long long z = blockIdx.z;
   const float* src = in + z * (long long)R * C;
-  float* dst = out + z * (long long)R * C;
+  float* dst = out + z * (long long)C * ldo;
   const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
   for (int j = threadIdx.y; j < 32; j += blockDim.y) {
     const int r = r0 + j, c = c0 + threadIdx.x;
@@ -972,7 +973,7 @@ __global__ void transpose_kernel(const float* __restrict__ in, int R, int C, flo
   __syncthreads();
   for (int j = threadIdx.y; j < 32; j += blockDim.y) {
     const int c = c0 + j, r = r0 + threadIdx.x;
-    if (r < R && c < C) dst[(long long)c * R + r] = tile[threadIdx.x][j];
+    if (r < R && c < C) dst[(long long)c * ldo + r] = tile[threadIdx.x][j];
   }
 }
 
@@ -1564,16 +1565,17 @@ extern "C" int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, i
   return 0;
 }
 
-extern "C" int sx_transpose(const float* in, int64_t Z, int32_t R, int32_t C, float* out, void* stream) {
+extern "C" int sx_transpose(const float* in, int64_t Z, int32_t R, int32_t C, int32_t ldo, float* out, void* stream) {
   SX_REQUIRE(Z <= 65535, "sx_transpose: batch %lld too large", (long long)Z);
-  if (R % 4 == 0 && C % 4 == 0 && al16(in) && al16(out)) {
+  SX_REQUIRE(R > 0 && C > 0 && ldo >= R, "sx_transpose: bad shape R=%d C=%d ldo=%d", R, C, ldo);
+  if (R % 4 == 0 && C % 4 == 0 && ldo % 4 == 0 && al16(in) && al16(out)) {
     dim3 gridv(sx_ceil_div(C, 128), sx_ceil_div(R, 32), (unsigned)Z);
-    transpose_v4_kernel<<<gridv, 256, 0, ST(stream)>>>(in, R, C, out);
+    transpose_v4_kernel<<<gridv, 256, 0, ST(stream)>>>(in, R, C, ldo, out);
     SX_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
   dim3 grid(sx_ceil_div(C, 32), sx_ceil_div(R, 32), (unsigned)Z), blk(32, 8);
-  transpose_kernel<<<grid, blk, 0, ST(stream)>>>(in, R, C, out);
+  transpose_kernel<<<grid, blk, 0, ST(stream)>>>(in, R, C, ldo, out);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -739,14 +739,15 @@ softmax_bwd_block(const float* __restrict__ dP, long long ldd, const float* __re
 }
 
 // ------------------------------------------------------------------------------------------------
-// batched transpose [Z,R,C] -> [Z,C,R], 32 x 128 tiles, float4 global accesses on both sides (R%4==0, C%4==0)
+// batched transpose [Z,R,C] -> [Z,C,R] with output row pitch ldo, 32 x 128 tiles, float4 global accesses on both sides
+// (R%4==0, C%4==0, ldo%4==0)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-transpose_v4_kernel(const float* __restrict__ in, int R, int C, float* __restrict__ out) {
+transpose_v4_kernel(const float* __restrict__ in, int R, int C, int ldo, float* __restrict__ out) {
   __shared__ float tile[32][129];
   const long long z = blockIdx.z;
   const float* src = in + z * (long long)R * C;
-  float* dst = out + z * (long long)R * C;
+  float* dst = out + z * (long long)C * ldo;
   const int c0 = blockIdx.x * 128, r0 = blockIdx.y * 32;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;          // 32 x 8
   for (int j = ty; j < 32; j += 8) {
@@ -763,7 +764,7 @@ transpose_v4_kernel(const float* __restrict__ in, int R, int C, float* __restric
     const int c = c0 + cl, r = r0 + r4;
     if (c < C && r < R) {
       const float4 v = make_float4(tile[r4][cl], tile[r4 + 1][cl], tile[r4 + 2][cl], tile[r4 + 3][cl]);
-      *reinterpret_cast<float4*>(dst + (long long)c * R + r) = v;
+      *reinterpret_cast<float4*>(dst + (long long)c * ldo + r) = v;
     }
   }
 }

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import os
 from typing import Optional
 
 import numpy as np
@@ -534,6 +535,50 @@ def round_tf32(x: torch.Tensor) -> torch.Tensor:
     return y
 
 
+# K-major copies of small MN-major operands.  TF32 wgmma reads only K-major shared memory, so sx_gemm rewrites an
+# MN-major TF32 operand through shared memory before the MMAs can use it, and such a launch runs at about half the
+# K-major rate (DESIGN §4).  Where the MN-major operand of a single-pass TF32 product is small against the work it
+# feeds (the grouped output Linear's Wo, the token-row Linear weights, the attractor-side keys and the value bank V'),
+# it is transposed once into a K-major copy (rows padded to 16 bytes for TMA); the product reads the same values, so the
+# result keeps its bits.  bf16 products use wgmma's transpose bits and tf32x3 products read contiguous split copies:
+# neither needs this.  SEGTRAN_KMAJOR_COPIES=0 (or set_kmajor_copies(False)) keeps the MN-major operands, to time the
+# two paths against each other.
+_KMAJOR_COPIES = os.environ.get("SEGTRAN_KMAJOR_COPIES", "1") != "0"
+
+
+def set_kmajor_copies(on: bool):
+    global _KMAJOR_COPIES
+    _KMAJOR_COPIES = bool(on)
+
+
+def _kmajor_copies(tag: str = "big") -> bool:
+    return _KMAJOR_COPIES and _PRECISION == "tf32" and not _three_pass(tag)
+
+
+def _transposed(x: torch.Tensor, Z: int, R: int, Cd: int) -> torch.Tensor:
+    """x holding [Z, R, Cd] densely -> new [Z, Cd, R] view with the row pitch padded to pad4(R) (sx_transpose)."""
+    x = x.contiguous()
+    y = _rowpad_empty((Z, Cd, R), x.device)
+    L.call("sx_transpose", x.data_ptr(), Z, R, Cd, y.stride(1), y.data_ptr(), _stream())
+    return y
+
+
+def _bank_operand(v: torch.Tensor, B: int, U2: int, M: int, Fd: int) -> torch.Tensor:
+    """The [B, M, Fd, U2] "N x K" operand of U[b,m] = P[b,m] V[b,:,m] for a value bank v [B, U2, M*Fd] (also the
+    keys of dQ = dS K): a K-major copy, or the MN-major view of v when the copies are off."""
+    if _kmajor_copies():
+        return _transposed(v, B, U2, M * Fd).unflatten(1, (M, Fd))
+    return v.view(B, U2, M, Fd).permute(0, 2, 3, 1)
+
+
+def _weight_t(Wr: torch.Tensor, Z: int, O: int, I: int) -> torch.Tensor:
+    """[Z, I, O] transpose of the TF32-rounded weights Wr [Z, O, I], the "N x K" operand of dX = dY W: a K-major copy,
+    or the MN-major view of Wr when the copies are off."""
+    if _kmajor_copies():
+        return _transposed(Wr, Z, O, I)
+    return Wr.reshape(Z, O, I).transpose(-1, -2)
+
+
 def colsum(x2d: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out[c] += sum_r x2d[r, c] (rows uniformly strided)."""
     if out is None:
@@ -580,7 +625,7 @@ class _Linear(torch.autograd.Function):
             dy2 = dh
         dx = dW = db = None
         if ctx.needs_input_grad[0]:
-            dx = gemm_nt(dy2, Wr.t(), round_out=False).view(shp)
+            dx = gemm_nt(dy2, _weight_t(Wr, 1, *Wr.shape)[0], round_out=False).view(shp)
         if ctx.needs_input_grad[1]:
             tgt = _grad_target(W)
             if tgt is not None:
@@ -995,7 +1040,7 @@ class _FoldedValueBank(torch.autograd.Function):
             d2 = d2.contiguous()
         da = dWv = dWm = None
         if ctx.needs_input_grad[0]:
-            da = gemm_nt(d2, Wf.view(M * Fd, Cd).t(), round_out=False)[0, 0].view(B, A, Cd)
+            da = gemm_nt(d2, _weight_t(Wf, 1, M * Fd, Cd)[0], round_out=False)[0, 0].view(B, A, Cd)
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             dWf = gemm_nt(d2.t(), a2.t(), round_out=False).view(M, 1, Fd, Cd)          # [m, o, c]
             if ctx.needs_input_grad[2]:                               # dWm[o,f] = sum_m dW'_m[o,:] . Wv_m[f,:]
@@ -1032,10 +1077,9 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
         B, _, U1, U2 = P.shape
         Fd = v.shape[-1] // M
         P = _rowpad(P)
-        vv = v.view(B, U2, M, Fd).permute(0, 2, 3, 1)
         G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
         H = torch.empty_like(G)
-        gemm_nt(P, vv, out=G, bias=bm, gelu=True, preact=H, drop_p=drop_p, seed=seed)
+        gemm_nt(P, _bank_operand(v, B, U2, M, Fd), out=G, bias=bm, gelu=True, preact=H, drop_p=drop_p, seed=seed)
         Wr = round_tf32(Wo).reshape(M, Fd, Fd)
         Y = torch.empty_like(G)
         gemm_nt(G, Wr.unsqueeze(0), out=Y, bias=bo.reshape(1, M, Fd), round_out=False)
@@ -1061,7 +1105,7 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
             tgt = _grad_target(bm)
             dbm_buf = tgt if tgt is not None else _zeros((Fd,), dY.device)
             dbm = None if tgt is not None else dbm_buf
-        gemm_nt(dY, Wr.transpose(-1, -2).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=ctx.seed, colsum=dbm_buf)
+        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=ctx.seed, colsum=dbm_buf)
         if ctx.needs_input_grad[6]:
             tgt = _grad_target(Wo)
             if tgt is not None:
@@ -1126,10 +1170,9 @@ class _SqueezeOutFused(torch.autograd.Function):
         need_bwd = any(ctx.needs_input_grad)
         pb = PosBias(table, pb_geom[0], pb_geom[1], pb_geom[2]) if table is not None else None
         P, S, lse, _rowmax, stat = attn_probs_fused(q, k, M, clip, att_p, att_seed, diag, need_scores=need_bwd, posbias=pb)
-        vv = vp.view(B, U2, M, Fd).permute(0, 2, 3, 1)
         G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
         H = torch.empty_like(G)
-        gemm_nt(P, vv, out=G, bias=bm, gelu=True, preact=H, drop_p=hid_p, seed=hid_seed)
+        gemm_nt(P, _bank_operand(vp, B, U2, M, Fd), out=G, bias=bm, gelu=True, preact=H, drop_p=hid_p, seed=hid_seed)
         Wr = round_tf32(Wo).reshape(M, Fd, Fd)
         Y = torch.empty_like(G)
         gemm_nt(G, Wr.unsqueeze(0), out=Y, bias=bo.reshape(1, M, Fd), round_out=False)
@@ -1159,7 +1202,7 @@ class _SqueezeOutFused(torch.autograd.Function):
             tgt = _grad_target(bm)
             dbm_buf = tgt if tgt is not None else _zeros((Fd,), dY.device)
             dbm = None if tgt is not None else dbm_buf
-        gemm_nt(dY, Wr.transpose(-1, -2).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=hid_p, seed=hid_seed, colsum=dbm_buf)
+        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=hid_p, seed=hid_seed, colsum=dbm_buf)
         if ctx.needs_input_grad[10]:
             tgt = _grad_target(Wo)
             if tgt is not None:
@@ -1191,7 +1234,7 @@ class _SqueezeOutFused(torch.autograd.Function):
             if ctx.needs_input_grad[0]:
                 bcast = Bq == 1 and B > 1
                 dq = _zeros_like(q) if bcast else torch.empty_like(q)
-                gemm_nt(dS, k.view(B, U2, M, d).permute(0, 2, 3, 1), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3),
+                gemm_nt(dS, _bank_operand(k, B, U2, M, d), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3),
                         alpha=scale, round_out=False, reduce_z1=bcast, split_k=1)
             if ctx.needs_input_grad[1]:
                 dk = torch.empty_like(k)
@@ -1263,7 +1306,7 @@ class _GroupLinear(torch.autograd.Function):
         dY = dY.contiguous()
         dG = dW = db = None
         if ctx.needs_input_grad[0]:
-            dG = gemm_nt(dY, Wr.transpose(-1, -2).unsqueeze(0), round_out=False)
+            dG = gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), round_out=False)
         Wo, bo = ctx.leaves
         if ctx.needs_input_grad[1]:
             tgt = _grad_target(Wo)
@@ -1438,7 +1481,7 @@ class _Transpose(torch.autograd.Function):
         x = x.contiguous()
         Z, R, Cd = x.shape
         y = torch.empty((Z, Cd, R), device=x.device, dtype=torch.float32)
-        L.call("sx_transpose", x.data_ptr(), Z, R, Cd, y.data_ptr(), _stream())
+        L.call("sx_transpose", x.data_ptr(), Z, R, Cd, R, y.data_ptr(), _stream())
         return y
 
     @staticmethod
@@ -2222,7 +2265,7 @@ def _consist_pack(x3: torch.Tensor, transpose_in: bool, rnd: int) -> torch.Tenso
     if Ap == A and x3.is_contiguous():
         out = torch.empty((B, N, A), device=x3.device, dtype=torch.float32)
         if transpose_in:
-            L.call("sx_transpose", x3.data_ptr(), B, A, N, out.data_ptr(), _stream())
+            L.call("sx_transpose", x3.data_ptr(), B, A, N, A, out.data_ptr(), _stream())
             src = out
         else:
             src = x3
