@@ -472,6 +472,29 @@ int sx_sw_accumulate(const float* scores, int32_t K, int32_t dx, int32_t dy, int
                      int32_t H, int32_t W, int32_t D, int32_t x0, int32_t y0, int32_t z0, void* stream);
 int sx_sw_finalize(float* preds, const float* cnt, int32_t K, int64_t V, int32_t brats, float* hard, void* stream);
 
+/* -------------------------------------------------------------------------------------------
+ * Evaluation metrics of a case (csrc/sx_metrics.cu; code/test_util3d.py:186-215 calculate_metric_percase and medpy 0.4's
+ * dc / jc / asd / assd / hd / hd95 with unit voxel spacing and connectivity 1).  The classes of a case are the leading
+ * index of [K][n0][n1][n2] uint8 masks (non-zero = foreground, n2 contiguous; a 2-D mask has n0 = 1), so a case costs
+ * the same launches for any K.  Distances are exact: every one is sqrt of an integer squared distance d2, and the
+ * statistics are read from integer histograms over d2 (bins 0 .. sum (n_i - 1)^2).
+ * sx_mask_counts: counts[k*ldc + {0,1,2,3}] = |A|, |B|, |A and B|, |A or B| of class k (int64; written).
+ * sx_surface: border = X and not erode(X), the erosion with the 2*ndim axis neighbours and a background outside the volume.
+ * sx_edt_sq: dist[k][v] = the squared Euclidean distance from voxel v to the nearest non-zero voxel of border[k] (int32;
+ *   2^28 when border[k] is empty).  Extents in [1, 4096] with sum (n_i - 1)^2 < 2^26.
+ * sx_surface_hist: hist[k*ldh + d2] = the number of non-zero voxels of src_border[k] with dist d2 (uint32; written).
+ * sx_surface_stats: hist[k*ldh + {0, nbins}] are the histograms of the two directions of class k (A's border on B's
+ *   transform, then B's on A's); out[k*ldo + 0..7] (fp64) = n of each direction, the mean distance of each (asd, 0 when
+ *   empty), the maximum of each, numpy's linear 95th percentile over both directions together (hd95), and n of both.
+ *   The mean's fp64 sum has one fixed order: two runs give the same bits.
+ * ------------------------------------------------------------------------------------------- */
+int sx_mask_counts(const uint8_t* A, const uint8_t* B, int32_t K, int64_t V, int64_t* counts, int64_t ldc, void* stream);
+int sx_surface(const uint8_t* X, int32_t K, int32_t ndim, int32_t n0, int32_t n1, int32_t n2, uint8_t* border, void* stream);
+int sx_edt_sq(const uint8_t* border, int32_t K, int32_t n0, int32_t n1, int32_t n2, int32_t* dist, void* stream);
+int sx_surface_hist(const uint8_t* src_border, const int32_t* dist, int32_t K, int64_t V, int32_t nbins, uint32_t* hist,
+                    int64_t ldh, void* stream);
+int sx_surface_stats(const uint32_t* hist, int32_t K, int32_t nbins, int64_t ldh, double* out, int64_t ldo, void* stream);
+
 /* debug knobs for bring-up (descriptor field overrides); not part of the stable ABI */
 int sx_gemm_debug_set(const char* key, int64_t value);
 

@@ -106,6 +106,11 @@ _PROTOS = {
     "sx_convert": [_P, _I, _L, _P, _I, _I, _P],
     "sx_sw_accumulate": [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "sx_sw_finalize": [_P, _P, _I, _L, _I, _P, _P],
+    "sx_mask_counts": [_P, _P, _I, _L, _P, _L, _P],
+    "sx_surface": [_P, _I, _I, _I, _I, _I, _P, _P],
+    "sx_edt_sq": [_P, _I, _I, _I, _I, _P, _P],
+    "sx_surface_hist": [_P, _P, _I, _L, _I, _P, _L, _P],
+    "sx_surface_stats": [_P, _I, _I, _L, _P, _L, _P],
     "sx_split_tf32": [_P, _L, _P, _P, _P],
     "sx_split_tf32_cat": [_P, _I, _I, _I, _I, _L, _L, _L, _L, _I, _I, _P, _P],
     "sx_colsum": [_P, _I, _L, _I, _L, _P, _P, _L, _P],
@@ -167,7 +172,7 @@ def check(rc, what):
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
 _LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
              "sx_attn_probs_fwd": 2, "sx_colsum": 2, "sx_colsum_batched": 2,
-             "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2, "sx_head_dropout_bwd": 2}
+             "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2, "sx_head_dropout_bwd": 2, "sx_edt_sq": 3}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing
 
