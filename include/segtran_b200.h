@@ -91,9 +91,6 @@ typedef struct {
   const uint64_t* drop_seed_dev; /* optional device seed added to drop_seed (CUDA-graph safe) */
   const float* addend;           /* optional fp32 tensor in C's layout: C = epilogue(alpha*A.B^T + addend); used by the
                                     error-compensated 3-pass TF32 mode (A_hi B_hi + A_lo B_hi + A_hi B_lo) */
-  float* colsum;                 /* optional [N] fp32: += column sums of the stored values over all rows and batch slices
-                                    (a bias gradient that would otherwise need its own pass over the output; float atomics,
-                                    so the order of the additions varies: sx_colsum on the output is the ordered form) */
   float* part;                   /* split_k > 1: scratch for the partial tiles (summed in split order); split_k is lowered
                                     to what part_floats holds (128*128 floats per output tile and split), to 1 if NULL */
   int64_t part_floats;
@@ -229,8 +226,7 @@ int sx_seed_derive(const uint64_t* base, uint64_t add, uint64_t* out, void* stre
 int sx_seed_advance(uint64_t* base, uint64_t inc, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Row-wise kernels (HBM-bound).  "act dtype" arguments are SX_F32 | SX_BF16; round_tf32 rounds fp32
- * outputs that feed a TF32 GEMM.  Dropout masks are counter-based: keep(i) = hash(seed, flat index)
+ * Row-wise kernels (HBM-bound), fp32 in and out; round_tf32 rounds outputs that feed a TF32 GEMM.  Dropout masks are counter-based: keep(i) = hash(seed, flat index)
  * >= p, so backward regenerates the forward mask from (seed, index) instead of storing it.
  * ------------------------------------------------------------------------------------------- */
 
@@ -251,8 +247,8 @@ int sx_pos_lsinu_bwd(const float* pos, const float* posmax, int64_t R, int32_t p
  * pe == NULL (pos_code_type 'bias' / 'none', :940): h = mask * dropout( LN_{g,b}(x) ), no second LayerNorm; C0,
  *   pe_bstride and posw are ignored, stats[r] = {mean, rstd, 0, 1} of x's row, and the backward takes dpe == NULL. */
 int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, const float* g, const float* b, const float* pe,
-                    int32_t C0, int64_t pe_bstride, float posw, const float* mask, float drop_p, uint64_t seed, const uint64_t* seed_dev, void* h,
-                    int32_t h_dtype, int32_t round_tf32, float* stats, void* stream);
+                    int32_t C0, int64_t pe_bstride, float posw, const float* mask, float drop_p, uint64_t seed, const uint64_t* seed_dev, float* h,
+                    int32_t round_tf32, float* stats, void* stream);
 /* dh fp32 -> dx [B,N,C]; dg, db [C] and dpe (same addressing as pe, may be NULL) are accumulated (+=). */
 int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32_t N, int32_t C, const float* g, const float* b,
                     const float* pe, int32_t C0, int64_t pe_bstride, float posw, const float* mask, float drop_p,
@@ -265,11 +261,11 @@ int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32_t N, int32
  *   diag (optional, device float[2]): [0] = running max of *amax, [1] += 1 when the clamp fired — the module's
  *   max_attn / clamp_count counters (:575-587) without the reference's two .item() host syncs per call. */
 int sx_softmax_fwd(const float* S, int64_t R, int32_t L, int64_t lds, const float* amax, float clip, float drop_p,
-                   uint64_t seed, const uint64_t* seed_dev, void* P, int32_t p_dtype, int64_t ldp, int32_t round_tf32, float* lse, float* diag,
+                   uint64_t seed, const uint64_t* seed_dev, float* P, int64_t ldp, int32_t round_tf32, float* lse, float* diag,
                    void* stream);
 int sx_softmax_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, const float* lse, int64_t R, int32_t L,
-                   const float* amax, float clip, float drop_p, uint64_t seed, const uint64_t* seed_dev, int64_t ldp_fwd, void* dS,
-                   int32_t ds_dtype, int64_t ldo, int32_t round_tf32, void* stream);
+                   const float* amax, float clip, float drop_p, uint64_t seed, const uint64_t* seed_dev, int64_t ldp_fwd, float* dS,
+                   int64_t ldo, int32_t round_tf32, void* stream);
 /* The same with a sliding-window positional bias (segtran_shared.py:578-605): row r is query token r % L of a
  * self-attention (L == the grid's cell count, posbias->table != NULL):
  *   S' = clamp_if(S) + bias(q, .);  P = dropout(softmax(S')),  lse = log-sum-exp of S'.
@@ -278,18 +274,18 @@ int sx_softmax_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, co
  * clamp mask, so clamped elements still feed the table.  dtable [(2R+1)^pd] is accumulated in a fixed order through
  * `part` (no float atomics). */
 int sx_softmax_posbias_fwd(const float* S, int64_t R, int32_t L, int64_t lds, const float* amax, float clip, float drop_p,
-                           uint64_t seed, const uint64_t* seed_dev, void* P, int32_t p_dtype, int64_t ldp, int32_t round_tf32,
+                           uint64_t seed, const uint64_t* seed_dev, float* P, int64_t ldp, int32_t round_tf32,
                            float* lse, float* diag, const sx_posbias* posbias, void* stream);
 int sx_softmax_posbias_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, const float* lse, int64_t R, int32_t L,
                            const float* amax, float clip, float drop_p, uint64_t seed, const uint64_t* seed_dev, int64_t ldp_fwd,
-                           void* dS, int32_t ds_dtype, int64_t ldo, int32_t round_tf32, const sx_posbias* posbias,
+                           float* dS, int64_t ldo, int32_t round_tf32, const sx_posbias* posbias,
                            float* dtable, float* part, int64_t part_floats, void* stream);
 
 /* LayerNorm with affine over rows, eps 1e-12 (first_norm_layer, segtran_shared.py:456).  stats [R,2]. */
-int sx_layernorm_fwd(const float* x, int64_t R, int32_t C, const float* g, const float* b, void* y, int32_t y_dtype,
+int sx_layernorm_fwd(const float* x, int64_t R, int32_t C, const float* g, const float* b, float* y,
                      int32_t round_tf32, float* stats, void* stream);
 int sx_layernorm_bwd(const float* dy, const float* x, int64_t R, int32_t C, const float* g, const float* stats,
-                     void* dx, int32_t dx_dtype, int32_t round_tf32, float* dg, float* db, float* part, int64_t part_floats, void* stream);
+                     float* dx, int32_t round_tf32, float* dg, float* db, float* part, int64_t part_floats, void* stream);
 
 /* MMPrivateOutput tail + LearnedSoftAggregate (segtran_shared.py:273-274, :318-325):
  *   Yn = LN_{g,b}(dropout(Y));  w = softmax_modes(Yn.ws + bs);  out = sum_m w_m Yn_m
@@ -299,8 +295,8 @@ int sx_ln_softaggr_fwd(const float* Y, int32_t B, int32_t M, int32_t N, int32_t 
                        float* wts, void* stream);
 int sx_ln_softaggr_bwd(const float* dout, const float* Y, int32_t B, int32_t M, int32_t N, int32_t F, const float* g,
                        const float* b, const float* ws, float drop_p, uint64_t seed, const uint64_t* seed_dev, const float* stats,
-                       const float* wts, void* dY, int32_t dy_dtype, int32_t round_tf32, float* dg, float* db,
-                       float* dws, float* dbs, float* dscore_scratch /* [B*M*N] or NULL */, float* part, int64_t part_floats, void* stream);
+                       const float* wts, float* dY, int32_t round_tf32, float* dg, float* db,
+                       float* dws, float* dbs, float* part, int64_t part_floats, void* stream);
 
 /* LearnedSoftAggregate on its own (segtran_shared.py:318-325; the no-FFN branch :453 with M modes — the Polyformer layer):
  *   w = softmax_modes(x_m . ws + bs);  out = sum_m w_m x_m.   x [B,M,N,F] -> out [B,N,F], wts [B,M,N].
@@ -310,8 +306,8 @@ int sx_softaggr_fwd(const float* x, int32_t B, int32_t M, int32_t N, int32_t F, 
 int sx_softaggr_bwd(const float* dout, const float* x, int32_t B, int32_t M, int32_t N, int32_t F, const float* ws,
                     const float* wts, float* dx, float* dscore, void* stream);
 /* dH = dropout'(dG) * gelu'(H)  (MMSharedMid backward, segtran_shared.py:243-245) */
-int sx_gelu_bwd(const float* dG, const void* H, int32_t h_dtype, int64_t n, float drop_p, uint64_t seed, const uint64_t* seed_dev, void* dH,
-                int32_t dh_dtype, int32_t round_tf32, void* stream);
+int sx_gelu_bwd(const float* dG, const float* H, int64_t n, float drop_p, uint64_t seed, const uint64_t* seed_dev, float* dH,
+                int32_t round_tf32, void* stream);
 /* dtype conversion / TF32 rounding of a flat buffer (weights once per step) */
 int sx_convert(const void* x, int32_t x_dtype, int64_t n, void* y, int32_t y_dtype, int32_t round_tf32, void* stream);
 /* hi = TF32(x), lo = TF32(x - hi) over a flat fp32 buffer: operand split of the 3-pass error-compensated TF32 products
@@ -322,12 +318,11 @@ int sx_split_tf32(const float* x, int64_t n, float* hi, float* lo, void* stream)
  * sx_gemm launch over K' = 3*Kp on the two outputs is the 3-pass product A_hi B_hi^T + A_lo B_hi^T + A_hi B_lo^T */
 int sx_split_tf32_cat(const float* x, int32_t Z1, int32_t Z0, int32_t R, int32_t K, int64_t sz1, int64_t sz0, int64_t sr,
                       int64_t sk, int32_t Kp, int32_t role, float* out, void* stream);
-/* out[c] += sum_r X[r,c]   (bias gradients) */
-int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, int64_t ld, float* out, float* part, int64_t part_floats, void* stream);
 /* out[0] += sum_i x[i]*y[i]  and  y = alpha * (*alpha_dev) * x : a linear loss head for benchmarks / checksums */
-int sx_dot(const float* x, const float* y, int64_t n, float* out, void* stream);
+int sx_dot(const float* x, const float* y, int64_t n, float* out, float* part, int64_t part_floats, void* stream);
 int sx_scale(const float* x, int64_t n, const float* alpha_dev, float alpha, float* y, void* stream);
-/* out[z0][c] += sum_{z1,r} X[z1][z0][r][c]  (per-mode bias gradient of MMPrivateOutput in one launch) */
+/* out[z0][c] += sum_{z1,r} X[z1][z0][r][c]  (bias gradients; Z1 = Z0 = 1 for a plain column sum, Z0 = modes for the
+   per-mode bias gradient of MMPrivateOutput in one launch) */
 int sx_colsum_batched(const float* X, int32_t Z1, int64_t stride_z1, int32_t Z0, int64_t stride_z0, int64_t R, int32_t C,
                       int64_t ld, float* out, float* part, int64_t part_floats, void* stream);
 /* y = a + b  (residual connection of MMSharedOutput, segtran_shared.py:305) */
@@ -348,7 +343,7 @@ int sx_head_contract_fwd(const float* curr, const float* W, const float* bias, i
 int sx_head_contract_bwd_data(const float* dL, const float* W, int32_t B, int32_t Cf, int64_t V, int32_t K,
                               float* dcurr, void* stream);
 int sx_head_contract_bwd_weight(const float* dL, const float* curr, int32_t B, int32_t Cf, int64_t V, int32_t K,
-                                float* dW, void* stream);
+                                float* dW, float* part, int64_t part_floats, void* stream);
 /* class scores of the fused tokens, exact fp32: out[b,k,n] = sum_f W[k,f] vf[b,n,f]   (Wc . vfeat_fused) */
 int sx_token_scores(const float* vf, const float* W, int32_t B, int32_t N, int32_t F, int32_t K, float* out,
                     void* stream);

@@ -37,7 +37,7 @@ class sx_gemm_args(C.Structure):
                 ("alpha", C.c_float), ("bias_mode", C.c_int32), ("bias", C.c_void_p), ("bias_stride_z0", C.c_int64),
                 ("bias_stride_z1", C.c_int64), ("act", C.c_int32), ("accumulate", C.c_int32), ("preact", C.c_void_p),
                 ("split_k", C.c_int32), ("_pad2", C.c_int32), ("amax", C.c_void_p), ("drop_p", C.c_float),
-                ("_pad3", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("addend", C.c_void_p), ("colsum", C.c_void_p),
+                ("_pad3", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("addend", C.c_void_p),
                 ("part", C.c_void_p), ("part_floats", C.c_int64)]
 
 
@@ -87,20 +87,20 @@ _PROTOS = {
     "sx_reduce_max": [_P, _L, _P, _P],
     "sx_pos_lsinu_fwd": [_P, _P, _L, _I, _P, _P, _I, _P, _P],
     "sx_pos_lsinu_bwd": [_P, _P, _L, _I, _P, _P, _I, _P, _P, _P, _P, _P, _L, _P],
-    "sx_prologue_fwd": [_P, _L, _I, _I, _P, _P, _P, _I, _L, _F, _P, _F, _U64, _P, _P, _I, _I, _P, _P],
+    "sx_prologue_fwd": [_P, _L, _I, _I, _P, _P, _P, _I, _L, _F, _P, _F, _U64, _P, _P, _I, _P, _P],
     "sx_prologue_bwd": [_P, _P, _L, _I, _I, _P, _P, _P, _I, _L, _F, _P, _F, _U64, _P, _P, _P, _P, _P, _P, _P, _P, _L, _P],
-    "sx_softmax_fwd": [_P, _L, _I, _L, _P, _F, _F, _U64, _P, _P, _I, _L, _I, _P, _P, _P],
-    "sx_softmax_bwd": [_P, _L, _P, _L, _P, _L, _I, _P, _F, _F, _U64, _P, _L, _P, _I, _L, _I, _P],
-    "sx_softmax_posbias_fwd": [_P, _L, _I, _L, _P, _F, _F, _U64, _P, _P, _I, _L, _I, _P, _P, C.POINTER(sx_posbias), _P],
-    "sx_softmax_posbias_bwd": [_P, _L, _P, _L, _P, _L, _I, _P, _F, _F, _U64, _P, _L, _P, _I, _L, _I, C.POINTER(sx_posbias),
+    "sx_softmax_fwd": [_P, _L, _I, _L, _P, _F, _F, _U64, _P, _P, _L, _I, _P, _P, _P],
+    "sx_softmax_bwd": [_P, _L, _P, _L, _P, _L, _I, _P, _F, _F, _U64, _P, _L, _P, _L, _I, _P],
+    "sx_softmax_posbias_fwd": [_P, _L, _I, _L, _P, _F, _F, _U64, _P, _P, _L, _I, _P, _P, C.POINTER(sx_posbias), _P],
+    "sx_softmax_posbias_bwd": [_P, _L, _P, _L, _P, _L, _I, _P, _F, _F, _U64, _P, _L, _P, _L, _I, C.POINTER(sx_posbias),
                                _P, _P, _L, _P],
-    "sx_layernorm_fwd": [_P, _L, _I, _P, _P, _P, _I, _I, _P, _P],
-    "sx_layernorm_bwd": [_P, _P, _L, _I, _P, _P, _P, _I, _I, _P, _P, _P, _L, _P],
+    "sx_layernorm_fwd": [_P, _L, _I, _P, _P, _P, _I, _P, _P],
+    "sx_layernorm_bwd": [_P, _P, _L, _I, _P, _P, _P, _I, _P, _P, _P, _L, _P],
     "sx_ln_softaggr_fwd": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _F, _U64, _P, _P, _P, _P, _P],
-    "sx_ln_softaggr_bwd": [_P, _P, _I, _I, _I, _I, _P, _P, _P, _F, _U64, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _L, _P],
+    "sx_ln_softaggr_bwd": [_P, _P, _I, _I, _I, _I, _P, _P, _P, _F, _U64, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _L, _P],
     "sx_softaggr_fwd": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P],
     "sx_softaggr_bwd": [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P],
-    "sx_gelu_bwd": [_P, _P, _I, _L, _F, _U64, _P, _P, _I, _I, _P],
+    "sx_gelu_bwd": [_P, _P, _L, _F, _U64, _P, _P, _I, _P],
     "sx_seed_derive": [_P, _U64, _P, _P],
     "sx_seed_advance": [_P, _U64, _P],
     "sx_convert": [_P, _I, _L, _P, _I, _I, _P],
@@ -113,16 +113,15 @@ _PROTOS = {
     "sx_surface_stats": [_P, _I, _I, _L, _P, _L, _P],
     "sx_split_tf32": [_P, _L, _P, _P, _P],
     "sx_split_tf32_cat": [_P, _I, _I, _I, _I, _L, _L, _L, _L, _I, _I, _P, _P],
-    "sx_colsum": [_P, _I, _L, _I, _L, _P, _P, _L, _P],
     "sx_transpose": [_P, _L, _I, _I, _I, _P, _P],
     "sx_colsum_batched": [_P, _I, _L, _I, _L, _L, _I, _L, _P, _P, _L, _P],
-    "sx_dot": [_P, _P, _L, _P, _P],
+    "sx_dot": [_P, _P, _L, _P, _P, _L, _P],
     "sx_add": [_P, _P, _L, _P, _P],
     "sx_rowsum": [_P, _L, _L, _L, _I, _P, _P, _L, _P],
     "sx_scale": [_P, _L, _P, _F, _P, _P],
     "sx_head_contract_fwd": [_P, _P, _P, _I, _I, _L, _I, _P, _I, _P],
     "sx_head_contract_bwd_data": [_P, _P, _I, _I, _L, _I, _P, _P],
-    "sx_head_contract_bwd_weight": [_P, _P, _I, _I, _L, _I, _P, _P],
+    "sx_head_contract_bwd_weight": [_P, _P, _I, _I, _L, _I, _P, _P, _L, _P],
     "sx_head_dropout_fwd": [C.POINTER(sx_head_dropout_args), _P, _P],
     "sx_head_dropout_bwd": [C.POINTER(sx_head_dropout_args), _P, _P, _I, _P, _P],
     "sx_token_scores": [_P, _P, _I, _I, _I, _I, _P, _P],
@@ -171,7 +170,7 @@ def check(rc, what):
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
 _LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
-             "sx_attn_probs_fwd": 2, "sx_colsum": 2, "sx_colsum_batched": 2,
+             "sx_attn_probs_fwd": 2, "sx_colsum_batched": 2, "sx_dot": 2, "sx_head_contract_bwd_weight": 2,
              "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2, "sx_head_dropout_bwd": 2, "sx_edt_sq": 3}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing

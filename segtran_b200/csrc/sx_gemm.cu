@@ -69,7 +69,6 @@ struct GemmParams {
   unsigned long long drop_seed;
   const unsigned long long* drop_seed_dev;
   const float* addend;   // optional fp32 tensor in C's layout added to alpha*acc before bias/activation (tf32x3 passes)
-  float* colsum;         // optional [N]: += column sums of the stored values over all rows and batch slices (bias gradients)
   int stream_out;        // output larger than half the L2: store with evict-first (st.global.cs), keep operands (evict-last)
 };
 
@@ -456,32 +455,6 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int i = 0; i < 16; ++i) f[i] = sx::round_tf32(f[i]);
       }
-      if (p.colsum) {
-        // this thread's 8 columns (j, e), summed over its 2 rows, then over the 8 lanes that share the columns
-        float cs[8];
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            float a = 0.f;
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              if (row0 + 8 * h + tr < p.M) a += f[4 * j + 2 * h + e];
-            a += __shfl_xor_sync(0xffffffffu, a, 4);
-            a += __shfl_xor_sync(0xffffffffu, a, 8);
-            a += __shfl_xor_sync(0xffffffffu, a, 16);
-            cs[2 * j + e] = a;
-          }
-        if (tr == 0) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int col = col0 + 8 * j + tc + e;
-              if (col < p.N) atomicAdd(p.colsum + col, cs[2 * j + e]);
-            }
-        }
-      }
       if (p.amax) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
@@ -604,7 +577,6 @@ extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
   SX_REQUIRE(!a->round_tf32 || (!a->accumulate && p.split_k == 1),
              "sx_gemm: round_tf32 cannot be combined with accumulate / split_k > 1 (a sum of rounded partials is not a TF32 "
              "value): round the finished output instead");
-  SX_REQUIRE(p.split_k == 1 || !a->colsum, "sx_gemm: colsum needs split_k=1");
   const long long tt = (long long)p.tiles_m * p.tiles_n * p.split_k * a->Z0 * p.Z1;
   SX_REQUIRE(tt < (1ll << 30), "sx_gemm: too many tiles");
   p.total_tiles = (int)tt;
@@ -620,7 +592,6 @@ extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
   p.bias_sz0 = a->bias_stride_z0; p.bias_sz1 = a->bias_stride_z1;
   p.act = a->act; p.accumulate = a->accumulate; p.preact = a->preact; p.amax = a->amax;
   p.addend = a->addend;
-  p.colsum = a->colsum;
   SX_REQUIRE(a->act != SX_ACT_GELU_BWD || (a->preact && a->c_dtype == SX_F32 && p.split_k == 1 && !a->accumulate),
              "sx_gemm: SX_ACT_GELU_BWD needs the fp32 pre-activation in `preact`, fp32 C, split_k=1, accumulate=0");
   SX_REQUIRE(!a->addend || (p.split_k == 1 && !a->accumulate && a->c_dtype == SX_F32), "sx_gemm: addend needs split_k=1, accumulate=0, fp32 C");

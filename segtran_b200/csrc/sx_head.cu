@@ -9,13 +9,14 @@
 //
 //   head_contract_fwd        L[b,k,v]   = sum_c W[k,c] curr[b,c,v] + bias[k]          (reads curr)
 //   head_contract_bwd_data   dcurr[b,c,v] = sum_k W[k,c] dL[b,k,v]                    (writes dcurr)
-//   head_contract_bwd_weight dW[k,c]   += sum_{b,v} dL[b,k,v] curr[b,c,v]             (reads curr)
+//   head_contract_bwd_weight dW[k,c]   += sum_{b,v} dL[b,k,v] curr[b,c,v]             (reads curr; V % 4 != 0)
 //   resize_axis_fwd / _bwd   1-D linear resampling along one axis (align_corners=False), PyTorch semantics;
 //                            tri/bi-linear interpolation is applied as a sequence of axis passes.
 //   sgemm_small              strided fp32 GEMM on CUDA cores for the tiny class-dimension products.
 #include <cstdlib>
 
 #include "sx_common.cuh"
+#include "sx_part.cuh"
 #include "sx_resample.cuh"
 
 namespace {
@@ -104,10 +105,11 @@ head_contract_bwd_data_kernel(const float* __restrict__ dL, const float* __restr
   }
 }
 
-// one warp per channel; lanes stride over a voxel chunk; dW[k,c] += sum_v dL[k,v] curr[c,v]
+// one warp per channel; lanes stride over a voxel chunk; the (chunk, batch) CTA's sums dW[k,c] = sum_v dL[k,v] curr[c,v]
+// go to its slot (blockIdx.z * gridDim.y + blockIdx.y, [K * Cf]) of `part`
 __global__ void __launch_bounds__(256)
 head_contract_bwd_weight_kernel(const float* __restrict__ dL, const float* __restrict__ curr, int Cf, long long V,
-                                int K, long long chunk, float* __restrict__ dW) {
+                                int K, long long chunk, float* __restrict__ part) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = blockIdx.x * 8 + warp;
   const int b = blockIdx.z;
@@ -130,7 +132,7 @@ head_contract_bwd_weight_kernel(const float* __restrict__ dL, const float* __res
   for (int k = 0; k < MAXK; ++k)
     if (k < K) {
       const float s = sx::warp_sum(acc[k]);
-      if (lane == 0) atomicAdd(&dW[k * Cf + c], s);
+      if (lane == 0) part[((long long)blockIdx.z * gridDim.y + blockIdx.y) * K * Cf + k * Cf + c] = s;
     }
 }
 
@@ -506,15 +508,19 @@ extern "C" int sx_head_contract_bwd_data(const float* dL, const float* W, int32_
 }
 
 extern "C" int sx_head_contract_bwd_weight(const float* dL, const float* curr, int32_t B, int32_t Cf, int64_t V,
-                                           int32_t K, float* dW, void* stream) {
+                                           int32_t K, float* dW, float* part, int64_t part_floats, void* stream) {
   SX_REQUIRE(K >= 1 && K <= MAXK, "sx_head_contract_bwd_weight: num_classes %d not in 1..%d", K, MAXK);
+  // one slot per (chunk, batch) CTA: chunks of 8192 voxels, fewer and longer when the scratch or the grid runs short
+  const int max_chunks = std::min(part_slots(part_floats, (long long)K * Cf) / B, 65535);
+  SX_REQUIRE(part && max_chunks >= 1, "sx_head_contract_bwd_weight: needs at least %lld floats of scratch",
+             (long long)B * K * Cf);
   long long chunk = 8192;
   int chunks = sx_ceil_div(V, chunk);
-  if (chunks > 65535) { chunk = (V + 65534) / 65535; chunks = sx_ceil_div(V, chunk); }
+  if (chunks > max_chunks) { chunk = sx_ceil_div(V, max_chunks); chunks = sx_ceil_div(V, chunk); }
   dim3 grid(sx_ceil_div(Cf, 8), chunks, B);
-  head_contract_bwd_weight_kernel<<<grid, 256, 0, ST(stream)>>>(dL, curr, Cf, V, K, chunk, dW);
+  head_contract_bwd_weight_kernel<<<grid, 256, 0, ST(stream)>>>(dL, curr, Cf, V, K, chunk, part);
   SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return part_reduce(part, chunks * B, K * Cf, PartDst{{dW, nullptr, nullptr, nullptr}, {K * Cf, 0, 0, 0}}, ST(stream));
 }
 
 static int ew_grid(long long total) {

@@ -17,6 +17,7 @@
 #include <algorithm>
 
 #include "sx_common.cuh"
+#include "sx_part.cuh"
 #include "sx_resample.cuh"
 
 namespace {
@@ -226,15 +227,6 @@ head_dropout_bwd_kernel(DropGeom g, const float* __restrict__ Wc, int kc, const 
   }
 }
 
-// dWc[i] += sum of the slots' column i, in slot order (the ordered reduction of sx_rows.cu's part_reduce)
-__global__ void slot_reduce_kernel(const float* __restrict__ part, int slots, int n, float* __restrict__ dst) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    float s = 0.f;
-    for (int g = 0; g < slots; ++g) s += part[(long long)g * n + i];
-    dst[i] += s;
-  }
-}
-
 int check_args(const sx_head_dropout_args* a, const char* who) {
   SX_REQUIRE(a != nullptr && a->src && a->Wc, "%s: null pointer", who);
   SX_REQUIRE(a->B >= 1 && a->B <= 65535 && a->Fs >= 1 && a->Ds >= 1 && a->HW >= 1 && a->K >= 1 && a->Dk >= 1,
@@ -319,8 +311,9 @@ static int launch_bwd(const DropGeom& g, const sx_head_dropout_args* a, const fl
         g, a->Wc + (long long)c0 * g.Fo, kc, dLs + (long long)c0 * Vo, (long long)a->K * Vo, dsrc,
         (accumulate || c0 > 0) ? 1 : 0, a->part, tps, tiles);
     SX_CHECK_CUDA(cudaGetLastError());
-    slot_reduce_kernel<<<sx_ceil_div(kc * g.Fo, 256), 256, 0, st>>>(a->part, grid, kc * g.Fo, dWc + (long long)c0 * g.Fo);
-    SX_CHECK_CUDA(cudaGetLastError());
+    if (int rc = part_reduce(a->part, grid, kc * g.Fo,
+                             PartDst{{dWc + (long long)c0 * g.Fo, nullptr, nullptr, nullptr}, {kc * g.Fo, 0, 0, 0}}, st))
+      return rc;
   }
   return 0;
 }

@@ -5,6 +5,7 @@
 #include <algorithm>
 
 #include "sx_common.cuh"
+#include "sx_part.cuh"
 #include "sx_posbias.cuh"
 
 namespace {
@@ -12,33 +13,18 @@ namespace {
 constexpr int ROW_WARPS = 8;
 constexpr float LN_EPS = 1e-12f;     // every LayerNorm on the path (segtran_shared.py:263, :371, :885, :888, :984)
 
-// Deterministic cross-CTA sums.  A kernel whose CTAs each hold partial column sums stores them in its slot (= CTA index
-// along the reduced dimension) of the caller's scratch `part`, laid out [slot][stride]; part_reduce then adds the slots
-// in slot order into the destinations.  Float atomics would add them in whatever order the CTAs finish, and the
-// last-bit differences grow through TF32 rounding and the optimiser: two runs of the same step on the same inputs would
-// not agree.  The number of slots adapts to the scratch size (part_floats / stride).
+__device__ __forceinline__ float rnd1(float v, int rnd) { return rnd ? sx::round_tf32(v) : v; }
 
-struct PartDst {                                                 // slot row = concatenation of up to 4 destination arrays
-  float* p[4];
-  int n[4];
-};
-
-__global__ void part_reduce_kernel(const float* __restrict__ part, int slots, int stride, int total, PartDst d) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    int a = 0, c = i;
-    while (c >= d.n[a]) { c -= d.n[a]; ++a; }
-    float s = 0.f;
-    for (int g = 0; g < slots; ++g) s += part[(long long)g * stride + i];
-    if (d.p[a]) d.p[a][c] += s;
+// Adds the warps' accumulator rows (row pitch `pitch` floats, the first n of each) in warp order and stores the CTA's
+// sums in its slot (blockIdx.x, pitch n) of `part`: the fixed-order column sums of the warp-per-row backward kernels.
+__device__ __forceinline__ void warps_to_slot(const float* sm, int warps, long long pitch, int n, float* __restrict__ part) {
+  __syncthreads();
+  for (int c = threadIdx.x; c < n; c += blockDim.x) {
+    float v = 0.f;
+    for (int w = 0; w < warps; ++w) v += sm[w * pitch + c];
+    part[(long long)blockIdx.x * n + c] = v;
   }
 }
-
-template <typename T> __device__ __forceinline__ float ldf(const T* p);
-template <> __device__ __forceinline__ float ldf<float>(const float* p) { return *p; }
-template <> __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
-template <typename T> __device__ __forceinline__ void stf(T* p, float v, int rnd);
-template <> __device__ __forceinline__ void stf<float>(float* p, float v, int rnd) { *p = rnd ? sx::round_tf32(v) : v; }
-template <> __device__ __forceinline__ void stf<__nv_bfloat16>(__nv_bfloat16* p, float v, int) { *p = __float2bfloat16_rn(v); }
 
 __device__ __forceinline__ void warp_mean_rstd(const float* row, int C, int lane, float& mean, float& rstd) {
   float s = 0.f;
@@ -160,11 +146,10 @@ __global__ void pos_param_grad_kernel(const float* __restrict__ de, const float*
 // fused prologue (segtran_shared.py:916, :930-934, :944-946):
 //   h = mask * dropout( LN( LN_{g,b}(x) + posw * pe[:, :C] ) )
 // ------------------------------------------------------------------------------------------------
-template <typename T>
 __global__ void prologue_fwd_kernel(const float* __restrict__ x, long long R, int N, int C, const float* __restrict__ g,
                                     const float* __restrict__ b, const float* __restrict__ pe, int C0,
                                     long long pe_bstride, float posw, const float* __restrict__ mask, float drop_p,
-                                    unsigned long long seed, const unsigned long long* __restrict__ seed_dev, T* __restrict__ h, float* __restrict__ stats, int rnd) {
+                                    unsigned long long seed, const unsigned long long* __restrict__ seed_dev, float* __restrict__ h, float* __restrict__ stats, int rnd) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
   extern __shared__ float sm[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -183,11 +168,11 @@ __global__ void prologue_fwd_kernel(const float* __restrict__ x, long long R, in
     float m2, r2;
     warp_mean_rstd(row, C, lane, m2, r2);
     const float mk = mask ? mask[r] : 1.f;
-    T* hr = h + r * C;
+    float* hr = h + r * C;
     for (int c = lane; c < C; c += 32) {
       float v = (row[c] - m2) * r2 * mk;
       if (drop_p > 0.f) v = sx::drop_keep1(seed, (unsigned long long)(r * C + c), sx::drop_p16(drop_p)) ? v * keep_scale : 0.f;
-      stf<T>(hr + c, v, rnd);
+      hr[c] = rnd1(v, rnd);
     }
     if (lane == 0) {
       stats[r * 4 + 0] = m1; stats[r * 4 + 1] = r1; stats[r * 4 + 2] = m2; stats[r * 4 + 3] = r2;
@@ -196,26 +181,26 @@ __global__ void prologue_fwd_kernel(const float* __restrict__ x, long long R, in
   }
 }
 
-// backward of the fused prologue.  dh fp32 [R,C]; produces dx [R,C], and accumulates dg, db [C] and
-// dpe[(b*pe_bstride) + n*C0 + c] (atomicAdd: the positional code is shared over batch and layers).
+// backward of the fused prologue for the widths and views prologue_bwd_cta rejects.  dh fp32 [R,C] -> dx [R,C], and
+// dt [R,C] = the gradient at the inner LayerNorm's input, which pos_grad_from_dt reduces into dpe (dt_out may be NULL
+// when no dpe is wanted).  dg / db: one accumulator row per warp (a lane owns the columns c = lane mod 32), the warps
+// added in order into the CTA's slot of `part`, as in prologue_nopos_bwd_kernel.
 __global__ void prologue_bwd_kernel(const float* __restrict__ dh, const float* __restrict__ x, long long R, int N,
                                     int C, const float* __restrict__ g, const float* __restrict__ b,
                                     const float* __restrict__ pe, int C0, long long pe_bstride, float posw,
                                     const float* __restrict__ mask, float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
-                                    const float* __restrict__ stats, float* __restrict__ dx, float* __restrict__ dg,
-                                    float* __restrict__ db, float* __restrict__ dpe) {
+                                    const float* __restrict__ stats, float* __restrict__ dx, float* __restrict__ dt_out,
+                                    float* __restrict__ part) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* sdg = sm;                       // [C] block accumulators
-  float* sdb = sm + C;
-  float* y1 = sm + 2 * C + warp * 3 * C; // per warp: yhat1 [C], yhat2 [C], d [C]
+  const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* acc = sm + (long long)warp * 5 * C;  // per warp: dg [C], db [C], yhat1 [C], yhat2 [C], d [C]
+  float* y1 = acc + 2 * C;
   float* y2 = y1 + C;
   float* dd = y2 + C;
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) sm[c] = 0.f;
-  __syncthreads();
+  for (int c = lane; c < 2 * C; c += 32) acc[c] = 0.f;
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
-  for (long long r = (long long)blockIdx.x * ROW_WARPS + warp; r < R; r += (long long)gridDim.x * ROW_WARPS) {
+  for (long long r = (long long)blockIdx.x * warps + warp; r < R; r += (long long)gridDim.x * warps) {
     const float m1 = stats[r * 4 + 0], r1 = stats[r * 4 + 1], m2 = stats[r * 4 + 2], r2 = stats[r * 4 + 3];
     const long long bi = r / N, ni = r % N;
     const float* per = pe + bi * pe_bstride + ni * C0;
@@ -232,12 +217,11 @@ __global__ void prologue_bwd_kernel(const float* __restrict__ dh, const float* _
     }
     s1 = sx::warp_sum(s1) / C; s2 = sx::warp_sum(s2) / C;
     float s3 = 0.f, s4 = 0.f;
-    float* dper = dpe ? dpe + bi * pe_bstride + ni * C0 : nullptr;
     for (int c = lane; c < C; c += 32) {
       const float dt = r2 * (dd[c] - s1 - y2[c] * s2);
-      atomicAdd(&sdg[c], dt * y1[c]);
-      atomicAdd(&sdb[c], dt);
-      if (dper) atomicAdd(&dper[c], posw * dt);
+      acc[c] += dt * y1[c];
+      acc[C + c] += dt;
+      if (dt_out) dt_out[r * C + c] = dt;
       const float da = dt * g[c];
       dd[c] = da;
       s3 += da; s4 += da * y1[c];
@@ -246,21 +230,16 @@ __global__ void prologue_bwd_kernel(const float* __restrict__ dh, const float* _
     for (int c = lane; c < C; c += 32) dx[r * C + c] = r1 * (dd[c] - s3 - y1[c] * s4);
     __syncwarp();
   }
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    atomicAdd(&dg[c], sdg[c]);
-    atomicAdd(&db[c], sdb[c]);
-  }
+  warps_to_slot(sm, warps, 5ll * C, 2 * C, part);
 }
 
 // ------------------------------------------------------------------------------------------------
 // softmax over rows with the reference's conditional clamp (segtran_shared.py:578-580, :601-605)
 //   if (*amax > clip) S = clamp(S, -clip, clip);  P = softmax(S);  Pd = dropout(P)
 // ------------------------------------------------------------------------------------------------
-template <typename T>
 __global__ void softmax_fwd_kernel(const float* __restrict__ S, long long R, int L, long long lds,
                                    const float* __restrict__ amax, float clip, float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
-                                   T* __restrict__ P, long long ldp, float* __restrict__ lse, int rnd,
+                                   float* __restrict__ P, long long ldp, float* __restrict__ lse, int rnd,
                                    float* __restrict__ diag) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
   extern __shared__ float sm[];
@@ -287,11 +266,11 @@ __global__ void softmax_fwd_kernel(const float* __restrict__ S, long long R, int
     for (int c = lane; c < L; c += 32) { const float e = __expf(row[c] - m); row[c] = e; s += e; }
     s = sx::warp_sum(s);
     const float inv = 1.f / s;
-    T* pr = P + r * ldp;
+    float* pr = P + r * ldp;
     for (int c = lane; c < L; c += 32) {
       float v = row[c] * inv;
       if (drop_p > 0.f) v = sx::drop_keep1(seed, (unsigned long long)(r * ldp + c), sx::drop_p16(drop_p)) ? v * keep_scale : 0.f;
-      stf<T>(pr + c, v, rnd);
+      pr[c] = rnd1(v, rnd);
     }
     if (lane == 0 && lse) lse[r] = m + __logf(s);
     __syncwarp();
@@ -299,11 +278,10 @@ __global__ void softmax_fwd_kernel(const float* __restrict__ S, long long R, int
 }
 
 // dS = P * (g - sum_j P_j g_j) with g = dPd * keep/(1-p); zero where the clamp was active.
-template <typename T>
 __global__ void softmax_bwd_kernel(const float* __restrict__ dP, long long ldd, const float* __restrict__ S,
                                    long long lds, const float* __restrict__ lse, long long R, int L,
                                    const float* __restrict__ amax, float clip, float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
-                                   long long ldp_fwd, T* __restrict__ dS, long long ldo, int rnd) {
+                                   long long ldp_fwd, float* __restrict__ dS, long long ldo, int rnd) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
   extern __shared__ float sm[];
   const int warps = blockDim.x >> 5;
@@ -329,7 +307,7 @@ __global__ void softmax_bwd_kernel(const float* __restrict__ dP, long long ldd, 
     for (int c = lane; c < L; c += 32) {
       float d = prow[c] * (grow[c] - dot);
       if (do_clip) { const float v = S[r * lds + c]; if (v < -clip || v > clip) d = 0.f; }
-      stf<T>(dS + r * ldo + c, d, rnd);
+      dS[r * ldo + c] = rnd1(d, rnd);
     }
     __syncwarp();
   }
@@ -343,11 +321,10 @@ __global__ void softmax_bwd_kernel(const float* __restrict__ dP, long long ldd, 
 // ------------------------------------------------------------------------------------------------
 constexpr int NOPOS_WARPS = 4;
 
-template <typename T>
 __global__ void __launch_bounds__(NOPOS_WARPS * 32)
 prologue_nopos_fwd_kernel(const float* __restrict__ x, long long R, int C, const float* __restrict__ g,
                           const float* __restrict__ b, const float* __restrict__ mask, float drop_p, unsigned long long seed,
-                          const unsigned long long* __restrict__ seed_dev, T* __restrict__ h, float* __restrict__ stats, int rnd) {
+                          const unsigned long long* __restrict__ seed_dev, float* __restrict__ h, float* __restrict__ stats, int rnd) {
   seed += seed_dev ? *seed_dev : 0ull;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
@@ -356,11 +333,11 @@ prologue_nopos_fwd_kernel(const float* __restrict__ x, long long R, int C, const
     float m1, r1;
     warp_mean_rstd(xr, C, lane, m1, r1);
     const float mk = mask ? mask[r] : 1.f;
-    T* hr = h + r * C;
+    float* hr = h + r * C;
     for (int c = lane; c < C; c += 32) {
       float v = ((xr[c] - m1) * r1 * g[c] + b[c]) * mk;
       if (drop_p > 0.f) v = sx::drop_keep1(seed, (unsigned long long)(r * C + c), sx::drop_p16(drop_p)) ? v * keep_scale : 0.f;
-      stf<T>(hr + c, v, rnd);
+      hr[c] = rnd1(v, rnd);
     }
     if (lane == 0) {
       stats[r * 4 + 0] = m1; stats[r * 4 + 1] = r1; stats[r * 4 + 2] = 0.f; stats[r * 4 + 3] = 1.f;
@@ -403,12 +380,7 @@ prologue_nopos_bwd_kernel(const float* __restrict__ dh, const float* __restrict_
       dx[r * C + c] = r1 * (dy_at(c) * g[c] - s1 - xh * s2);
     }
   }
-  __syncthreads();
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) {
-    float v = 0.f;
-    for (int w = 0; w < NOPOS_WARPS; ++w) v += sm[(long long)w * 2 * C + c];
-    part[(long long)blockIdx.x * 2 * C + c] = v;
-  }
+  warps_to_slot(sm, NOPOS_WARPS, 2ll * C, 2 * C, part);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -456,11 +428,10 @@ __device__ __forceinline__ void posbias_stage_row(const float* __restrict__ sr, 
   __syncthreads();
 }
 
-template <typename T>
 __global__ void __launch_bounds__(PB_THREADS)
 softmax_posbias_fwd_kernel(const float* __restrict__ S, long long R, int L, long long lds, const float* __restrict__ amax,
                            float clip, float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
-                           T* __restrict__ P, long long ldp, float* __restrict__ lse, int rnd, float* __restrict__ diag,
+                           float* __restrict__ P, long long ldp, float* __restrict__ lse, int rnd, float* __restrict__ diag,
                            const float* __restrict__ table, const sxpb::Geom G) {
   seed += seed_dev ? *seed_dev : 0ull;
   extern __shared__ float sm[];
@@ -481,23 +452,22 @@ softmax_posbias_fwd_kernel(const float* __restrict__ S, long long R, int L, long
     for (int c = threadIdx.x; c < L; c += PB_THREADS) { const float e = __expf(row[c] - m); row[c] = e; s += e; }
     s = block_sum(s, red);
     const float inv = 1.f / s;
-    T* pr = P + r * ldp;
+    float* pr = P + r * ldp;
     for (int c = threadIdx.x; c < L; c += PB_THREADS) {
       float v = row[c] * inv;
       if (drop_p > 0.f) v = sx::drop_keep1(seed, (unsigned long long)(r * ldp + c), sx::drop_p16(drop_p)) ? v * keep_scale : 0.f;
-      stf<T>(pr + c, v, rnd);
+      pr[c] = rnd1(v, rnd);
     }
     if (threadIdx.x == 0 && lse) lse[r] = m + __logf(s);
     __syncthreads();
   }
 }
 
-template <typename T>
 __global__ void __launch_bounds__(PB_THREADS)
 softmax_posbias_bwd_kernel(const float* __restrict__ dP, long long ldd, const float* __restrict__ S, long long lds,
                            const float* __restrict__ lse, long long R, int L, const float* __restrict__ amax, float clip,
                            float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
-                           long long ldp_fwd, T* __restrict__ dS, long long ldo, int rnd, const float* __restrict__ table,
+                           long long ldp_fwd, float* __restrict__ dS, long long ldo, int rnd, const float* __restrict__ table,
                            const sxpb::Geom G, float* __restrict__ part) {
   seed += seed_dev ? *seed_dev : 0ull;
   extern __shared__ float sm[];
@@ -527,7 +497,7 @@ softmax_posbias_bwd_kernel(const float* __restrict__ dP, long long ldd, const fl
       grow[c] = d;
       float o = d;
       if (do_clip) { const float v = S[r * lds + c]; if (v < -clip || v > clip) o = 0.f; }
-      stf<T>(dS + r * ldo + c, o, rnd);
+      dS[r * ldo + c] = rnd1(o, rnd);
     }
     __syncthreads();
     int qc[3];
@@ -544,9 +514,8 @@ softmax_posbias_bwd_kernel(const float* __restrict__ dP, long long ldd, const fl
 // ------------------------------------------------------------------------------------------------
 // LayerNorm with affine over rows (first_norm_layer, segtran_shared.py:456)
 // ------------------------------------------------------------------------------------------------
-template <typename T>
 __global__ void layernorm_fwd_kernel(const float* __restrict__ x, long long R, int C, const float* __restrict__ g,
-                                     const float* __restrict__ b, T* __restrict__ y, float* __restrict__ stats,
+                                     const float* __restrict__ b, float* __restrict__ y, float* __restrict__ stats,
                                      int rnd) {
   extern __shared__ float sm[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -556,44 +525,39 @@ __global__ void layernorm_fwd_kernel(const float* __restrict__ x, long long R, i
     __syncwarp();
     float m, rs;
     warp_mean_rstd(row, C, lane, m, rs);
-    for (int c = lane; c < C; c += 32) stf<T>(y + r * C + c, (row[c] - m) * rs * g[c] + b[c], rnd);
+    for (int c = lane; c < C; c += 32) y[r * C + c] = rnd1((row[c] - m) * rs * g[c] + b[c], rnd);
     if (lane == 0) { stats[r * 2] = m; stats[r * 2 + 1] = rs; }
     __syncwarp();
   }
 }
 
-template <typename T>
+// backward for the widths and views layernorm_bwd_rows_fast rejects: per-warp dg | db rows, added in warp order into
+// the CTA's slot of `part`
 __global__ void layernorm_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, long long R, int C,
-                                     const float* __restrict__ g, const float* __restrict__ stats, T* __restrict__ dx,
-                                     float* __restrict__ dg, float* __restrict__ db, int rnd) {
+                                     const float* __restrict__ g, const float* __restrict__ stats, float* __restrict__ dx,
+                                     float* __restrict__ part, int rnd) {
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* sdg = sm;
-  float* sdb = sm + C;
-  float* yh = sm + 2 * C + warp * 2 * C;
+  const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* acc = sm + (long long)warp * 4 * C;  // per warp: dg [C], db [C], yhat [C], d [C]
+  float* yh = acc + 2 * C;
   float* dd = yh + C;
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) sm[c] = 0.f;
-  __syncthreads();
-  for (long long r = (long long)blockIdx.x * ROW_WARPS + warp; r < R; r += (long long)gridDim.x * ROW_WARPS) {
+  for (int c = lane; c < 2 * C; c += 32) acc[c] = 0.f;
+  for (long long r = (long long)blockIdx.x * warps + warp; r < R; r += (long long)gridDim.x * warps) {
     const float m = stats[r * 2], rs = stats[r * 2 + 1];
     float s1 = 0.f, s2 = 0.f;
     for (int c = lane; c < C; c += 32) {
       const float a = (x[r * C + c] - m) * rs, d0 = dy[r * C + c];
-      atomicAdd(&sdg[c], d0 * a);
-      atomicAdd(&sdb[c], d0);
+      acc[c] += d0 * a;
+      acc[C + c] += d0;
       const float d = d0 * g[c];
       yh[c] = a; dd[c] = d;
       s1 += d; s2 += d * a;
     }
     s1 = sx::warp_sum(s1) / C; s2 = sx::warp_sum(s2) / C;
-    for (int c = lane; c < C; c += 32) stf<T>(dx + r * C + c, rs * (dd[c] - s1 - yh[c] * s2), rnd);
+    for (int c = lane; c < C; c += 32) dx[r * C + c] = rnd1(rs * (dd[c] - s1 - yh[c] * s2), rnd);
     __syncwarp();
   }
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    atomicAdd(&dg[c], sdg[c]);
-    atomicAdd(&db[c], sdb[c]);
-  }
+  warps_to_slot(sm, warps, 4ll * C, 2 * C, part);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -610,11 +574,11 @@ __global__ void ln_softaggr_fwd_kernel(const float* __restrict__ Y, int B, int M
                                        float* __restrict__ wts) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* rows = sm + (long long)warp * M * F;       // normalised rows of the M modes
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   const long long T_ = (long long)B * N;
-  for (long long t = (long long)blockIdx.x * ROW_WARPS + warp; t < T_; t += (long long)gridDim.x * ROW_WARPS) {
+  for (long long t = (long long)blockIdx.x * warps + warp; t < T_; t += (long long)gridDim.x * warps) {
     const long long bi = t / N, ni = t % N;
     float sc[MAX_MODES];
     for (int m = 0; m < M; ++m) {
@@ -656,28 +620,26 @@ __global__ void ln_softaggr_fwd_kernel(const float* __restrict__ Y, int B, int M
   }
 }
 
-// backward: dout [B,N,F] -> dY [B,M,N,F] (T), plus dg, db, dws [F], dbs [1] (atomic accumulation).
-template <typename T>
+// backward: dout [B,N,F] -> dY [B,M,N,F], plus dg, db, dws [F] and dbs [1]: per-warp rows [dg | db | dws | dbs], added
+// in warp order into the CTA's slot of `part`
 __global__ void ln_softaggr_bwd_kernel(const float* __restrict__ dout, const float* __restrict__ Y, int B, int M,
                                        int N, int F, const float* __restrict__ g, const float* __restrict__ b,
                                        const float* __restrict__ ws, float drop_p, unsigned long long seed, const unsigned long long* __restrict__ seed_dev,
                                        const float* __restrict__ stats, const float* __restrict__ wts,
-                                       T* __restrict__ dY, float* __restrict__ dg, float* __restrict__ db,
-                                       float* __restrict__ dws, float* __restrict__ dbs, int rnd) {
+                                       float* __restrict__ dY, float* __restrict__ part, int rnd) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
   extern __shared__ float sm[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* sdg = sm;
-  float* sdb = sm + F;
-  float* sdw = sm + 2 * F;
-  float* yh = sm + 3 * F + (long long)warp * 2 * F;   // per warp: yhat [F], d [F]
+  const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* acc = sm + (long long)warp * (5 * F + 1);  // per warp: dg [F], db [F], dws [F], dbs [1], yhat [F], d [F]
+  float* sdb = acc + F;
+  float* sdw = sdb + F;
+  float* yh = sdw + F + 1;
   float* dd = yh + F;
-  for (int c = threadIdx.x; c < 3 * F; c += blockDim.x) sm[c] = 0.f;
-  __syncthreads();
+  for (int c = lane; c < 3 * F + 1; c += 32) acc[c] = 0.f;
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   const long long T_ = (long long)B * N;
   float dbs_acc = 0.f;
-  for (long long t = (long long)blockIdx.x * ROW_WARPS + warp; t < T_; t += (long long)gridDim.x * ROW_WARPS) {
+  for (long long t = (long long)blockIdx.x * warps + warp; t < T_; t += (long long)gridDim.x * warps) {
     const long long bi = t / N, ni = t % N;
     const float* go = dout + t * F;
     // pass 1: dw_m = <dout, Yn_m>
@@ -710,9 +672,9 @@ __global__ void ln_softaggr_bwd_kernel(const float* __restrict__ dout, const flo
         const float a = (v - mean) * rstd;
         const float yn = a * g[c] + b[c];
         const float dyn = w[m] * go[c] + dscore * ws[c];
-        atomicAdd(&sdw[c], dscore * yn);
-        atomicAdd(&sdg[c], dyn * a);
-        atomicAdd(&sdb[c], dyn);
+        sdw[c] += dscore * yn;
+        acc[c] += dyn * a;
+        sdb[c] += dyn;
         const float d = dyn * g[c];
         yh[c] = a; dd[c] = d;
         s1 += d; s2 += d * a;
@@ -722,18 +684,13 @@ __global__ void ln_softaggr_bwd_kernel(const float* __restrict__ dout, const flo
         float d = rstd * (dd[c] - s1 - yh[c] * s2);
         if (drop_p > 0.f)
           d = sx::drop_keep1(seed, (unsigned long long)(ro * F + c), sx::drop_p16(drop_p)) ? d * keep_scale : 0.f;
-        stf<T>(dY + ro * F + c, d, rnd);
+        dY[ro * F + c] = rnd1(d, rnd);
       }
       __syncwarp();
     }
   }
-  __syncthreads();
-  for (int c = threadIdx.x; c < F; c += blockDim.x) {
-    atomicAdd(&dg[c], sdg[c]);
-    atomicAdd(&db[c], sdb[c]);
-    atomicAdd(&dws[c], sdw[c]);
-  }
-  if (lane == 0) atomicAdd(dbs, dbs_acc);     // identical in all lanes of the warp
+  if (lane == 0) sdw[F] = dbs_acc;            // identical in all lanes of the warp
+  warps_to_slot(sm, warps, 5ll * F + 1, 3 * F + 1, part);
 }
 
 #include "sx_rows_fast.cuh"
@@ -743,15 +700,14 @@ __global__ void ln_softaggr_bwd_kernel(const float* __restrict__ dout, const flo
 // elementwise helpers
 // ------------------------------------------------------------------------------------------------
 // dH = dGd * keep/(1-p) * gelu'(H)   (MMSharedMid backward, segtran_shared.py:243-245)
-template <typename TH, typename TO>
-__global__ void gelu_bwd_kernel(const float* __restrict__ dG, const TH* __restrict__ H, long long n, float drop_p,
-                                unsigned long long seed, const unsigned long long* __restrict__ seed_dev, TO* __restrict__ dH, int rnd) {
+__global__ void gelu_bwd_kernel(const float* __restrict__ dG, const float* __restrict__ H, long long n, float drop_p,
+                                unsigned long long seed, const unsigned long long* __restrict__ seed_dev, float* __restrict__ dH, int rnd) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float d = dG[i];
     if (drop_p > 0.f) d = sx::drop_keep1(seed, (unsigned long long)i, sx::drop_p16(drop_p)) ? d * keep_scale : 0.f;
-    stf<TO>(dH + i, d * sx::gelu_erf_grad(ldf<TH>(H + i)), rnd);
+    dH[i] = rnd1(d * sx::gelu_erf_grad(H[i]), rnd);
   }
 }
 
@@ -769,10 +725,15 @@ __global__ void gelu_bwd_f4_kernel(const float4* __restrict__ dG, const float4* 
   }
 }
 
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ void store_cvt(float* p, float v, int rnd) { *p = rnd1(v, rnd); }
+__device__ __forceinline__ void store_cvt(__nv_bfloat16* p, float v, int) { *p = __float2bfloat16_rn(v); }
+
 template <typename TI, typename TO>
 __global__ void convert_kernel(const TI* __restrict__ x, long long n, TO* __restrict__ y, int rnd) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    stf<TO>(y + i, ldf<TI>(x + i), rnd);
+    store_cvt(y + i, to_f32(x[i]), rnd);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -876,27 +837,10 @@ __global__ void split_cat_kernel(const float* __restrict__ x, int Z0, int R, int
   }
 }
 
-// out[c] += sum_r X[r, c]   (bias gradients).  blockDim (32, 8)
-template <typename T>
-__global__ void colsum_kernel(const T* __restrict__ X, long long R, int C, long long ld, float* __restrict__ out) {
-  const int c = blockIdx.x * 32 + threadIdx.x;
-  float acc = 0.f;
-  if (c < C)
-    for (long long r = (long long)blockIdx.y * blockDim.y + threadIdx.y; r < R; r += (long long)gridDim.y * blockDim.y)
-      acc += ldf<T>(X + r * ld + c);
-  __shared__ float s[8][33];
-  s[threadIdx.y][threadIdx.x] = acc;
-  __syncthreads();
-  if (threadIdx.y == 0 && c < C) {
-    float t = 0.f;
-    for (int y = 0; y < 8; ++y) t += s[y][threadIdx.x];
-    atomicAdd(&out[c], t);
-  }
-}
-
-// out[z0*C + c] += sum_{z1,r} X[z1*sz1 + z0*sz0 + r*ld + c]   (per-mode bias gradients in one launch).  blockDim (32, 8)
-__global__ void colsum_batched_kernel(const float* __restrict__ X, int Z1, long long sz1, long long sz0, long long R,
-                                      int C, long long ld, float* __restrict__ out) {
+// out[z0*C + c] += sum_{z1,r} X[z1*sz1 + z0*sz0 + r*ld + c]   (bias gradients, per mode in one launch).  blockDim
+// (32, 8), grid (C/32, row blocks, Z0); the partial sums of row block y go to slot y of `part` ([Z0 * C])
+__global__ void colsum_kernel(const float* __restrict__ X, int Z1, long long sz1, long long sz0, long long R, int C,
+                              long long ld, float* __restrict__ part) {
   const int c = blockIdx.x * 32 + threadIdx.x;
   const int z0 = blockIdx.z;
   float acc = 0.f;
@@ -912,11 +856,11 @@ __global__ void colsum_batched_kernel(const float* __restrict__ X, int Z1, long 
   if (threadIdx.y == 0 && c < C) {
     float t = 0.f;
     for (int y = 0; y < 8; ++y) t += s[y][threadIdx.x];
-    atomicAdd(&out[(long long)z0 * C + c], t);
+    part[((long long)blockIdx.y * gridDim.z + z0) * C + c] = t;
   }
 }
 
-// float4 flavour of both column sums: lane = 4 consecutive columns (512 B per warp and row), 4 rows in flight per thread.
+// float4 flavour of colsum_kernel: lane = 4 consecutive columns (512 B per warp and row), 4 rows in flight per thread.
 // out[z0*C + c] += sum_{z1,r} X[z1*sz1 + z0*sz0 + r*ld + c];  blockDim (32, 8), grid (C/128, row blocks, Z0); the partial
 // sums of row block y go to slot y of `part` ([Z0 * C]) and part_reduce adds them into out
 __global__ void __launch_bounds__(256)
@@ -977,8 +921,8 @@ __global__ void transpose_kernel(const float* __restrict__ in, int R, int C, int
   }
 }
 
-// out[0] += sum_i x[i] * y[i]     (linear synthetic loss / checksums)
-__global__ void dot_kernel(const float* __restrict__ x, const float* __restrict__ y, long long n, float* out) {
+// sum_i x[i] * y[i] (linear synthetic loss / checksums): block b's sum goes to slot b of `part`
+__global__ void dot_kernel(const float* __restrict__ x, const float* __restrict__ y, long long n, float* __restrict__ part) {
   float acc = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     acc = fmaf(x[i], y[i], acc);
@@ -989,7 +933,7 @@ __global__ void dot_kernel(const float* __restrict__ x, const float* __restrict_
   if (threadIdx.x < 32) {
     acc = threadIdx.x < (blockDim.x >> 5) ? s[threadIdx.x] : 0.f;
     acc = sx::warp_sum(acc);
-    if (threadIdx.x == 0) atomicAdd(out, acc);
+    if (threadIdx.x == 0) part[blockIdx.x] = acc;
   }
 }
 
@@ -1027,17 +971,6 @@ __global__ void scale_kernel(const float* __restrict__ x, long long n, const flo
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     y[i] = a * x[i];
 }
-
-// dst arrays += the sum of `slots` slot rows of part (row pitch `stride` >= the summed array lengths), in slot order
-int part_reduce(const float* part, int slots, int stride, PartDst d, cudaStream_t st) {
-  const int total = d.n[0] + d.n[1] + d.n[2] + d.n[3];
-  part_reduce_kernel<<<sx_ceil_div(total, 256), 256, 0, st>>>(part, slots, stride, total, d);
-  SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// most slots of pitch `stride` that fit a scratch of part_floats floats
-int part_slots(int64_t part_floats, long long stride) { return (int)std::min<long long>(part_floats / stride, 1 << 30); }
 
 int grid_for_rows(long long rows, int per_block, int sms) {
   long long g = (rows + per_block - 1) / per_block;
@@ -1098,29 +1031,31 @@ extern "C" int sx_pos_lsinu_bwd(const float* pos, const float* posmax, int64_t R
   return part_reduce(part, 16, C * pd + C, PartDst{{dW, db, nullptr, nullptr}, {C * pd, C, 0, 0}}, ST(stream));
 }
 
+// warps per CTA of a warp-per-row kernel that stages `floats_per_warp` floats in shared memory: at most 8, and 0 when
+// one warp's share does not fit
+static int smem_warps(long long floats_per_warp) {
+  return (int)std::min<long long>(ROW_WARPS, (200 * 1024) / (floats_per_warp * 4));
+}
+
 extern "C" int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, const float* g, const float* b,
                                const float* pe, int32_t C0, int64_t pe_bstride, float posw, const float* mask,
-                               float drop_p, uint64_t seed, const uint64_t* seed_dev, void* h, int32_t h_dtype, int32_t round_tf32, float* stats,
+                               float drop_p, uint64_t seed, const uint64_t* seed_dev, float* h, int32_t round_tf32, float* stats,
                                void* stream) {
   if (!pe) {                                        // no positional code: h = mask * dropout(LN_{g,b}(x))
     const long long R = (long long)B * N;
     const int grid = grid_for_rows(R, NOPOS_WARPS, sms_cached());
-    if (h_dtype == SX_F32)
-      prologue_nopos_fwd_kernel<float><<<grid, NOPOS_WARPS * 32, 0, ST(stream)>>>(
-          x, R, C, g, b, mask, drop_p, seed, (const unsigned long long*)seed_dev, (float*)h, stats, round_tf32);
-    else
-      prologue_nopos_fwd_kernel<__nv_bfloat16><<<grid, NOPOS_WARPS * 32, 0, ST(stream)>>>(
-          x, R, C, g, b, mask, drop_p, seed, (const unsigned long long*)seed_dev, (__nv_bfloat16*)h, stats, 0);
+    prologue_nopos_fwd_kernel<<<grid, NOPOS_WARPS * 32, 0, ST(stream)>>>(
+        x, R, C, g, b, mask, drop_p, seed, (const unsigned long long*)seed_dev, h, stats, round_tf32);
     SX_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
-  if (h_dtype == SX_F32 && C % 4 == 0 && C <= 2048 && C0 % 4 == 0 && pe_bstride % 4 == 0 && al16(x) && al16(h) && al16(pe) &&
+  if (C % 4 == 0 && C <= 2048 && C0 % 4 == 0 && pe_bstride % 4 == 0 && al16(x) && al16(h) && al16(pe) &&
       al16(g) && al16(b)) {
     // CTA-per-row kernel: the row in registers, 16-byte accesses at every width
     const long long R = (long long)B * N;
 #define SX_LAUNCH(NV_, TT_)                                                                                             \
   prologue_fwd_cta<NV_, TT_><<<(int)std::min<long long>(R, (long long)sms_cached() * (1024 / TT_)), TT_, 0, ST(stream)>>>( \
-      x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, (float*)h, stats, \
+      x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, h, stats, \
       round_tf32)
     if (C <= 512) SX_LAUNCH(1, 128); else if (C <= 1024) SX_LAUNCH(2, 128); else SX_LAUNCH(2, 256);
 #undef SX_LAUNCH
@@ -1131,15 +1066,9 @@ extern "C" int sx_prologue_fwd(const float* x, int64_t B, int32_t N, int32_t C, 
   SX_REQUIRE(smem <= 200 * 1024, "sx_prologue_fwd: C=%d too large", C);
   const long long R = (long long)B * N;
   const int grid = grid_for_rows(R, ROW_WARPS, sms_cached());
-  if (h_dtype == SX_F32) {
-    if (set_smem(prologue_fwd_kernel<float>, smem)) return -2;
-    prologue_fwd_kernel<float><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(
-        x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, (float*)h, stats, round_tf32);
-  } else {
-    if (set_smem(prologue_fwd_kernel<__nv_bfloat16>, smem)) return -2;
-    prologue_fwd_kernel<__nv_bfloat16><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(
-        x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, (__nv_bfloat16*)h, stats, 0);
-  }
+  if (set_smem(prologue_fwd_kernel, smem)) return -2;
+  prologue_fwd_kernel<<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(
+      x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, h, stats, round_tf32);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1148,10 +1077,11 @@ extern "C" int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32
                                const float* b, const float* pe, int32_t C0, int64_t pe_bstride, float posw,
                                const float* mask, float drop_p, uint64_t seed, const uint64_t* seed_dev, const float* stats, float* dx, float* dg,
                                float* db, float* dpe, float* dt_scratch, float* part, int64_t part_floats, void* stream) {
+  const long long R = (long long)B * N;
+  SX_REQUIRE(part && part_floats >= 2ll * C, "sx_prologue_bwd: needs at least %lld floats of scratch", 2ll * C);
+  const PartDst dgb{{dg, db, nullptr, nullptr}, {C, C, 0, 0}};
   if (!pe) {
     SX_REQUIRE(!dpe, "sx_prologue_bwd: dpe must be NULL without a positional code");
-    const long long R = (long long)B * N;
-    SX_REQUIRE(part && part_floats >= 2ll * C, "sx_prologue_bwd: needs at least %lld floats of scratch", 2ll * C);
     const int grid = std::min(grid_for_rows(R, NOPOS_WARPS, sms_cached()), part_slots(part_floats, 2ll * C));
     const size_t smem = (size_t)NOPOS_WARPS * 2 * C * 4;
     SX_REQUIRE(smem <= 200 * 1024, "sx_prologue_bwd: C=%d too large", C);
@@ -1159,18 +1089,17 @@ extern "C" int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32
     prologue_nopos_bwd_kernel<<<grid, NOPOS_WARPS * 32, smem, ST(stream)>>>(
         dh, x, R, C, g, mask, drop_p, seed, (const unsigned long long*)seed_dev, stats, dx, part);
     SX_CHECK_CUDA(cudaGetLastError());
-    return part_reduce(part, grid, 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream));
+    return part_reduce(part, grid, 2 * C, dgb, ST(stream));
   }
-  if (C % 4 == 0 && C <= 2048 && C0 % 4 == 0 && pe_bstride % 4 == 0 && al16(dh) && al16(x) && al16(dx) && al16(pe) && al16(g) &&
-      al16(b) && (!dpe || (dt_scratch && al16(dt_scratch) && al16(dpe)))) {
+  SX_REQUIRE(!dpe || dt_scratch, "sx_prologue_bwd: dpe needs dt_scratch");
+  float* dt = dpe ? dt_scratch : nullptr;
+  const bool vec = C % 4 == 0 && C0 % 4 == 0 && pe_bstride % 4 == 0 && (!dpe || (al16(dt_scratch) && al16(dpe)));
+  if (vec && C <= 2048 && al16(dh) && al16(x) && al16(dx) && al16(pe) && al16(g) && al16(b)) {
     // CTA-per-row kernel: x / dh read once, dx (and dt, when the positional-code gradient needs it) written once, dg / db
     // accumulated in registers
-    const long long R = (long long)B * N;
-    float* dt = dpe ? dt_scratch : nullptr;
     auto pgrid = [&](int tt) {
       return (int)std::min<long long>(std::min<long long>(R, (long long)sms_cached() * (768 / tt)), part_slots(part_floats, 2 * C));
     };
-    SX_REQUIRE(part && part_floats >= 2ll * C, "sx_prologue_bwd: needs at least %lld floats of scratch", 2ll * C);
 #define SX_LAUNCH(NV_, TT_)                                                                                             \
   prologue_bwd_cta<NV_, TT_><<<pgrid(TT_), TT_, 0, ST(stream)>>>(                                                    \
       dh, x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, stats, dx, dt, \
@@ -1178,65 +1107,37 @@ extern "C" int sx_prologue_bwd(const float* dh, const float* x, int64_t B, int32
     if (C <= 512) SX_LAUNCH(1, 128); else if (C <= 1024) SX_LAUNCH(2, 128); else SX_LAUNCH(2, 256);
 #undef SX_LAUNCH
     SX_CHECK_CUDA(cudaGetLastError());
-    if (part_reduce(part, pgrid(C <= 1024 ? 128 : 256), 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream))) return -2;
-    if (dpe) {
-      pos_grad_from_dt_fast<<<grid_for_rows((long long)N * (C / 4), 256, sms_cached()), 256, 0, ST(stream)>>>(
-          dt_scratch, (int)B, N, C, C0, pe_bstride, posw, dpe);
-      SX_CHECK_CUDA(cudaGetLastError());
-    }
-    return 0;
-  }
-  if (dt_scratch && C % 4 == 0 && C0 % 4 == 0 && pe_bstride % 4 == 0 && nv_for(C) && al16(dh) && al16(x) && al16(dx) &&
-      al16(pe) && al16(g) && al16(b) && al16(dt_scratch) && (!dpe || al16(dpe))) {
-    const long long R = (long long)B * N;
-    const int grid = grid_for_rows(R, FAST_WARPS, sms_cached() * 2);
-#define SX_LAUNCH(NV_)                                                                                                \
-  prologue_bwd_rows_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(dh, x, R, N, C, g, b, pe, C0, pe_bstride, posw, \
-                                                                        mask, drop_p, seed, (const unsigned long long*)seed_dev, stats, dx, dt_scratch)
-    switch (nv_for(C)) { case 2: SX_LAUNCH(2); break; case 4: SX_LAUNCH(4); break; case 8: SX_LAUNCH(8); break;
-                         default: SX_LAUNCH(16); }
-#undef SX_LAUNCH
+    if (part_reduce(part, pgrid(C <= 1024 ? 128 : 256), 2 * C, dgb, ST(stream))) return -2;
+  } else {
+    const int warps = smem_warps(5ll * C);
+    SX_REQUIRE(warps >= 1, "sx_prologue_bwd: C=%d too large", C);
+    const size_t smem = (size_t)warps * 5 * C * 4;
+    const int grid = std::min(grid_for_rows(R, warps * 4, sms_cached()), part_slots(part_floats, 2ll * C));
+    if (set_smem(prologue_bwd_kernel, smem)) return -2;
+    prologue_bwd_kernel<<<grid, warps * 32, smem, ST(stream)>>>(
+        dh, x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, stats, dx, dt, part);
     SX_CHECK_CUDA(cudaGetLastError());
-    int gy = (int)((R + 8 * 64 - 1) / (8 * 64));
-    const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128));
-    if (gy > cap) gy = cap;
-    gy = std::min(gy, part_slots(part_floats, 2 * C));
-    SX_REQUIRE(part && gy >= 1, "sx: needs at least %lld floats of scratch", 2ll * C);
-    if (gy < 1) gy = 1;
-    dim3 grid2(sx_ceil_div(C, 128), gy), blk(32, 8);
-    ln_param_grad_cols_fast<<<grid2, blk, 0, ST(stream)>>>(dt_scratch, x, R, C, stats, 4, part);
-    SX_CHECK_CUDA(cudaGetLastError());
-    if (part_reduce(part, gy, 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream))) return -2;
-    if (dpe) {
-      pos_grad_from_dt_fast<<<grid_for_rows((long long)N * (C / 4), 256, sms_cached()), 256, 0, ST(stream)>>>(
-          dt_scratch, (int)B, N, C, C0, pe_bstride, posw, dpe);
-      SX_CHECK_CUDA(cudaGetLastError());
-    }
-    return 0;
+    if (part_reduce(part, grid, 2 * C, dgb, ST(stream))) return -2;
   }
-  const size_t smem = (size_t)(2 + 3 * ROW_WARPS) * C * 4;
-  SX_REQUIRE(smem <= 220 * 1024, "sx_prologue_bwd: C=%d too large", C);
-  if (set_smem(prologue_bwd_kernel, smem)) return -2;
-  const long long R = (long long)B * N;
-  prologue_bwd_kernel<<<grid_for_rows(R, ROW_WARPS * 4, sms_cached()), ROW_WARPS * 32, smem, ST(stream)>>>(
-      dh, x, R, N, C, g, b, pe, C0, pe_bstride, posw, mask, drop_p, seed, (const unsigned long long*)seed_dev, stats, dx, dg, db, dpe);
-  SX_CHECK_CUDA(cudaGetLastError());
+  if (dpe) {
+    if (vec)
+      pos_grad_from_dt<4><<<grid_for_rows((long long)N * (C / 4), 256, sms_cached()), 256, 0, ST(stream)>>>(
+          dt, (int)B, N, C, C0, pe_bstride, posw, dpe);
+    else
+      pos_grad_from_dt<1><<<grid_for_rows((long long)N * C, 256, sms_cached()), 256, 0, ST(stream)>>>(
+          dt, (int)B, N, C, C0, pe_bstride, posw, dpe);
+    SX_CHECK_CUDA(cudaGetLastError());
+  }
   return 0;
 }
 
-static int softmax_warps(int L, int per_row_floats) {
-  int w = (int)((200 * 1024) / ((size_t)L * per_row_floats * 4));
-  if (w > 8) w = 8;
-  return w;
-}
-
 extern "C" int sx_softmax_fwd(const float* S, int64_t R, int32_t L, int64_t lds, const float* amax, float clip,
-                              float drop_p, uint64_t seed, const uint64_t* seed_dev, void* P, int32_t p_dtype, int64_t ldp, int32_t round_tf32,
+                              float drop_p, uint64_t seed, const uint64_t* seed_dev, float* P, int64_t ldp, int32_t round_tf32,
                               float* lse, float* diag, void* stream) {
-  if (p_dtype == SX_F32 && L % 4 == 0 && lds % 4 == 0 && ldp % 4 == 0 && al16(S) && al16(P) && nv_for(L)) {
+  if (L % 4 == 0 && lds % 4 == 0 && ldp % 4 == 0 && al16(S) && al16(P) && nv_for(L)) {
     const int grid = grid_for_rows(R, FAST_WARPS, sms_cached() * 2);
 #define SX_LAUNCH(NV_)                                                                                          \
-  softmax_fwd_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, (float*)P, \
+  softmax_fwd_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, P, \
                                                                   ldp, lse, round_tf32, diag)
     switch (nv_for(L)) { case 2: SX_LAUNCH(2); break; case 4: SX_LAUNCH(4); break; case 8: SX_LAUNCH(8); break;
                          default: SX_LAUNCH(16); }
@@ -1244,102 +1145,84 @@ extern "C" int sx_softmax_fwd(const float* S, int64_t R, int32_t L, int64_t lds,
     SX_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
-  if (p_dtype == SX_F32 && L % 4 == 0 && lds % 4 == 0 && ldp % 4 == 0 && al16(S) && al16(P) && L <= 8192) {
+  if (L % 4 == 0 && lds % 4 == 0 && ldp % 4 == 0 && al16(S) && al16(P) && L <= 8192) {
     const int grid = (int)(R < (long long)sms_cached() * 16 ? R : (long long)sms_cached() * 16);
 #define SX_LAUNCH(E_)                                                                                          \
   softmax_fwd_block<E_><<<grid, 256, 0, ST(stream)>>>(S, R, L, lds, amax, clip, drop_p, seed,                     \
-                                                      (const unsigned long long*)seed_dev, (float*)P, ldp, lse,  \
+                                                      (const unsigned long long*)seed_dev, P, ldp, lse,          \
                                                       round_tf32, diag)
     if (L <= 3072) SX_LAUNCH(3); else if (L <= 6144) SX_LAUNCH(6); else SX_LAUNCH(8);
 #undef SX_LAUNCH
     SX_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
-  const int w = softmax_warps(L, 1);
+  const int w = smem_warps(L);
   SX_REQUIRE(w >= 1, "sx_softmax_fwd: row length %d too large", L);
   const size_t smem = (size_t)w * L * 4;
   const int grid = grid_for_rows(R, w, sms_cached());
-  if (p_dtype == SX_F32) {
-    if (set_smem(softmax_fwd_kernel<float>, smem)) return -2;
-    softmax_fwd_kernel<float><<<grid, w * 32, smem, ST(stream)>>>(S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, (float*)P, ldp,
-                                                                   lse, round_tf32, diag);
-  } else {
-    if (set_smem(softmax_fwd_kernel<__nv_bfloat16>, smem)) return -2;
-    softmax_fwd_kernel<__nv_bfloat16><<<grid, w * 32, smem, ST(stream)>>>(S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev,
-                                                                          (__nv_bfloat16*)P, ldp, lse, 0, diag);
-  }
+  if (set_smem(softmax_fwd_kernel, smem)) return -2;
+  softmax_fwd_kernel<<<grid, w * 32, smem, ST(stream)>>>(S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, P, ldp,
+                                                         lse, round_tf32, diag);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
 extern "C" int sx_softmax_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, const float* lse, int64_t R,
                               int32_t L, const float* amax, float clip, float drop_p, uint64_t seed, const uint64_t* seed_dev, int64_t ldp_fwd,
-                              void* dS, int32_t ds_dtype, int64_t ldo, int32_t round_tf32, void* stream) {
-  if (ds_dtype == SX_F32 && L % 4 == 0 && lds % 4 == 0 && ldd % 4 == 0 && ldo % 4 == 0 && al16(S) && al16(dP) &&
-      al16(dS) && nv_for(L)) {
+                              float* dS, int64_t ldo, int32_t round_tf32, void* stream) {
+  if (L % 4 == 0 && lds % 4 == 0 && ldd % 4 == 0 && ldo % 4 == 0 && al16(S) && al16(dP) && al16(dS) && nv_for(L)) {
     const int grid = grid_for_rows(R, FAST_WARPS, sms_cached() * 2);
 #define SX_LAUNCH(NV_)                                                                                             \
   softmax_bwd_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, \
-                                                                  ldp_fwd, (float*)dS, ldo, round_tf32)
+                                                                  ldp_fwd, dS, ldo, round_tf32)
     switch (nv_for(L)) { case 2: SX_LAUNCH(2); break; case 4: SX_LAUNCH(4); break; case 8: SX_LAUNCH(8); break;
                          default: SX_LAUNCH(16); }
 #undef SX_LAUNCH
     SX_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
-  if (ds_dtype == SX_F32 && L % 4 == 0 && lds % 4 == 0 && ldd % 4 == 0 && ldo % 4 == 0 && al16(S) && al16(dP) &&
-      al16(dS) && L <= 8192) {
+  if (L % 4 == 0 && lds % 4 == 0 && ldd % 4 == 0 && ldo % 4 == 0 && al16(S) && al16(dP) && al16(dS) && L <= 8192) {
     const int grid = (int)(R < (long long)sms_cached() * 16 ? R : (long long)sms_cached() * 16);
 #define SX_LAUNCH(E_)                                                                                            \
   softmax_bwd_block<E_><<<grid, 256, 0, ST(stream)>>>(dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed,         \
-                                                      (const unsigned long long*)seed_dev, ldp_fwd, (float*)dS, ldo, \
+                                                      (const unsigned long long*)seed_dev, ldp_fwd, dS, ldo,       \
                                                       round_tf32)
     if (L <= 3072) SX_LAUNCH(3); else if (L <= 6144) SX_LAUNCH(6); else SX_LAUNCH(8);
 #undef SX_LAUNCH
     SX_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
-  const int w = softmax_warps(L, 2);
+  const int w = smem_warps(2ll * L);
   SX_REQUIRE(w >= 1, "sx_softmax_bwd: row length %d too large", L);
   const size_t smem = (size_t)w * 2 * L * 4;
   const int grid = grid_for_rows(R, w, sms_cached());
-  if (ds_dtype == SX_F32) {
-    if (set_smem(softmax_bwd_kernel<float>, smem)) return -2;
-    softmax_bwd_kernel<float><<<grid, w * 32, smem, ST(stream)>>>(dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev,
-                                                                   ldp_fwd, (float*)dS, ldo, round_tf32);
-  } else {
-    if (set_smem(softmax_bwd_kernel<__nv_bfloat16>, smem)) return -2;
-    softmax_bwd_kernel<__nv_bfloat16><<<grid, w * 32, smem, ST(stream)>>>(
-        dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, ldp_fwd, (__nv_bfloat16*)dS, ldo, 0);
-  }
+  if (set_smem(softmax_bwd_kernel, smem)) return -2;
+  softmax_bwd_kernel<<<grid, w * 32, smem, ST(stream)>>>(dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev,
+                                                         ldp_fwd, dS, ldo, round_tf32);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
-extern "C" int sx_layernorm_fwd(const float* x, int64_t R, int32_t C, const float* g, const float* b, void* y,
-                                int32_t y_dtype, int32_t round_tf32, float* stats, void* stream) {
+extern "C" int sx_layernorm_fwd(const float* x, int64_t R, int32_t C, const float* g, const float* b, float* y,
+                                int32_t round_tf32, float* stats, void* stream) {
   const size_t smem = (size_t)ROW_WARPS * C * 4;
   SX_REQUIRE(smem <= 200 * 1024, "sx_layernorm_fwd: C=%d too large", C);
   const int grid = grid_for_rows(R, ROW_WARPS, sms_cached());
-  if (y_dtype == SX_F32) {
-    if (set_smem(layernorm_fwd_kernel<float>, smem)) return -2;
-    layernorm_fwd_kernel<float><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(x, R, C, g, b, (float*)y, stats, round_tf32);
-  } else {
-    if (set_smem(layernorm_fwd_kernel<__nv_bfloat16>, smem)) return -2;
-    layernorm_fwd_kernel<__nv_bfloat16><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(x, R, C, g, b, (__nv_bfloat16*)y,
-                                                                                    stats, 0);
-  }
+  if (set_smem(layernorm_fwd_kernel, smem)) return -2;
+  layernorm_fwd_kernel<<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(x, R, C, g, b, y, stats, round_tf32);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
 extern "C" int sx_layernorm_bwd(const float* dy, const float* x, int64_t R, int32_t C, const float* g,
-                                const float* stats, void* dx, int32_t dx_dtype, int32_t round_tf32, float* dg, float* db,
+                                const float* stats, float* dx, int32_t round_tf32, float* dg, float* db,
                                 float* part, int64_t part_floats, void* stream) {
-  if (dx_dtype == SX_F32 && C % 4 == 0 && nv_for(C) && al16(dy) && al16(x) && al16(dx) && al16(g)) {
+  SX_REQUIRE(part && part_floats >= 2ll * C, "sx_layernorm_bwd: needs at least %lld floats of scratch", 2ll * C);
+  const PartDst dgb{{dg, db, nullptr, nullptr}, {C, C, 0, 0}};
+  if (C % 4 == 0 && nv_for(C) && al16(dy) && al16(x) && al16(dx) && al16(g)) {
     const int grid = grid_for_rows(R, FAST_WARPS, sms_cached() * 2);
 #define SX_LAUNCH(NV_)                                                                                         \
-  layernorm_bwd_rows_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(dy, x, R, C, g, stats, (float*)dx, round_tf32)
+  layernorm_bwd_rows_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(dy, x, R, C, g, stats, dx, round_tf32)
     switch (nv_for(C)) { case 2: SX_LAUNCH(2); break; case 4: SX_LAUNCH(4); break; case 8: SX_LAUNCH(8); break;
                          default: SX_LAUNCH(16); }
 #undef SX_LAUNCH
@@ -1348,28 +1231,20 @@ extern "C" int sx_layernorm_bwd(const float* dy, const float* x, int64_t R, int3
     const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128));
     if (gy > cap) gy = cap;
     gy = std::min(gy, part_slots(part_floats, 2 * C));
-    SX_REQUIRE(part && gy >= 1, "sx: needs at least %lld floats of scratch", 2ll * C);
     if (gy < 1) gy = 1;
     dim3 grid2(sx_ceil_div(C, 128), gy), blk(32, 8);
     ln_param_grad_cols_fast<<<grid2, blk, 0, ST(stream)>>>(dy, x, R, C, stats, 2, part);
     SX_CHECK_CUDA(cudaGetLastError());
-    if (part_reduce(part, gy, 2 * C, PartDst{{dg, db, nullptr, nullptr}, {C, C, 0, 0}}, ST(stream))) return -2;
-    return 0;
+    return part_reduce(part, gy, 2 * C, dgb, ST(stream));
   }
-  const size_t smem = (size_t)(2 + 2 * ROW_WARPS) * C * 4;
-  SX_REQUIRE(smem <= 220 * 1024, "sx_layernorm_bwd: C=%d too large", C);
-  const int grid = grid_for_rows(R, ROW_WARPS * 4, sms_cached());
-  if (dx_dtype == SX_F32) {
-    if (set_smem(layernorm_bwd_kernel<float>, smem)) return -2;
-    layernorm_bwd_kernel<float><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(dy, x, R, C, g, stats, (float*)dx, dg, db,
-                                                                             round_tf32);
-  } else {
-    if (set_smem(layernorm_bwd_kernel<__nv_bfloat16>, smem)) return -2;
-    layernorm_bwd_kernel<__nv_bfloat16><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(dy, x, R, C, g, stats,
-                                                                                    (__nv_bfloat16*)dx, dg, db, 0);
-  }
+  const int warps = smem_warps(4ll * C);
+  SX_REQUIRE(warps >= 1, "sx_layernorm_bwd: C=%d too large", C);
+  const size_t smem = (size_t)warps * 4 * C * 4;
+  const int grid = std::min(grid_for_rows(R, warps * 4, sms_cached()), part_slots(part_floats, 2ll * C));
+  if (set_smem(layernorm_bwd_kernel, smem)) return -2;
+  layernorm_bwd_kernel<<<grid, warps * 32, smem, ST(stream)>>>(dy, x, R, C, g, stats, dx, part, round_tf32);
   SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return part_reduce(part, grid, 2 * C, dgb, ST(stream));
 }
 
 extern "C" int sx_ln_softaggr_fwd(const float* Y, int32_t B, int32_t M, int32_t N, int32_t F, const float* g,
@@ -1390,23 +1265,11 @@ extern "C" int sx_ln_softaggr_fwd(const float* Y, int32_t B, int32_t M, int32_t 
     SX_CHECK_CUDA(cudaGetLastError());
     return 0;
   }
-  if (F % 4 == 0 && nv_for(F) && al16(Y) && al16(out) && al16(g) && al16(b) && al16(ws)) {
-    const int grid = grid_for_rows((long long)B * N, FAST_WARPS, sms_cached() * 2);
-#define SX_LAUNCH(NV_)                                                                                          \
-  ln_softaggr_fwd_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(Y, B, M, N, F, g, b, ws, bs, drop_p, seed, (const unsigned long long*)seed_dev, out, \
-                                                                      stats, wts)
-    switch (nv_for(F)) { case 2: SX_LAUNCH(2); break; case 4: SX_LAUNCH(4); break; case 8: SX_LAUNCH(8); break;
-                         default: SX_LAUNCH(16); }
-#undef SX_LAUNCH
-    SX_CHECK_CUDA(cudaGetLastError());
-    return 0;
-  }
-  int warps = (int)((200 * 1024) / ((size_t)M * F * 4));
-  if (warps > ROW_WARPS) warps = ROW_WARPS;
-  SX_REQUIRE(warps == ROW_WARPS, "sx_ln_softaggr_fwd: M*F=%d too large for 8 rows in shared memory", M * F);
-  const size_t smem = (size_t)ROW_WARPS * M * F * 4;
+  const int warps = smem_warps((long long)M * F);
+  SX_REQUIRE(warps >= 1, "sx_ln_softaggr_fwd: M*F=%d too large", M * F);
+  const size_t smem = (size_t)warps * M * F * 4;
   if (set_smem(ln_softaggr_fwd_kernel, smem)) return -2;
-  ln_softaggr_fwd_kernel<<<grid_for_rows((long long)B * N, ROW_WARPS, sms_cached()), ROW_WARPS * 32, smem, ST(stream)>>>(
+  ln_softaggr_fwd_kernel<<<grid_for_rows((long long)B * N, warps, sms_cached()), warps * 32, smem, ST(stream)>>>(
       Y, B, M, N, F, g, b, ws, bs, drop_p, seed, (const unsigned long long*)seed_dev, out, stats, wts);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -1414,20 +1277,20 @@ extern "C" int sx_ln_softaggr_fwd(const float* Y, int32_t B, int32_t M, int32_t 
 
 extern "C" int sx_ln_softaggr_bwd(const float* dout, const float* Y, int32_t B, int32_t M, int32_t N, int32_t F,
                                   const float* g, const float* b, const float* ws, float drop_p, uint64_t seed, const uint64_t* seed_dev,
-                                  const float* stats, const float* wts, void* dY, int32_t dy_dtype, int32_t round_tf32,
-                                  float* dg, float* db, float* dws, float* dbs, float* dscore_scratch, float* part, int64_t part_floats, void* stream) {
+                                  const float* stats, const float* wts, float* dY, int32_t round_tf32,
+                                  float* dg, float* db, float* dws, float* dbs, float* part, int64_t part_floats, void* stream) {
   SX_REQUIRE(M >= 1 && M <= MAX_MODES, "sx_ln_softaggr_bwd: num_modes %d not in 1..%d", M, MAX_MODES);
-  if (dy_dtype == SX_F32 && F % 4 == 0 && F <= 2048 && (M == 1 || M == 2 || M == 4) && al16(Y) && al16(dout) && al16(dY) &&
+  const long long T = (long long)B * N;
+  if (F % 4 == 0 && F <= 2048 && (M == 1 || M == 2 || M == 4) && al16(Y) && al16(dout) && al16(dY) &&
       al16(g) && al16(b) && al16(ws)) {
     // CTA-per-token kernel: Y and dout read once, dY written once, column gradients accumulated in registers
-    const long long T = (long long)B * N;
     const int grid = (int)std::min<long long>(std::min<long long>(T, (long long)sms_cached() * (F <= 1024 ? 3 : 2)),
                                               part_slots(part_floats, 3 * F + 4));
     SX_REQUIRE(part && grid >= 1, "sx_ln_softaggr_bwd: needs at least %lld floats of scratch", 3ll * F + 4);
 #define SX_LAUNCH(NV_, MM_, TT_)                                                                                        \
   ln_softaggr_bwd_cta<NV_, MM_, TT_><<<grid, TT_, 0, ST(stream)>>>(dout, Y, B, N, F, g, b, ws, drop_p, seed,            \
                                                                     (const unsigned long long*)seed_dev, stats, wts,    \
-                                                                    (float*)dY, round_tf32, part)
+                                                                    dY, round_tf32, part)
 #define SX_MODES(NV_, TT_) do { if (M == 4) SX_LAUNCH(NV_, 4, TT_); else if (M == 2) SX_LAUNCH(NV_, 2, TT_); else SX_LAUNCH(NV_, 1, TT_); } while (0)
     if (F <= 512) SX_MODES(1, 128); else if (F <= 1024) SX_MODES(2, 128); else SX_MODES(2, 256);
 #undef SX_MODES
@@ -1435,58 +1298,26 @@ extern "C" int sx_ln_softaggr_bwd(const float* dout, const float* Y, int32_t B, 
     SX_CHECK_CUDA(cudaGetLastError());
     return part_reduce(part, grid, 3 * F + 4, PartDst{{dg, db, dws, dbs}, {F, F, F, 1}}, ST(stream));
   }
-  if (dy_dtype == SX_F32 && dscore_scratch && F % 4 == 0 && nv_for(F) && al16(Y) && al16(dout) && al16(dY) && al16(g) &&
-      al16(b) && al16(ws)) {
-    const int grid = grid_for_rows((long long)B * N, FAST_WARPS, sms_cached() * 2);
-#define SX_LAUNCH(NV_)                                                                                              \
-  ln_softaggr_bwd_rows_fast<NV_><<<grid, FAST_WARPS * 32, 0, ST(stream)>>>(dout, Y, B, M, N, F, g, b, ws, drop_p, seed, (const unsigned long long*)seed_dev, \
-                                                                           stats, wts, (float*)dY, dscore_scratch, dbs, \
-                                                                           round_tf32)
-    switch (nv_for(F)) { case 2: SX_LAUNCH(2); break; case 4: SX_LAUNCH(4); break; case 8: SX_LAUNCH(8); break;
-                         default: SX_LAUNCH(16); }
-#undef SX_LAUNCH
-    SX_CHECK_CUDA(cudaGetLastError());
-    const long long R = (long long)B * M * N;
-    int gy = (int)((R + 8 * 64 - 1) / (8 * 64));
-    const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(F, 128));
-    if (gy > cap) gy = cap;
-    if (gy < 1) gy = 1;
-    dim3 grid2(sx_ceil_div(F, 128), gy), blk(32, 8);
-    ln_softaggr_bwd_cols_fast<<<grid2, blk, 0, ST(stream)>>>(dout, Y, B, M, N, F, g, b, ws, drop_p, seed, (const unsigned long long*)seed_dev, stats, wts,
-                                                             dscore_scratch, dg, db, dws);
-    SX_CHECK_CUDA(cudaGetLastError());
-    return 0;
-  }
-  const size_t smem = (size_t)(3 + 2 * ROW_WARPS) * F * 4;
-  SX_REQUIRE(smem <= 220 * 1024, "sx_ln_softaggr_bwd: F=%d too large", F);
-  const int grid = grid_for_rows((long long)B * N, ROW_WARPS * 4, sms_cached());
-  if (dy_dtype == SX_F32) {
-    if (set_smem(ln_softaggr_bwd_kernel<float>, smem)) return -2;
-    ln_softaggr_bwd_kernel<float><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(
-        dout, Y, B, M, N, F, g, b, ws, drop_p, seed, (const unsigned long long*)seed_dev, stats, wts, (float*)dY, dg, db, dws, dbs, round_tf32);
-  } else {
-    if (set_smem(ln_softaggr_bwd_kernel<__nv_bfloat16>, smem)) return -2;
-    ln_softaggr_bwd_kernel<__nv_bfloat16><<<grid, ROW_WARPS * 32, smem, ST(stream)>>>(
-        dout, Y, B, M, N, F, g, b, ws, drop_p, seed, (const unsigned long long*)seed_dev, stats, wts, (__nv_bfloat16*)dY, dg, db, dws, dbs, 0);
-  }
+  const int warps = smem_warps(5ll * F + 1);
+  SX_REQUIRE(warps >= 1, "sx_ln_softaggr_bwd: F=%d too large", F);
+  const size_t smem = (size_t)warps * (5 * F + 1) * 4;
+  const int grid = std::min(grid_for_rows(T, warps * 4, sms_cached()), part_slots(part_floats, 3ll * F + 1));
+  SX_REQUIRE(part && grid >= 1, "sx_ln_softaggr_bwd: needs at least %lld floats of scratch", 3ll * F + 1);
+  if (set_smem(ln_softaggr_bwd_kernel, smem)) return -2;
+  ln_softaggr_bwd_kernel<<<grid, warps * 32, smem, ST(stream)>>>(
+      dout, Y, B, M, N, F, g, b, ws, drop_p, seed, (const unsigned long long*)seed_dev, stats, wts, dY, part, round_tf32);
   SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return part_reduce(part, grid, 3 * F + 1, PartDst{{dg, db, dws, dbs}, {F, F, F, 1}}, ST(stream));
 }
 
-extern "C" int sx_gelu_bwd(const float* dG, const void* H, int32_t h_dtype, int64_t n, float drop_p, uint64_t seed, const uint64_t* seed_dev,
-                           void* dH, int32_t dh_dtype, int32_t round_tf32, void* stream) {
-  const int grid = grid_for_rows(n, 256 * 8, sms_cached());
-  SX_REQUIRE(h_dtype == dh_dtype, "sx_gelu_bwd: H and dH dtypes must match");
-  if (h_dtype == SX_F32 && n % 4 == 0 && al16(dG) && al16(H) && al16(dH))
+extern "C" int sx_gelu_bwd(const float* dG, const float* H, int64_t n, float drop_p, uint64_t seed, const uint64_t* seed_dev,
+                           float* dH, int32_t round_tf32, void* stream) {
+  if (n % 4 == 0 && al16(dG) && al16(H) && al16(dH))
     gelu_bwd_f4_kernel<<<grid_for_rows(n / 4, 256 * 4, sms_cached()), 256, 0, ST(stream)>>>(
         (const float4*)dG, (const float4*)H, n / 4, drop_p, seed, (const unsigned long long*)seed_dev, (float4*)dH, round_tf32);
-  else if (h_dtype == SX_F32)
-    gelu_bwd_kernel<float, float><<<grid, 256, 0, ST(stream)>>>(dG, (const float*)H, n, drop_p, seed, (const unsigned long long*)seed_dev, (float*)dH,
-                                                                 round_tf32);
   else
-    gelu_bwd_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, ST(stream)>>>(dG, (const __nv_bfloat16*)H, n, drop_p,
-                                                                                seed, (const unsigned long long*)seed_dev,
-                                                                                (__nv_bfloat16*)dH, 0);
+    gelu_bwd_kernel<<<grid_for_rows(n, 256 * 8, sms_cached()), 256, 0, ST(stream)>>>(
+        dG, H, n, drop_p, seed, (const unsigned long long*)seed_dev, dH, round_tf32);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1543,28 +1374,6 @@ extern "C" int sx_split_tf32_cat(const float* x, int32_t Z1, int32_t Z0, int32_t
   return 0;
 }
 
-extern "C" int sx_colsum(const void* X, int32_t x_dtype, int64_t R, int32_t C, int64_t ld, float* out, float* part, int64_t part_floats, void* stream) {
-  int gy = (int)((R + 255) / 256);
-  if (gy > 64) gy = 64;
-  if (gy < 1) gy = 1;
-  dim3 grid(sx_ceil_div(C, 32), gy), blk(32, 8);
-  if (x_dtype == SX_F32 && C % 4 == 0 && ld % 4 == 0 && al16(X)) {
-    int gy4 = (int)((R + 127) / 128);
-    const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128));
-    if (gy4 > cap) gy4 = cap;
-    gy4 = std::min(gy4, part_slots(part_floats, C));
-    SX_REQUIRE(part && gy4 >= 1, "sx_colsum: needs at least %d floats of scratch", C);
-    colsum_v4_kernel<<<dim3(sx_ceil_div(C, 128), gy4, 1), blk, 0, ST(stream)>>>((const float*)X, 1, 0, 0, R, C, ld, part);
-    SX_CHECK_CUDA(cudaGetLastError());
-    return part_reduce(part, gy4, C, PartDst{{out, nullptr, nullptr, nullptr}, {C, 0, 0, 0}}, ST(stream));
-  } else if (x_dtype == SX_F32)
-    colsum_kernel<float><<<grid, blk, 0, ST(stream)>>>((const float*)X, R, C, ld, out);
-  else
-    colsum_kernel<__nv_bfloat16><<<grid, blk, 0, ST(stream)>>>((const __nv_bfloat16*)X, R, C, ld, out);
-  SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
-}
-
 extern "C" int sx_transpose(const float* in, int64_t Z, int32_t R, int32_t C, int32_t ldo, float* out, void* stream) {
   SX_REQUIRE(Z <= 65535, "sx_transpose: batch %lld too large", (long long)Z);
   SX_REQUIRE(R > 0 && C > 0 && ldo >= R, "sx_transpose: bad shape R=%d C=%d ldo=%d", R, C, ldo);
@@ -1580,10 +1389,12 @@ extern "C" int sx_transpose(const float* in, int64_t Z, int32_t R, int32_t C, in
   return 0;
 }
 
-extern "C" int sx_dot(const float* x, const float* y, int64_t n, float* out, void* stream) {
-  dot_kernel<<<grid_for_rows(n, 256 * 8, sms_cached()), 256, 0, ST(stream)>>>(x, y, n, out);
+extern "C" int sx_dot(const float* x, const float* y, int64_t n, float* out, float* part, int64_t part_floats, void* stream) {
+  SX_REQUIRE(part && part_floats >= 1, "sx_dot: needs scratch");
+  const int grid = std::min(grid_for_rows(n, 256 * 8, sms_cached()), part_slots(part_floats, 1));
+  dot_kernel<<<grid, 256, 0, ST(stream)>>>(x, y, n, part);
   SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return part_reduce(part, grid, 1, PartDst{{out, nullptr, nullptr, nullptr}, {1, 0, 0, 0}}, ST(stream));
 }
 
 extern "C" int sx_scale(const float* x, int64_t n, const float* alpha_dev, float alpha, float* y, void* stream) {
@@ -1607,23 +1418,22 @@ extern "C" int sx_rowsum(const float* X, int64_t R, int64_t C, int64_t ld, int32
 extern "C" int sx_colsum_batched(const float* X, int32_t Z1, int64_t stride_z1, int32_t Z0, int64_t stride_z0, int64_t R,
                                  int32_t C, int64_t ld, float* out, float* part, int64_t part_floats, void* stream) {
   SX_REQUIRE(Z0 >= 1 && Z0 <= 65535 && Z1 >= 1, "sx_colsum_batched: bad batch dims");
-  int gy = (int)((R + 255) / 256);
-  if (gy > 32) gy = 32;
-  if (gy < 1) gy = 1;
-  dim3 grid(sx_ceil_div(C, 32), gy, Z0), blk(32, 8);
+  const int slots = part_slots(part_floats, (long long)Z0 * C);
+  SX_REQUIRE(part && slots >= 1, "sx_colsum_batched: needs at least %lld floats of scratch", (long long)Z0 * C);
+  dim3 blk(32, 8);
+  int gy;
   if (C % 4 == 0 && ld % 4 == 0 && stride_z0 % 4 == 0 && stride_z1 % 4 == 0 && al16(X)) {
-    int gy4 = (int)((R + 127) / 128);
+    gy = (int)((R + 127) / 128);
     const int cap = sx_ceil_div(sms_cached() * 8, sx_ceil_div(C, 128) * Z0);
-    if (gy4 > cap) gy4 = cap;
-    gy4 = std::min(gy4, part_slots(part_floats, (long long)Z0 * C));
-    SX_REQUIRE(part && gy4 >= 1, "sx_colsum_batched: needs at least %lld floats of scratch", (long long)Z0 * C);
-    colsum_v4_kernel<<<dim3(sx_ceil_div(C, 128), gy4, Z0), blk, 0, ST(stream)>>>(X, Z1, stride_z1, stride_z0, R, C, ld, part);
-    SX_CHECK_CUDA(cudaGetLastError());
-    return part_reduce(part, gy4, Z0 * C, PartDst{{out, nullptr, nullptr, nullptr}, {Z0 * C, 0, 0, 0}}, ST(stream));
-  } else
-    colsum_batched_kernel<<<grid, blk, 0, ST(stream)>>>(X, Z1, stride_z1, stride_z0, R, C, ld, out);
+    if (gy > cap) gy = cap;
+    gy = std::min(gy, slots);
+    colsum_v4_kernel<<<dim3(sx_ceil_div(C, 128), gy, Z0), blk, 0, ST(stream)>>>(X, Z1, stride_z1, stride_z0, R, C, ld, part);
+  } else {
+    gy = std::max(1, std::min({(int)std::min<long long>((R + 255) / 256, 32), slots}));
+    colsum_kernel<<<dim3(sx_ceil_div(C, 32), gy, Z0), blk, 0, ST(stream)>>>(X, Z1, stride_z1, stride_z0, R, C, ld, part);
+  }
   SX_CHECK_CUDA(cudaGetLastError());
-  return 0;
+  return part_reduce(part, gy, Z0 * C, PartDst{{out, nullptr, nullptr, nullptr}, {Z0 * C, 0, 0, 0}}, ST(stream));
 }
 
 namespace {
@@ -1652,8 +1462,7 @@ extern "C" int sx_add(const float* a, const float* b, int64_t n, float* y, void*
 }
 
 extern "C" int sx_softmax_posbias_fwd(const float* S, int64_t R, int32_t L, int64_t lds, const float* amax, float clip,
-                                      float drop_p, uint64_t seed, const uint64_t* seed_dev, void* P, int32_t p_dtype,
-                                      int64_t ldp, int32_t round_tf32, float* lse, float* diag, const sx_posbias* posbias,
+                                      float drop_p, uint64_t seed, const uint64_t* seed_dev, float* P, int64_t ldp, int32_t round_tf32, float* lse, float* diag, const sx_posbias* posbias,
                                       void* stream) {
   const char* err = sxpb::check(posbias, L);
   SX_REQUIRE(err == nullptr, "sx_softmax_posbias_fwd: %s", err);
@@ -1662,24 +1471,17 @@ extern "C" int sx_softmax_posbias_fwd(const float* S, int64_t R, int32_t L, int6
   const size_t smem = (size_t)(32 + L) * 4;
   SX_REQUIRE(smem <= 200 * 1024, "sx_softmax_posbias_fwd: L=%d too large", L);
   const int grid = (int)std::min<long long>(R, (long long)sms_cached() * 8);
-  if (p_dtype == SX_F32) {
-    if (set_smem(softmax_posbias_fwd_kernel<float>, smem)) return -2;
-    softmax_posbias_fwd_kernel<float><<<grid, PB_THREADS, smem, ST(stream)>>>(
-        S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, (float*)P, ldp, lse, round_tf32, diag,
-        posbias->table, G);
-  } else {
-    if (set_smem(softmax_posbias_fwd_kernel<__nv_bfloat16>, smem)) return -2;
-    softmax_posbias_fwd_kernel<__nv_bfloat16><<<grid, PB_THREADS, smem, ST(stream)>>>(
-        S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, (__nv_bfloat16*)P, ldp, lse, 0, diag,
-        posbias->table, G);
-  }
+  if (set_smem(softmax_posbias_fwd_kernel, smem)) return -2;
+  softmax_posbias_fwd_kernel<<<grid, PB_THREADS, smem, ST(stream)>>>(
+      S, R, L, lds, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, P, ldp, lse, round_tf32, diag,
+      posbias->table, G);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
 extern "C" int sx_softmax_posbias_bwd(const float* dP, int64_t ldd, const float* S, int64_t lds, const float* lse, int64_t R,
                                       int32_t L, const float* amax, float clip, float drop_p, uint64_t seed,
-                                      const uint64_t* seed_dev, int64_t ldp_fwd, void* dS, int32_t ds_dtype, int64_t ldo,
+                                      const uint64_t* seed_dev, int64_t ldp_fwd, float* dS, int64_t ldo,
                                       int32_t round_tf32, const sx_posbias* posbias, float* dtable, float* part,
                                       int64_t part_floats, void* stream) {
   const char* err = sxpb::check(posbias, L);
@@ -1691,17 +1493,10 @@ extern "C" int sx_softmax_posbias_bwd(const float* dP, int64_t ldd, const float*
   const size_t smem = (size_t)(32 + G.T + 2 * (size_t)L) * 4;
   SX_REQUIRE(smem <= 200 * 1024, "sx_softmax_posbias_bwd: L=%d too large", L);
   const int grid = (int)std::min<long long>(std::min<long long>(R, (long long)sms_cached() * 4), part_slots(part_floats, G.T));
-  if (ds_dtype == SX_F32) {
-    if (set_smem(softmax_posbias_bwd_kernel<float>, smem)) return -2;
-    softmax_posbias_bwd_kernel<float><<<grid, PB_THREADS, smem, ST(stream)>>>(
-        dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, ldp_fwd, (float*)dS, ldo,
-        round_tf32, posbias->table, G, part);
-  } else {
-    if (set_smem(softmax_posbias_bwd_kernel<__nv_bfloat16>, smem)) return -2;
-    softmax_posbias_bwd_kernel<__nv_bfloat16><<<grid, PB_THREADS, smem, ST(stream)>>>(
-        dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, ldp_fwd,
-        (__nv_bfloat16*)dS, ldo, 0, posbias->table, G, part);
-  }
+  if (set_smem(softmax_posbias_bwd_kernel, smem)) return -2;
+  softmax_posbias_bwd_kernel<<<grid, PB_THREADS, smem, ST(stream)>>>(
+      dP, ldd, S, lds, lse, R, L, amax, clip, drop_p, seed, (const unsigned long long*)seed_dev, ldp_fwd, dS, ldo,
+      round_tf32, posbias->table, G, part);
   SX_CHECK_CUDA(cudaGetLastError());
   return part_reduce(part, grid, G.T, PartDst{{dtable, nullptr, nullptr, nullptr}, {G.T, 0, 0, 0}}, ST(stream));
 }

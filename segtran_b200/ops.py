@@ -366,7 +366,7 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
                preact: Optional[torch.Tensor] = None, accumulate: bool = False, split_k: Optional[int] = None,
                amax: Optional[torch.Tensor] = None, drop_p: float = 0.0, seed: int = 0, round_out: bool = True,
                reduce_z1: bool = False, addend: Optional[torch.Tensor] = None,
-               gelu_bwd: Optional[torch.Tensor] = None, colsum: Optional[torch.Tensor] = None) -> torch.Tensor:
+               gelu_bwd: Optional[torch.Tensor] = None) -> torch.Tensor:
     """a [..., M, K], b [..., N, K] (strided fp32 views; either dim may be the contiguous one) ->
     out [z1, z0, M, N] fp32.  With reduce_z1 the z1 batch dim is summed into one output (atomic accumulate)."""
     _req_cuda(a, b, out, bias, preact, amax)
@@ -437,17 +437,11 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
         g.amax = amax.data_ptr()
     g.drop_p = drop_p
     g.drop_seed, g.drop_seed_dev = _seed_args(seed)
-    if colsum is not None:
-        if colsum.dtype != torch.float32 or colsum.numel() != N or not colsum.is_contiguous() or accumulate or reduce_z1:
-            raise L.SxError("gemm_nt: colsum must be a contiguous fp32 [N] tensor, without accumulate / reduce_z1")
     if addend is not None:
         if addend.dtype != torch.float32 or tuple(addend.shape[-2:]) != (M, N) or _as4(addend).stride() != o4.stride():
             raise L.SxError("gemm_nt: addend must be an fp32 tensor in the output's layout")
         g.addend = addend.data_ptr()
     L.call("sx_gemm", C.byref(g), _stream())
-    if colsum is not None:                   # column sums of the stored values, in a fixed order (sx_colsum)
-        o2 = o4.view(-1, N)
-        L.call("sx_colsum", o2.data_ptr(), L.SX_F32, o2.shape[0], N, o2.stride(0), colsum.data_ptr(), *_part_args(o2.device), _stream())
     if round_after and fresh:                # (caller-provided accumulators are gradient buffers: never rounded)
         L.call("sx_convert", out.data_ptr(), L.SX_F32, out.numel(), out.data_ptr(), L.SX_F32, 1, _stream())
     return out
@@ -458,21 +452,20 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] = N
             preact: Optional[torch.Tensor] = None, accumulate: bool = False, split_k: Optional[int] = None,
             amax: Optional[torch.Tensor] = None, drop_p: float = 0.0, seed: int = 0, round_out: bool = True,
             reduce_z1: bool = False, gelu_bwd: Optional[torch.Tensor] = None,
-            addend: Optional[torch.Tensor] = None, colsum: Optional[torch.Tensor] = None,
-            tag: str = "big") -> torch.Tensor:
+            addend: Optional[torch.Tensor] = None, tag: str = "big") -> torch.Tensor:
     """C[..., m, n] = epilogue(alpha * sum_k a[..., m, k] b[..., n, k]) on the wgmma GEMM.  One launch on TF32-rounded
     operands, or — in 'tf32x3' mode / for call-site classes the precision policy maps to it — three passes on the hi/lo
     operand splits (fp32-grade products)."""
     if not _three_pass(tag):
         return _gemm_nt_1(a, b, out=out, alpha=alpha, bias=bias, bias_mode=bias_mode, gelu=gelu, preact=preact,
                           accumulate=accumulate, split_k=split_k, amax=amax, drop_p=drop_p, seed=seed,
-                          round_out=round_out, reduce_z1=reduce_z1, gelu_bwd=gelu_bwd, addend=addend, colsum=colsum)
+                          round_out=round_out, reduce_z1=reduce_z1, gelu_bwd=gelu_bwd, addend=addend)
     _req_cuda(a, b)
     # ONE launch over K-concatenated operand splits: [A_hi | A_lo | A_hi] . [B_hi | B_hi | B_lo]^T (fp32 accumulation in registers
     # over the three partial products), so every epilogue / accumulate / split-K option works unchanged
     return _gemm_nt_1(_split_cat(a, 0), _split_cat(b, 1), out=out, alpha=alpha, bias=bias, bias_mode=bias_mode, gelu=gelu,
                       preact=preact, accumulate=accumulate, split_k=split_k, amax=amax, drop_p=drop_p, seed=seed,
-                      round_out=round_out, reduce_z1=reduce_z1, gelu_bwd=gelu_bwd, addend=addend, colsum=colsum)
+                      round_out=round_out, reduce_z1=reduce_z1, gelu_bwd=gelu_bwd, addend=addend)
 
 
 def _split_cat(t: torch.Tensor, role: int) -> torch.Tensor:
@@ -583,7 +576,8 @@ def colsum(x2d: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tenso
     """out[c] += sum_r x2d[r, c] (rows uniformly strided)."""
     if out is None:
         out = _zeros((x2d.shape[1],), x2d.device)
-    L.call("sx_colsum", x2d.data_ptr(), L.SX_F32, x2d.shape[0], x2d.shape[1], x2d.stride(0), out.data_ptr(), *_part_args(x2d.device), _stream())
+    L.call("sx_colsum_batched", x2d.data_ptr(), 1, 0, 1, 0, x2d.shape[0], x2d.shape[1], x2d.stride(0), out.data_ptr(),
+           *_part_args(x2d.device), _stream())
     return out
 
 
@@ -620,8 +614,8 @@ class _Linear(torch.autograd.Function):
         dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
         if gelu:
             dh = torch.empty_like(dy2)
-            L.call("sx_gelu_bwd", dy2.data_ptr(), h.data_ptr(), L.SX_F32, dy2.numel(), drop_p, *_seed_args(seed), dh.data_ptr(),
-                   L.SX_F32, _rt(), _stream())
+            L.call("sx_gelu_bwd", dy2.data_ptr(), h.data_ptr(), dy2.numel(), drop_p, *_seed_args(seed), dh.data_ptr(), _rt(),
+                   _stream())
             dy2 = dh
         dx = dW = db = None
         if ctx.needs_input_grad[0]:
@@ -862,7 +856,7 @@ class _Softmax(torch.autograd.Function):
         R = S.numel() // Lr
         P = _rowpad_empty(S.shape, S.device)
         lse = torch.empty(R, device=S.device, dtype=torch.float32)
-        L.call("sx_softmax_fwd", S.data_ptr(), R, Lr, ld, _ptr(amax), clip, drop_p, *_seed_args(seed), P.data_ptr(), L.SX_F32,
+        L.call("sx_softmax_fwd", S.data_ptr(), R, Lr, ld, _ptr(amax), clip, drop_p, *_seed_args(seed), P.data_ptr(),
                P.stride(-2), _rt(), lse.data_ptr(), _ptr(diag), _stream())
         ctx.save_for_backward(S, lse, amax)
         ctx.meta = (clip, drop_p, seed, P.stride(-2))
@@ -877,7 +871,7 @@ class _Softmax(torch.autograd.Function):
         R = S.numel() // Lr
         dS = _rowpad_empty(S.shape, S.device)
         L.call("sx_softmax_bwd", dP.data_ptr(), dP.stride(-2), S.data_ptr(), S.stride(-2), lse.data_ptr(), R, Lr,
-               _ptr(amax), clip, drop_p, *_seed_args(seed), ldp, dS.data_ptr(), L.SX_F32, dS.stride(-2), _rt(), _stream())
+               _ptr(amax), clip, drop_p, *_seed_args(seed), ldp, dS.data_ptr(), dS.stride(-2), _rt(), _stream())
         return dS, None, None, None, None, None
 
 
@@ -890,7 +884,7 @@ def softmax_posbias_backward(dP, ldd, S, lds, lse, R, Lr, amax, clip, drop_p, se
     buf = tgt if tgt is not None else _zeros((table.numel(),), table.device)
     desc = _posbias_desc(table, R_, grid, w)
     L.call("sx_softmax_posbias_bwd", dP.data_ptr(), ldd, S.data_ptr(), lds, lse.data_ptr(), R, Lr, _ptr(amax), clip, drop_p,
-           *_seed_args(seed), ldp_fwd, dS.data_ptr(), L.SX_F32, ldo, _rt(), C.byref(desc), buf.data_ptr(),
+           *_seed_args(seed), ldp_fwd, dS.data_ptr(), ldo, _rt(), C.byref(desc), buf.data_ptr(),
            *_part_args(dS.device), _stream())
     if tgt is not None or not table_needs_grad:
         return None
@@ -910,7 +904,7 @@ class _SoftmaxPosBias(torch.autograd.Function):
         lse = torch.empty(R, device=S.device, dtype=torch.float32)
         desc = _posbias_desc(table, *pb_geom)
         L.call("sx_softmax_posbias_fwd", S.data_ptr(), R, Lr, ld, _ptr(amax), clip, drop_p, *_seed_args(seed), P.data_ptr(),
-               L.SX_F32, P.stride(-2), _rt(), lse.data_ptr(), _ptr(diag), C.byref(desc), _stream())
+               P.stride(-2), _rt(), lse.data_ptr(), _ptr(diag), C.byref(desc), _stream())
         ctx.save_for_backward(S, lse, amax, table)
         ctx.meta = (clip, drop_p, seed, P.stride(-2), pb_geom)
         ctx.leaf = table
@@ -990,8 +984,8 @@ class _AttnPVGelu(torch.autograd.Function):
         B, _, U1, U2 = P.shape
         dG = dG.contiguous()
         dH = torch.empty_like(dG)
-        L.call("sx_gelu_bwd", dG.data_ptr(), H.data_ptr(), L.SX_F32, dG.numel(), drop_p, *_seed_args(ctx.seed),
-               dH.data_ptr(), L.SX_F32, _rt(), _stream())
+        L.call("sx_gelu_bwd", dG.data_ptr(), H.data_ptr(), dG.numel(), drop_p, *_seed_args(ctx.seed), dH.data_ptr(), _rt(),
+               _stream())
         dP = dv = db = None
         if ctx.needs_input_grad[0]:
             dP = _rowpad_empty((B, M, U1, U2), P.device)
@@ -1099,13 +1093,14 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
         dP = dv = dbm = dW = dbo = None
         # dH = mask * (dY Wo) * gelu'(H), TF32-rounded for the two GEMMs that consume it
         dH = torch.empty_like(H)
-        # ... and the column sums of dH (= the gradient of MMSharedMid's bias) are accumulated by the same epilogue
         dbm_buf = None
         if has_bm and ctx.needs_input_grad[3]:
             tgt = _grad_target(bm)
             dbm_buf = tgt if tgt is not None else _zeros((Fd,), dY.device)
             dbm = None if tgt is not None else dbm_buf
-        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=ctx.seed, colsum=dbm_buf)
+        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=ctx.seed)
+        if dbm_buf is not None:             # column sums of dH = the gradient of MMSharedMid's bias
+            colsum(dH.view(-1, Fd), out=dbm_buf)
         if ctx.needs_input_grad[6]:
             tgt = _grad_target(Wo)
             if tgt is not None:
@@ -1153,7 +1148,7 @@ class _SqueezeOutFused(torch.autograd.Function):
     (:447, :243-245, :267) as ONE autograd node:
       forward : sx_attn_probs_fwd (wgmma scores -> in-register softmax -> P)  ->  P.V' GEMM (bias/GELU/dropout epilogue)
                 -> grouped output Linear;
-      backward: dH GEMM (GELU'/dropout epilogue + bias-gradient column sums) -> dP GEMM -> sx_softmax_bwd on the saved raw
+      backward: dH GEMM (GELU'/dropout epilogue) -> bias-gradient column sums -> dP GEMM -> sx_softmax_bwd on the saved raw
                 scores (P recomputed from S and the row log-sum-exp, the row term sum_a P_a dP_a taken from the SAME dP values
                 it is subtracted from) -> dV', dQ, dK, dWo, dbo products.
     A flash-attention style backward (row term from sum_f dU_f U_f in the dH epilogue, softmax backward in the dP GEMM
@@ -1195,14 +1190,16 @@ class _SqueezeOutFused(torch.autograd.Function):
         Bq, d = q.shape[0], q.shape[-1] // M
         dY = dY.contiguous()
         dq = dk = dvp = dbm = dW = dbo = None
-        # dH = mask * (dY Wo) * gelu'(H); the same epilogue accumulates the column sums of dH (MMSharedMid's bias gradient)
+        # dH = mask * (dY Wo) * gelu'(H), then the column sums of dH (MMSharedMid's bias gradient)
         dH = torch.empty_like(H)
         dbm_buf = None
         if has_bm and ctx.needs_input_grad[7]:
             tgt = _grad_target(bm)
             dbm_buf = tgt if tgt is not None else _zeros((Fd,), dY.device)
             dbm = None if tgt is not None else dbm_buf
-        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=hid_p, seed=hid_seed, colsum=dbm_buf)
+        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=hid_p, seed=hid_seed)
+        if dbm_buf is not None:
+            colsum(dH.view(-1, Fd), out=dbm_buf)
         if ctx.needs_input_grad[10]:
             tgt = _grad_target(Wo)
             if tgt is not None:
@@ -1229,7 +1226,7 @@ class _SqueezeOutFused(torch.autograd.Function):
                                               ld, table, pb_geom, ctx.needs_input_grad[13])
             else:
                 L.call("sx_softmax_bwd", dP.data_ptr(), ld, S.data_ptr(), ld, lse.data_ptr(), B * M * U1, U2,
-                       stat[2:].data_ptr(), clip, att_p, *_seed_args(att_seed), ld, dS.data_ptr(), L.SX_F32, ld, _rt(), _stream())
+                       stat[2:].data_ptr(), clip, att_p, *_seed_args(att_seed), ld, dS.data_ptr(), ld, _rt(), _stream())
             scale = 1.0 / math.sqrt(d)
             if ctx.needs_input_grad[0]:
                 bcast = Bq == 1 and B > 1
@@ -1265,7 +1262,7 @@ class _LayerNorm(torch.autograd.Function):
         R = x.numel() // Cd
         y = torch.empty_like(x)
         stats = torch.empty((R, 2), device=x.device, dtype=torch.float32)
-        L.call("sx_layernorm_fwd", x.data_ptr(), R, Cd, g.data_ptr(), b.data_ptr(), y.data_ptr(), L.SX_F32, rnd,
+        L.call("sx_layernorm_fwd", x.data_ptr(), R, Cd, g.data_ptr(), b.data_ptr(), y.data_ptr(), rnd,
                stats.data_ptr(), _stream())
         ctx.save_for_backward(x, g, stats)
         ctx.leaves = (g, b)
@@ -1281,7 +1278,7 @@ class _LayerNorm(torch.autograd.Function):
         dgb, dg = _sink_or_zeros(ctx.leaves[0])
         dbb, db = _sink_or_zeros(ctx.leaves[1])
         L.call("sx_layernorm_bwd", dy.data_ptr(), x.data_ptr(), R, Cd, g.data_ptr(), stats.data_ptr(), dx.data_ptr(),
-               L.SX_F32, ctx.rnd_bwd, dgb.data_ptr(), dbb.data_ptr(), *_part_args(dy.device), _stream())
+               ctx.rnd_bwd, dgb.data_ptr(), dbb.data_ptr(), *_part_args(dy.device), _stream())
         return dx, dg, db, None, None
 
 
@@ -1353,10 +1350,9 @@ class _LnSoftAggr(torch.autograd.Function):
         dbb, db = _sink_or_zeros(ctx.leaves[1])
         dwsb, dws = _sink_or_zeros(ctx.leaves[2])
         dbsb, dbs = _sink_or_zeros(ctx.leaves[3])
-        scratch = torch.empty(B * M * N, device=Y.device, dtype=torch.float32)
         L.call("sx_ln_softaggr_bwd", dout.data_ptr(), Y.data_ptr(), B, M, N, Fd, g.data_ptr(), b.data_ptr(),
-               ws.data_ptr(), drop_p, *_seed_args(seed), stats.data_ptr(), wts.data_ptr(), dY.data_ptr(), L.SX_F32, _rt(), dgb.data_ptr(),
-               dbb.data_ptr(), dwsb.data_ptr(), dbsb.data_ptr(), scratch.data_ptr(), *_part_args(dout.device), _stream())
+               ws.data_ptr(), drop_p, *_seed_args(seed), stats.data_ptr(), wts.data_ptr(), dY.data_ptr(), _rt(), dgb.data_ptr(),
+               dbb.data_ptr(), dwsb.data_ptr(), dbsb.data_ptr(), *_part_args(dout.device), _stream())
         return dY, dg, db, dws, dbs, None, None
 
 
@@ -1447,7 +1443,7 @@ class _Prologue(torch.autograd.Function):
         h = torch.empty_like(x)
         stats = torch.empty((B * N, 4), device=x.device, dtype=torch.float32)
         L.call("sx_prologue_fwd", x.data_ptr(), B, N, Cd, g.data_ptr(), b.data_ptr(), _ptr(pe), C0, pe_bstride,
-               posw, _ptr(mask), drop_p, *_seed_args(seed), h.data_ptr(), L.SX_F32, _rt(), stats.data_ptr(), _stream())
+               posw, _ptr(mask), drop_p, *_seed_args(seed), h.data_ptr(), _rt(), stats.data_ptr(), _stream())
         ctx.save_for_backward(x, g, b, pe, mask, stats)
         ctx.meta = (posw, drop_p, seed, pe_bstride)
         ctx.leaves = (g, b)
@@ -1496,7 +1492,7 @@ class _Dot(torch.autograd.Function):
     def forward(ctx, x, w):
         x = x.contiguous()
         out = _zeros((1,), x.device)
-        L.call("sx_dot", x.data_ptr(), w.data_ptr(), x.numel(), out.data_ptr(), _stream())
+        L.call("sx_dot", x.data_ptr(), w.data_ptr(), x.numel(), out.data_ptr(), *_part_args(x.device), _stream())
         ctx.save_for_backward(w)
         ctx.shape = x.shape
         return out
@@ -1809,7 +1805,7 @@ class _AttnProbs(torch.autograd.Function):
                                           ctx.seed, ldp, dS, dS.stride(-2), table, pb_geom, ctx.needs_input_grad[8])
         else:
             L.call("sx_softmax_bwd", dP.data_ptr(), dP.stride(-2), S.data_ptr(), S.stride(-2), lse.data_ptr(), B * M * U1, U2,
-                   stat[2:].data_ptr(), clip, drop_p, *_seed_args(ctx.seed), ldp, dS.data_ptr(), L.SX_F32, dS.stride(-2),
+                   stat[2:].data_ptr(), clip, drop_p, *_seed_args(ctx.seed), ldp, dS.data_ptr(), dS.stride(-2),
                    _rt(), _stream())
         dq, dk = _score_grads(dS, q, k, M, alpha, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         return dq, dk, None, None, None, None, None, None, dT, None
@@ -1878,7 +1874,8 @@ class _HeadContract(torch.autograd.Function):
             dWcb = gemm_nt(dL.view(B, 1, K, V), curr.view(B, 1, Cf, V), reduce_z1=True, round_out=False).view(K, Cf)
         else:                                         # TMA needs 16-byte row pitches: CUDA-core reduction instead
             dWcb = _zeros((K, Cf), curr.device)
-            L.call("sx_head_contract_bwd_weight", dL.data_ptr(), curr.data_ptr(), B, Cf, V, K, dWcb.data_ptr(), _stream())
+            L.call("sx_head_contract_bwd_weight", dL.data_ptr(), curr.data_ptr(), B, Cf, V, K, dWcb.data_ptr(),
+                   *_part_args(dL.device), _stream())
         dcc = _zeros((K,), curr.device)               # d(const)[k] = sum_{b,v} dL
         L.call("sx_rowsum", dL.data_ptr(), B * K, V, V, K, dcc.data_ptr(), *_part_args(dL.device), _stream())
         if Wb2 is not None:

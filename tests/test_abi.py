@@ -27,11 +27,11 @@ def test_library_exports_every_declared_symbol():
     assert l.sx_version() == 1
 
 
-def test_gemm_args_struct_layout_matches_header():
+def test_gemm_args_layout_matches_header():
     import ctypes as C
     from segtran_b200 import _lib
     assert C.sizeof(_lib.sx_operand) == 40
-    assert C.sizeof(_lib.sx_gemm_args) == 264 and _lib.sx_gemm_args.part.offset == 248
+    assert C.sizeof(_lib.sx_gemm_args) == 256 and _lib.sx_gemm_args.part.offset == 240
     assert _lib.sx_gemm_args.A.offset == 24 and _lib.sx_gemm_args.C.offset == 104
 
 

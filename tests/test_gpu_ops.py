@@ -115,7 +115,7 @@ def test_epilogue_gelu_matches_fp64_erf():
     assert float(err.max()) < 4e-7, float(err.max())
 
 
-def test_gemm_gelu_bwd_epilogue_equals_separate_pass():
+def test_gemm_gelu_bwd_epilogue_equals_separate_gelu_bwd_and_colsum():
     """SX_ACT_GELU_BWD: C = dropmask * (A B^T) * gelu'(h) in the GEMM epilogue == plain GEMM followed by sx_gelu_bwd with
     the same seed (bit-for-bit the same mask), and == the analytic fp64 expression when dropout is off."""
     import segtran_b200._lib as L
@@ -131,15 +131,16 @@ def test_gemm_gelu_bwd_epilogue_equals_separate_pass():
     fused = ops.gemm_nt(a, b, gelu_bwd=h, drop_p=0.3, seed=seed, round_out=False)
     plain = ops.gemm_nt(a, b, round_out=False)
     sep = torch.empty_like(plain)
-    L.call("sx_gelu_bwd", plain.data_ptr(), h.data_ptr(), L.SX_F32, plain.numel(), 0.3, 0, seed.data_ptr(),
-           sep.data_ptr(), L.SX_F32, 0, torch.cuda.current_stream().cuda_stream)
+    L.call("sx_gelu_bwd", plain.data_ptr(), h.data_ptr(), plain.numel(), 0.3, 0, seed.data_ptr(), sep.data_ptr(), 0,
+           torch.cuda.current_stream().cuda_stream)
     assert torch.equal(fused == 0, sep == 0)
     close(fused.double(), sep.double(), 1e-6)
     frac = float((fused == 0).float().mean())
     assert abs(frac - 0.3) < 0.01
-    # column sums of the stored values (bias gradient) accumulated by the same epilogue, on top of what is already there
+    # column sums of the stored values (bias gradient), accumulated on top of what is already there
     cs = torch.ones(136, device="cuda")
-    out = ops.gemm_nt(a, b, gelu_bwd=h, drop_p=0.3, seed=seed, round_out=False, colsum=cs)
+    out = ops.gemm_nt(a, b, gelu_bwd=h, drop_p=0.3, seed=seed, round_out=False)
+    ops.colsum(out.view(-1, 136), out=cs)
     close(cs.double(), 1.0 + out.double().sum(dim=(0, 1, 2)), 1e-5)
 
 

@@ -52,7 +52,8 @@ def cases():
         ops.gemm_nt(P, ops._bank_operand(vp, B, U2, M, FD), out=G, bias=bm, gelu=True, preact=H, drop_p=0.2, seed=7)
 
     def dh():
-        ops.gemm_nt(dY, ops._weight_t(Wr, M, FD, FD).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=0.2, seed=7, colsum=dbm)
+        ops.gemm_nt(dY, ops._weight_t(Wr, M, FD, FD).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=0.2, seed=7)
+        ops.colsum(dH.view(-1, FD), out=dbm)
 
     def dqf():
         ops.gemm_nt(P, ops._bank_operand(k, B, U2, M, D), out=dq.view(B, U1, M, D).permute(0, 2, 1, 3), alpha=0.0625,
