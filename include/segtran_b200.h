@@ -305,7 +305,8 @@ int sx_softaggr_fwd(const float* x, int32_t B, int32_t M, int32_t N, int32_t F, 
                     float* wts, void* stream);
 int sx_softaggr_bwd(const float* dout, const float* x, int32_t B, int32_t M, int32_t N, int32_t F, const float* ws,
                     const float* wts, float* dx, float* dscore, void* stream);
-/* dH = dropout'(dG) * gelu'(H)  (MMSharedMid backward, segtran_shared.py:243-245) */
+/* dH = dropout'(dG) * gelu'(H)  (MMSharedMid backward, segtran_shared.py:243-245); H == NULL: dH = dropout'(dG), the
+   backward of a dropout epilogue without an activation (MultiHeadFeatTrans's output Linear, segtran_ablation.py:137-143) */
 int sx_gelu_bwd(const float* dG, const float* H, int64_t n, float drop_p, uint64_t seed, const uint64_t* seed_dev, float* dH,
                 int32_t round_tf32, void* stream);
 /* dtype conversion / TF32 rounding of a flat buffer (weights once per step) */

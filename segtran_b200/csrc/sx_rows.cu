@@ -699,7 +699,9 @@ __global__ void ln_softaggr_bwd_kernel(const float* __restrict__ dout, const flo
 // ------------------------------------------------------------------------------------------------
 // elementwise helpers
 // ------------------------------------------------------------------------------------------------
-// dH = dGd * keep/(1-p) * gelu'(H)   (MMSharedMid backward, segtran_shared.py:243-245)
+// dH = dGd * keep/(1-p) * gelu'(H)   (MMSharedMid backward, segtran_shared.py:243-245); GELU = false: dH = dGd * keep/(1-p),
+// the backward of a dropout epilogue without an activation (the output Linear of MultiHeadFeatTrans, segtran_ablation.py:137-143)
+template <bool GELU>
 __global__ void gelu_bwd_kernel(const float* __restrict__ dG, const float* __restrict__ H, long long n, float drop_p,
                                 unsigned long long seed, const unsigned long long* __restrict__ seed_dev, float* __restrict__ dH, int rnd) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
@@ -707,11 +709,13 @@ __global__ void gelu_bwd_kernel(const float* __restrict__ dG, const float* __res
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float d = dG[i];
     if (drop_p > 0.f) d = sx::drop_keep1(seed, (unsigned long long)i, sx::drop_p16(drop_p)) ? d * keep_scale : 0.f;
-    dH[i] = rnd1(d * sx::gelu_erf_grad(H[i]), rnd);
+    if constexpr (GELU) d *= sx::gelu_erf_grad(H[i]);
+    dH[i] = rnd1(d, rnd);
   }
 }
 
 // fp32 float4 version (n % 4 == 0, 16-byte aligned)
+template <bool GELU>
 __global__ void gelu_bwd_f4_kernel(const float4* __restrict__ dG, const float4* __restrict__ H, long long n4, float drop_p,
                                    unsigned long long seed, const unsigned long long* __restrict__ seed_dev, float4* __restrict__ dH, int rnd) {
   seed += seed_dev ? *seed_dev : 0ull;      // per-call device seed (CUDA-graph safe)
@@ -719,8 +723,10 @@ __global__ void gelu_bwd_f4_kernel(const float4* __restrict__ dG, const float4* 
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 d = dG[i];
     if (drop_p > 0.f) d = drop4(d, drop_p, keep_scale, seed, (unsigned long long)(i * 4));
-    const float4 h = H[i];
-    d.x *= sx::gelu_erf_grad(h.x); d.y *= sx::gelu_erf_grad(h.y); d.z *= sx::gelu_erf_grad(h.z); d.w *= sx::gelu_erf_grad(h.w);
+    if constexpr (GELU) {
+      const float4 h = H[i];
+      d.x *= sx::gelu_erf_grad(h.x); d.y *= sx::gelu_erf_grad(h.y); d.z *= sx::gelu_erf_grad(h.z); d.w *= sx::gelu_erf_grad(h.w);
+    }
     dH[i] = rnd4(d, rnd);
   }
 }
@@ -1312,12 +1318,16 @@ extern "C" int sx_ln_softaggr_bwd(const float* dout, const float* Y, int32_t B, 
 
 extern "C" int sx_gelu_bwd(const float* dG, const float* H, int64_t n, float drop_p, uint64_t seed, const uint64_t* seed_dev,
                            float* dH, int32_t round_tf32, void* stream) {
-  if (n % 4 == 0 && al16(dG) && al16(H) && al16(dH))
-    gelu_bwd_f4_kernel<<<grid_for_rows(n / 4, 256 * 4, sms_cached()), 256, 0, ST(stream)>>>(
-        (const float4*)dG, (const float4*)H, n / 4, drop_p, seed, (const unsigned long long*)seed_dev, (float4*)dH, round_tf32);
-  else
-    gelu_bwd_kernel<<<grid_for_rows(n, 256 * 8, sms_cached()), 256, 0, ST(stream)>>>(
-        dG, H, n, drop_p, seed, (const unsigned long long*)seed_dev, dH, round_tf32);
+  const auto* sd = (const unsigned long long*)seed_dev;
+  if (n % 4 == 0 && al16(dG) && al16(H) && al16(dH)) {
+    const int grid = grid_for_rows(n / 4, 256 * 4, sms_cached());
+    if (H) gelu_bwd_f4_kernel<true><<<grid, 256, 0, ST(stream)>>>((const float4*)dG, (const float4*)H, n / 4, drop_p, seed, sd, (float4*)dH, round_tf32);
+    else gelu_bwd_f4_kernel<false><<<grid, 256, 0, ST(stream)>>>((const float4*)dG, nullptr, n / 4, drop_p, seed, sd, (float4*)dH, round_tf32);
+  } else {
+    const int grid = grid_for_rows(n, 256 * 8, sms_cached());
+    if (H) gelu_bwd_kernel<true><<<grid, 256, 0, ST(stream)>>>(dG, H, n, drop_p, seed, sd, dH, round_tf32);
+    else gelu_bwd_kernel<false><<<grid, 256, 0, ST(stream)>>>(dG, nullptr, n, drop_p, seed, sd, dH, round_tf32);
+  }
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

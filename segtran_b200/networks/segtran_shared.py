@@ -10,9 +10,10 @@ Supported configuration = the one the reference's drivers force (train3d.py:174-
 squeezed attention (or plain cross attention), pos_code_type 'lsinu', mid_type 'shared',
 trans_output_type 'private'|'shared', tie_qk 'shared'|'loose'|'none', pool_modes_feat 'softmax', plus
 --nosqueeze and --squeezeuseffn, the positional-code ablations --pos bias (sliding-window biases inside the
-attention softmax, plain attention only) and --pos none, and the mince transformer (--mince with --nosqueeze: plain
-attention on several downsampled copies of the token grid).  The other ablation-only switches (multihead, rand/sinu
-position codes) raise NotImplementedError.
+attention softmax, plain attention only) and --pos none, the mince transformer (--mince with --nosqueeze: plain
+attention on several downsampled copies of the token grid) and the multi-head ablation (--multihead with --nosqueeze:
+MultiHeadFeatTrans).  The other ablation-only switches (rand/sinu position codes, mid_type 'private') raise
+NotImplementedError.
 """
 from __future__ import annotations
 
@@ -393,8 +394,110 @@ class ExpandedFeatTrans(nn.Module):
         return self._norm_aggregate(y)
 
 
+# ---------------------------------------------------------------------------------------------------
+# multi-head ablation (--multihead; reference segtran_ablation.py:93-253): parameter holders with the ablation module's
+# names and creation order, built on the layer's config after MultiHeadFeatTrans has set num_modes = 1
+# ---------------------------------------------------------------------------------------------------
+class AblationMMSharedMid(nn.Module):
+    """The ablation's MMSharedMid (segtran_ablation.py:93-121): one Linear(F->F) + erf-GELU, and no dropout."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.num_modes, self.feat_dim = config.num_modes, config.feat_dim
+        self.shared_linear = nn.Linear(self.feat_dim, self.feat_dim)
+        self.mid_act_fn = config.act_fun
+
+
+class AblationMMPrivateOutput(nn.Module):
+    """The ablation's MMPrivateOutput (segtran_ablation.py:125-145) with one mode: Conv1d(F, F, 1) + dropout + LayerNorm;
+    the residual is computed and discarded, as in MMPrivateOutput."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.num_modes, self.feat_dim = config.num_modes, config.feat_dim
+        fam = self.feat_dim * self.num_modes
+        self.group_linear = nn.Conv1d(fam, fam, 1, groups=self.num_modes)
+        self.resout_norm_layer = nn.LayerNorm(self.feat_dim, eps=1e-12, elementwise_affine=True)
+        self.dropout = nn.Dropout(config.hidden_dropout_prob)
+
+
+class AblationMMSharedOutput(nn.Module):
+    """The ablation's MMSharedOutput (segtran_ablation.py:149-178): Linear(F->F) + residual + dropout + LayerNorm; the
+    residual is kept."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.num_modes, self.feat_dim = config.num_modes, config.feat_dim
+        self.shared_linear = nn.Linear(self.feat_dim, self.feat_dim)
+        self.resout_norm_layer = nn.LayerNorm(self.feat_dim, eps=1e-12, elementwise_affine=True)
+        self.dropout = nn.Dropout(config.hidden_dropout_prob)
+
+
+class MultiHeadFeatTrans(nn.Module):
+    """Multi-head attention output in place of the multi-mode expansion (reference segtran_ablation.py:183-253): the M
+    attention modes are M heads of dh = F / M channels.
+        V = x Wv^T + bv  [B,U2,F];  U[:, :, h*dh:(h+1)*dh] = P_h V[:, :, h*dh:(h+1)*dh];  G = gelu(U Wm^T + bm)
+        'private': Y = LN(dropout(G Wo^T + bo))        'shared': Y = LN(dropout(G Ws^T + bs + U))
+    -> [B,U1,F], no soft aggregation.  Not an ExpandedFeatTrans: SegtranInitWeights gives first_linear no identity bias,
+    as in the reference.  Like the reference, it sets num_modes = 1 on the layer's config (its CrossAttFeatTrans has
+    already read M)."""
+
+    def __init__(self, config, name):
+        super().__init__()
+        self.config, self.name = config, name
+        self.in_feat_dim, self.feat_dim, self.num_modes = config.in_feat_dim, config.feat_dim, config.num_modes
+        if self.feat_dim % self.num_modes:
+            # the reference fails at its reshape (segtran_ablation.py:239)
+            raise ValueError("MultiHeadFeatTrans: feat_dim %d is not divisible by %d heads" % (self.feat_dim, self.num_modes))
+        if config.mid_type != 'shared':
+            _unsupported("mid_type=%r with ablate_multihead" % (config.mid_type,))
+        if config.trans_output_type not in ('private', 'shared'):
+            _unsupported("trans_output_type=%r" % (config.trans_output_type,))
+        self.feat_dim_onehead = self.feat_dim // self.num_modes
+        self.feat_dim_allhead = self.feat_dim_onehead * self.num_modes
+        self.first_linear = nn.Linear(self.in_feat_dim, self.feat_dim_allhead)
+        config.num_modes = 1                    # (:203) intermediate and output see one mode
+        self.mid_type = config.mid_type
+        self.intermediate = AblationMMSharedMid(config)
+        if config.trans_output_type == 'shared':
+            self.output = AblationMMSharedOutput(config)
+        else:
+            self.output = AblationMMPrivateOutput(config)
+
+    def supports_fused_attention(self):
+        return True
+
+    def forward_from_qk(self, input_feat, q, k, clip, att_p, diag, posbias=None):
+        """Fused attention entry (the contract of ExpandedFeatTrans.forward_from_qk): the probabilities come from the
+        fused scores / clamp / positional-bias / softmax / dropout kernel (ops.attn_probs)."""
+        M = self.num_modes
+        d = q.shape[-1] // M
+        probs = ops.attn_probs(q, k, M, 1.0 / math.sqrt(d), clip, att_p,
+                               ops.new_dropout_seed(q.device) if att_p > 0 else 0, diag, posbias)
+        return self.forward(input_feat, probs)
+
+    def forward(self, input_feat, attention_probs):
+        """input_feat [B,U2,C]; attention_probs [B,M,U1,U2] -> [B,U1,F] (:228-253)."""
+        v = ops.linear(input_feat, self.first_linear.weight, self.first_linear.bias, tag="proj")       # [B,U2,F]
+        u = ops.attn_pv(attention_probs, v, self.num_modes, heads=True)                                # [B,U1,F]
+        mid = self.intermediate.shared_linear
+        g = ops.linear(u, mid.weight, mid.bias, gelu=True, tag="proj")
+        out = self.output
+        p = out.dropout.p if self.training else 0.0
+        seed = ops.new_dropout_seed(u.device) if p > 0 else 0
+        if isinstance(out, AblationMMSharedOutput):
+            z = ops.linear(g, out.shared_linear.weight, out.shared_linear.bias, drop_p=p, seed=seed, tag="proj",
+                           round_out=False, addend=u)
+        else:
+            z = ops.linear(g, out.group_linear.weight, out.group_linear.bias, drop_p=p, seed=seed, tag="proj",
+                           round_out=False)
+        ln = out.resout_norm_layer
+        return ops.layer_norm(z, ln.weight, ln.bias, round_out=False)
+
+
 class CrossAttFeatTrans(nn.Module):
-    """Cross attention with tied Q/K projection + ExpandedFeatTrans (reference :478-610)."""
+    """Cross attention with tied Q/K projection + ExpandedFeatTrans, or MultiHeadFeatTrans with ablate_multihead
+    (reference :478-610)."""
 
     def __init__(self, config, name):
         super().__init__()
@@ -413,8 +516,9 @@ class CrossAttFeatTrans(nn.Module):
         else:
             self.pos_code_weight = 1
         if config.ablate_multihead:
-            _unsupported("ablate_multihead")
-        self.out_trans = ExpandedFeatTrans(config, name)
+            self.out_trans = MultiHeadFeatTrans(config, name)
+        else:
+            self.out_trans = ExpandedFeatTrans(config, name)
         self.att_dropout = nn.Dropout(config.attention_probs_dropout_prob)
         self.keep_attn_scores = config.use_attn_consist_loss
         self.tie_qk_scheme = config.tie_qk_scheme
@@ -660,6 +764,11 @@ class SqueezedAttFeatTrans(nn.Module):
         self.in_feat_dim, self.num_attractors = config.in_feat_dim, config.num_attractors
         if config.use_mince_transformer:
             _unsupported("the mince transformer")
+        if config.ablate_multihead:
+            raise NotImplementedError("segtran_b200: ablate_multihead with squeezed attention is not implemented (the "
+                                      "reference crashes there: MultiHeadFeatTrans reshapes the attractor-side output "
+                                      "with the token count, segtran_ablation.py:239; its drivers turn --multihead into "
+                                      "--nosqueeze)")
         config1 = copy.copy(config)
         config1.feat_dim = config1.in_feat_dim
         config1.num_modes = 1

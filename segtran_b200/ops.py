@@ -585,11 +585,13 @@ def colsum(x2d: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tenso
 # autograd functions
 # ------------------------------------------------------------------------------------------------
 class _Linear(torch.autograd.Function):
-    """y = dropout(act(x W^T + b)).  nn.Linear call sites segtran_shared.py:243, :414, :559-560.  `tag` = precision class
-    of the three products (forward, dx, dW), see the precision policy above."""
+    """y = dropout(act(x W^T + b [+ addend])).  nn.Linear call sites segtran_shared.py:243, :414, :559-560; a weight with
+    trailing unit dims (a 1x1 Conv1d, [O, I, 1]) is read as [O, I].  addend (shape of y): a residual added before the
+    activation and the dropout (segtran_ablation.py:175-176).  `tag` = precision class of the three products (forward, dx,
+    dW), see the precision policy above."""
 
     @staticmethod
-    def forward(ctx, x, W, b, gelu, drop_p, seed, tag, round_y):
+    def forward(ctx, x, W, b, gelu, drop_p, seed, tag, round_y, addend):
         shp = x.shape
         x2 = x.reshape(-1, shp[-1])
         if not x2.is_contiguous():
@@ -598,50 +600,83 @@ class _Linear(torch.autograd.Function):
         O = W.shape[0]
         y = torch.empty((x2.shape[0], O), device=x.device, dtype=torch.float32)
         h = torch.empty_like(y) if gelu else None
-        gemm_nt(x2, Wr, out=y, bias=b, gelu=gelu, preact=h, drop_p=drop_p, seed=seed, tag=tag, round_out=round_y)
+        a2 = None
+        if addend is not None:
+            a2 = addend.reshape(-1, O)
+            if not a2.is_contiguous():
+                a2 = a2.contiguous()
+        gemm_nt(x2, Wr.view(O, -1), out=y, bias=b, gelu=gelu, preact=h, drop_p=drop_p, seed=seed, tag=tag,
+                round_out=round_y, addend=a2)
         ctx.save_for_backward(x2, Wr, h)
-        ctx.meta = (shp, b is not None, gelu, drop_p, seed, tag)
+        ctx.meta = (shp, b is not None, gelu, drop_p, seed, tag, None if addend is None else addend.shape)
         ctx.leaves = (W, b)
         return y.view(*shp[:-1], O)
 
     @staticmethod
     def backward(ctx, dy):
         x2, Wr, h = ctx.saved_tensors
-        shp, has_b, gelu, drop_p, seed, tag = ctx.meta
+        shp, has_b, gelu, drop_p, seed, tag, add_shape = ctx.meta
         W, b = ctx.leaves
         if _three_pass(tag) and _PRECISION == "tf32":       # 3-pass forward, single-pass backward: TF32-rounded weight
             Wr = round_tf32(W)
+        O = W.shape[0]
+        Wr2 = Wr.view(O, -1)
         dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
-        if gelu:
+        if gelu or drop_p > 0:                              # gelu'(h) and / or the dropout mask (h = None: the mask only)
             dh = torch.empty_like(dy2)
-            L.call("sx_gelu_bwd", dy2.data_ptr(), h.data_ptr(), dy2.numel(), drop_p, *_seed_args(seed), dh.data_ptr(), _rt(),
+            L.call("sx_gelu_bwd", dy2.data_ptr(), _ptr(h), dy2.numel(), drop_p, *_seed_args(seed), dh.data_ptr(), _rt(),
                    _stream())
             dy2 = dh
-        dx = dW = db = None
+        dx = dW = db = da = None
         if ctx.needs_input_grad[0]:
-            dx = gemm_nt(dy2, _weight_t(Wr, 1, *Wr.shape)[0], round_out=False).view(shp)
+            dx = gemm_nt(dy2, _weight_t(Wr2, 1, *Wr2.shape)[0], round_out=False).view(shp)
         if ctx.needs_input_grad[1]:
             tgt = _grad_target(W)
             if tgt is not None:
-                gemm_nt(dy2.t(), x2.t(), out=tgt, accumulate=True, round_out=False)
+                gemm_nt(dy2.t(), x2.t(), out=tgt.view(O, -1), accumulate=True, round_out=False)
             else:
-                dW = gemm_nt(dy2.t(), x2.t(), round_out=False).view(Wr.shape)
+                dW = gemm_nt(dy2.t(), x2.t(), round_out=False).view(W.shape)
         if has_b and ctx.needs_input_grad[2]:
             tgt = _grad_target(b)
             if tgt is not None:
                 colsum(dy2, out=tgt)
             else:
                 db = colsum(dy2)
-        return dx, dW, db, None, None, None, None, None
+        if add_shape is not None and ctx.needs_input_grad[8]:
+            da = dy2.view(add_shape)
+        return dx, dW, db, None, None, None, None, None, da
 
 
-def linear(x, W, b=None, gelu=False, drop_p=0.0, seed=0, tag="big", round_out=True):
-    """round_out: round y to TF32 (set False when every consumer of y is a 3-pass contraction or not a GEMM)."""
-    return _Linear.apply(x, W, b, gelu, drop_p, seed, tag, round_out)
+def linear(x, W, b=None, gelu=False, drop_p=0.0, seed=0, tag="big", round_out=True, addend=None):
+    """round_out: round y to TF32 (set False when every consumer of y is a 3-pass contraction or not a GEMM).
+    addend: a tensor of y's shape added to x W^T + b before the activation and the dropout."""
+    return _Linear.apply(x, W, b, gelu, drop_p, seed, tag, round_out, addend)
+
+
+def _heads_aligned(dh: int, Fd: int) -> bool:
+    """Head slices [., h*dh:(h+1)*dh] of rows of Fd channels start on 16-byte boundaries (TMA) at the GEMM element size."""
+    es = 2 if _PRECISION == "bf16" else 4
+    return (dh * es) % 16 == 0 and (Fd * es) % 16 == 0
+
+
+def _head_rows(x: torch.Tensor, B: int, R: int, M: int, dh: int) -> torch.Tensor:
+    """[B, M, R, dh] K-major operand of the head slices of x [B, R, M*dh]: the strided view, or a copy with 16-byte row
+    pitches when the slices are not TMA-aligned."""
+    v = x.view(B, R, M, dh).permute(0, 2, 1, 3)
+    return v if _heads_aligned(dh, M * dh) else _rowpad(v)
+
+
+def _head_cols(x: torch.Tensor, B: int, R: int, M: int, dh: int, kmajor: bool) -> torch.Tensor:
+    """[B, M, dh, R] "N x K" operand of the head slices of x [B, R, M*dh]: a K-major copy (rows padded to 16 bytes) when
+    `kmajor` or when the slices are not TMA-aligned, else the MN-major view of x."""
+    if kmajor or not _heads_aligned(dh, M * dh):
+        return _transposed(x, B, R, M * dh).unflatten(1, (M, dh))
+    return x.view(B, R, M, dh).permute(0, 2, 3, 1)
 
 
 class _AttnScores(torch.autograd.Function):
     """S[b,m] = scale * Q[b,:,m] K[b,:,m]^T (+ row_bias[u1])   (segtran_shared.py:566-567); tracks max(S) on the device.
+    A per-mode width d that is not a multiple of 4 (16-byte TMA alignment) reads padded copies of the mode slices.
     q may have batch 1 (the batch-invariant attractor queries): it is broadcast, and its gradient reduced over b.
     row_bias [U1] (single-mode only) is the per-query constant of the re-associated in-squeeze (see
     SqueezedAttFeatTrans): it is added after the scaling, so it must already be scaled."""
@@ -652,8 +687,8 @@ class _AttnScores(torch.autograd.Function):
         B, U2 = k.shape[0], k.shape[1]
         d = Cq // M
         scale = 1.0 / math.sqrt(d) if alpha is None else float(alpha)
-        qv = q.view(Bq, U1, M, d).permute(0, 2, 1, 3)         # [Bq,M,U1,d] strided view, d contiguous
-        kv = k.view(B, U2, M, d).permute(0, 2, 1, 3)
+        qv = _head_rows(q, Bq, U1, M, d)                       # [Bq,M,U1,d] strided view, d contiguous
+        kv = _head_rows(k, B, U2, M, d)
         S = _rowpad_empty((B, M, U1, U2), q.device)
         if row_bias is not None and M != 1:
             raise L.SxError("attn_scores: row_bias needs a single mode")
@@ -685,16 +720,18 @@ def _score_grads(dS, q, k, M, scale, need_q, need_k, tag="big"):
     Bq, U1, Cq = q.shape
     B, U2 = k.shape[0], k.shape[1]
     d = Cq // M
+    al = _heads_aligned(d, Cq)              # otherwise the mode slices are read through padded K-major copies
     dq = dk = None
     if need_q:
         # dQ[b,m] (U1 x d) = scale * dS[b,m] (U1 x U2) . K[b,m] (U2 x d)
         bcast = Bq == 1 and B > 1
         dq = _zeros_like(q) if bcast else torch.empty_like(q)
-        gemm_nt(dS, k.view(B, U2, M, d).permute(0, 2, 3, 1), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3),
-                alpha=scale, round_out=False, reduce_z1=bcast, split_k=1, tag=tag)
+        gemm_nt(dS, k.view(B, U2, M, d).permute(0, 2, 3, 1) if al else _head_cols(k, B, U2, M, d, True),
+                out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, reduce_z1=bcast, split_k=1,
+                tag=tag)
     if need_k:
         dk = torch.empty_like(k)
-        gemm_nt(dS.transpose(-1, -2), q.view(Bq, U1, M, d).permute(0, 2, 3, 1),
+        gemm_nt(dS.transpose(-1, -2), q.view(Bq, U1, M, d).permute(0, 2, 3, 1) if al else _head_cols(q, Bq, U1, M, d, True),
                 out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, tag=tag)
     return dq, dk
 
@@ -924,28 +961,46 @@ class _SoftmaxPosBias(torch.autograd.Function):
 
 
 class _AttnPV(torch.autograd.Function):
-    """U[b,m] = P[b,m] V[b,:,m]   with V [B,U2,M*F], channel = m*F+f  (segtran_shared.py:414-419, :447)."""
+    """U[b,m] = P[b,m] V[b,:,m]   with V [B,U2,M*F], channel = m*F+f  (segtran_shared.py:414-419, :447).
+    heads: U is written head-concatenated, [B,U1,M*F] with U[b,:,m*F+f] (MultiHeadFeatTrans, segtran_ablation.py:230-240),
+    straight from the GEMM epilogue (row pitch M*F, head stride F), so the Linear that consumes it reads it K-major."""
 
     @staticmethod
-    def forward(ctx, P, v, M, tag, round_out):
+    def forward(ctx, P, v, M, tag, round_out, heads):
         B, _, U1, U2 = P.shape
         Fd = v.shape[-1] // M
-        vv = v.view(B, U2, M, Fd).permute(0, 2, 3, 1)          # [B,M,F,U2]: the "N x K" operand, F contiguous
         P = _rowpad(P)
-        U = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
-        gemm_nt(P, vv, out=U, tag=tag, round_out=round_out)
+        if heads:
+            U = torch.empty((B, U1, M * Fd), device=P.device, dtype=torch.float32)
+            gemm_nt(P, _head_cols(v, B, U2, M, Fd, _kmajor_copies(tag)), out=U.view(B, U1, M, Fd).permute(0, 2, 1, 3),
+                    tag=tag, round_out=round_out)
+        else:
+            vv = v.view(B, U2, M, Fd).permute(0, 2, 3, 1)          # [B,M,F,U2]: the "N x K" operand, F contiguous
+            U = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
+            gemm_nt(P, vv, out=U, tag=tag, round_out=round_out)
         ctx.save_for_backward(P, v)
-        ctx.meta = (M, Fd)
+        ctx.meta = (M, Fd, heads)
         ctx.tag = tag
         return U
 
     @staticmethod
     def backward(ctx, dU):
         P, v = ctx.saved_tensors
-        M, Fd = ctx.meta
+        M, Fd, heads = ctx.meta
         B, _, U1, U2 = P.shape
         dU = dU.contiguous()
         dP = dv = None
+        if heads:
+            if ctx.needs_input_grad[0]:
+                # dP_h = dU_h V_h^T: both operands K-major head slices (dh contiguous)
+                dP = _rowpad_empty((B, M, U1, U2), P.device)
+                gemm_nt(_head_rows(dU, B, U1, M, Fd), _head_rows(v, B, U2, M, Fd), out=dP, round_out=False, tag=ctx.tag)
+            if ctx.needs_input_grad[1]:
+                # dV_h = P_h^T dU_h, written into V's head-interleaved layout
+                dv = torch.empty_like(v)
+                gemm_nt(P.transpose(-1, -2), _head_cols(dU, B, U1, M, Fd, False),
+                        out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3), round_out=False, tag=ctx.tag)
+            return dP, dv, None, None, None, None
         if ctx.needs_input_grad[0]:
             # dP[b,m] (U1 x U2) = dU[b,m] (U1 x F) . V[b,m]^T  -> operand "B" = V[b,m] as [U2, F]
             dP = _rowpad_empty((B, M, U1, U2), P.device)
@@ -955,7 +1010,7 @@ class _AttnPV(torch.autograd.Function):
             # dV[b,m] (U2 x F) = P[b,m]^T (U2 x U1) . dU[b,m] (U1 x F)
             gemm_nt(P.transpose(-1, -2), dU.transpose(-1, -2), out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3),
                     round_out=False, tag=ctx.tag)
-        return dP, dv, None, None, None
+        return dP, dv, None, None, None, None
 
 
 class _AttnPVGelu(torch.autograd.Function):
@@ -1528,15 +1583,16 @@ def softmax_posbias(S, posbias, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=
     return _SoftmaxPosBias.apply(S, amax, clip, drop_p, seed, diag, table, geom)
 
 
-def attn_pv(P, v, M, tag="big", round_out=True):
-    return _AttnPV.apply(P, v, M, tag, round_out)
+def attn_pv(P, v, M, tag="big", round_out=True, heads=False):
+    """P [B,M,U1,U2], v [B,U2,M*F] -> [B,M,U1,F], or with heads=True the head-concatenated [B,U1,M*F]."""
+    return _AttnPV.apply(P, v, M, tag, round_out, bool(heads))
 
 
-def layer_norm(x, g, b, consumer_tag=None, producer_tag=None):
+def layer_norm(x, g, b, consumer_tag=None, producer_tag=None, round_out=True):
     """consumer_tag / producer_tag: precision class of the contractions that consume y / that produced x (they decide
-    whether y, respectively dx, is TF32-rounded here)."""
-    return _LayerNorm.apply(x, g, b, _rt() if consumer_tag is None else rt_for(consumer_tag),
-                            _rt() if producer_tag is None else rt_for(producer_tag))
+    whether y, respectively dx, is TF32-rounded here).  round_out=False: y feeds no contraction (kept unrounded)."""
+    rnd = (_rt() if consumer_tag is None else rt_for(consumer_tag)) if round_out else 0
+    return _LayerNorm.apply(x, g, b, rnd, _rt() if producer_tag is None else rt_for(producer_tag))
 
 
 def group_linear(G, Wo, bo):
