@@ -299,7 +299,8 @@ class ExpandedFeatTrans(nn.Module):
             and self.first_linear.bias is None and self.first_linear.weight.shape[1] % 4 == 0 and self.feat_dim % 4 == 0
 
     def supports_fused_attention(self):
-        """The expansion block whose P.V / mid / output chain hangs off one autograd node (ops.squeeze_out_fused)."""
+        """The expansion block whose P.V / mid / output chain is one autograd node (ops.attn_pv_gelu_group_linear), which
+        ops.squeeze_out_fused feeds with the fused attention probabilities."""
         return self.has_FFN and isinstance(self.output, MMPrivateOutput) and isinstance(self.intermediate, MMSharedMid)
 
     def _value_bank(self, input_feat, tag="big"):
@@ -321,7 +322,8 @@ class ExpandedFeatTrans(nn.Module):
 
     def forward_from_qk(self, input_feat, q, k, clip, att_p, diag, posbias=None):
         """Fused attention entry: q [Bq,U1,M*d], k [B,U2,M*d] (projected, TF32-rounded) instead of the probabilities —
-        scores, clamp, positional bias, softmax and attention dropout run inside ops.squeeze_out_fused (csrc/sx_attn.cu)."""
+        scores, clamp, positional bias, softmax and attention dropout run in one kernel (csrc/sx_attn.cu), whose
+        probabilities ops.squeeze_out_fused hands to the P.V' / mid / output node."""
         mid = self.intermediate
         vp = self._value_bank(input_feat, ops.small_tag(input_feat.shape[1], q.shape[1]))
         p = mid.dropout.p if self.training else 0.0

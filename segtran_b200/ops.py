@@ -147,6 +147,16 @@ def _sink_or_zeros(p, like=None):
     return z, z
 
 
+def _param_grad(p, a, b, shape, **kw):
+    """Gradient of parameter p computed by the GEMM a b^T (output viewed as `shape`): accumulated straight into p.grad when
+    direct accumulation applies (returns None then), else returned as a new tensor of p's shape."""
+    tgt = _grad_target(p)
+    if tgt is not None:
+        gemm_nt(a, b, out=tgt.view(shape), accumulate=True, round_out=False, **kw)
+        return None
+    return gemm_nt(a, b, round_out=False, **kw).view(p.shape)
+
+
 def _rt() -> int:
     """round-to-TF32 flag handed to producer kernels (off in the 3-pass validation mode)."""
     return 1 if _PRECISION == "tf32" else 0
@@ -556,14 +566,6 @@ def _transposed(x: torch.Tensor, Z: int, R: int, Cd: int) -> torch.Tensor:
     return y
 
 
-def _bank_operand(v: torch.Tensor, B: int, U2: int, M: int, Fd: int) -> torch.Tensor:
-    """The [B, M, Fd, U2] "N x K" operand of U[b,m] = P[b,m] V[b,:,m] for a value bank v [B, U2, M*Fd] (also the
-    keys of dQ = dS K): a K-major copy, or the MN-major view of v when the copies are off."""
-    if _kmajor_copies():
-        return _transposed(v, B, U2, M * Fd).unflatten(1, (M, Fd))
-    return v.view(B, U2, M, Fd).permute(0, 2, 3, 1)
-
-
 def _weight_t(Wr: torch.Tensor, Z: int, O: int, I: int) -> torch.Tensor:
     """[Z, I, O] transpose of the TF32-rounded weights Wr [Z, O, I], the "N x K" operand of dX = dY W: a K-major copy,
     or the MN-major view of Wr when the copies are off."""
@@ -631,11 +633,7 @@ class _Linear(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = gemm_nt(dy2, _weight_t(Wr2, 1, *Wr2.shape)[0], round_out=False).view(shp)
         if ctx.needs_input_grad[1]:
-            tgt = _grad_target(W)
-            if tgt is not None:
-                gemm_nt(dy2.t(), x2.t(), out=tgt.view(O, -1), accumulate=True, round_out=False)
-            else:
-                dW = gemm_nt(dy2.t(), x2.t(), round_out=False).view(W.shape)
+            dW = _param_grad(W, dy2.t(), x2.t(), (O, -1))
         if has_b and ctx.needs_input_grad[2]:
             tgt = _grad_target(b)
             if tgt is not None:
@@ -715,24 +713,24 @@ class _AttnScores(torch.autograd.Function):
         return dq, dk, None, None, drb, None, None
 
 
-def _score_grads(dS, q, k, M, scale, need_q, need_k, tag="big"):
-    """Gradients of S = scale * Q K^T per mode: dQ = scale dS K, dK = scale dS^T Q (q may have batch 1: broadcast)."""
+def _score_grads(dS, q, k, M, scale, need_q, need_k, tag="big", kmajor_k=False):
+    """Gradients of S = scale * Q K^T per mode: dQ = scale dS K, dK = scale dS^T Q (q may have batch 1: broadcast).
+    Both read the MN-major views of the keys and queries (padded K-major copies when the mode slices are not TMA-aligned);
+    kmajor_k: dQ reads a K-major copy of the keys instead (the squeeze-out's attractor keys, small against dS)."""
     Bq, U1, Cq = q.shape
     B, U2 = k.shape[0], k.shape[1]
     d = Cq // M
-    al = _heads_aligned(d, Cq)              # otherwise the mode slices are read through padded K-major copies
     dq = dk = None
     if need_q:
         # dQ[b,m] (U1 x d) = scale * dS[b,m] (U1 x U2) . K[b,m] (U2 x d)
         bcast = Bq == 1 and B > 1
         dq = _zeros_like(q) if bcast else torch.empty_like(q)
-        gemm_nt(dS, k.view(B, U2, M, d).permute(0, 2, 3, 1) if al else _head_cols(k, B, U2, M, d, True),
-                out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, reduce_z1=bcast, split_k=1,
-                tag=tag)
+        gemm_nt(dS, _head_cols(k, B, U2, M, d, kmajor_k), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3), alpha=scale,
+                round_out=False, reduce_z1=bcast, split_k=1, tag=tag)
     if need_k:
         dk = torch.empty_like(k)
-        gemm_nt(dS.transpose(-1, -2), q.view(Bq, U1, M, d).permute(0, 2, 3, 1) if al else _head_cols(q, Bq, U1, M, d, True),
-                out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, tag=tag)
+        gemm_nt(dS.transpose(-1, -2), _head_cols(q, Bq, U1, M, d, False), out=dk.view(B, U2, M, d).permute(0, 2, 1, 3),
+                alpha=scale, round_out=False, tag=tag)
     return dq, dk
 
 
@@ -784,7 +782,7 @@ def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_sc
     in registers and the softmax runs on the accumulator fragments (reference segtran_shared.py:566-567, :569-580, :601, :605).
     q [Bq,U1,M*d] (Bq = 1 broadcasts), k [B,U2,M*d], both contiguous fp32 (TF32-rounded by their producers).
     posbias (PosBias, self-attention only): adds the sliding-window bias inside the softmax, after the clamp; S, rowmax
-    and the clamp statistics stay on the raw scores (its table gradient comes from softmax_posbias_backward).
+    and the clamp statistics stay on the raw scores (its table gradient comes from softmax_backward).
     alpha: the score scale (default 1/sqrt(d) of the per-mode width; the mince transformer scales zero-padded channel
     windows by the full width).
     -> (P [B,M,U1,U2] view of a row-padded buffer, S or None (raw scaled scores, same layout), lse [B,M,U1],
@@ -883,54 +881,42 @@ def matvec(x, v):
     return _MatVec.apply(x, v)
 
 
-class _Softmax(torch.autograd.Function):
-    """P = dropout(softmax(clamp_if(S)))  (segtran_shared.py:578-580, :601-605); output rounded for the P.V GEMM."""
-
-    @staticmethod
-    def forward(ctx, S, amax, clip, drop_p, seed, diag):
-        S = _rowpad(S)
-        Lr, ld = S.shape[-1], S.stride(-2)
-        R = S.numel() // Lr
-        P = _rowpad_empty(S.shape, S.device)
-        lse = torch.empty(R, device=S.device, dtype=torch.float32)
-        L.call("sx_softmax_fwd", S.data_ptr(), R, Lr, ld, _ptr(amax), clip, drop_p, *_seed_args(seed), P.data_ptr(),
-               P.stride(-2), _rt(), lse.data_ptr(), _ptr(diag), _stream())
-        ctx.save_for_backward(S, lse, amax)
-        ctx.meta = (clip, drop_p, seed, P.stride(-2))
-        return P
-
-    @staticmethod
-    def backward(ctx, dP):
-        S, lse, amax = ctx.saved_tensors
-        clip, drop_p, seed, ldp = ctx.meta
-        dP = _rowpad(dP)
-        Lr = S.shape[-1]
-        R = S.numel() // Lr
-        dS = _rowpad_empty(S.shape, S.device)
-        L.call("sx_softmax_bwd", dP.data_ptr(), dP.stride(-2), S.data_ptr(), S.stride(-2), lse.data_ptr(), R, Lr,
-               _ptr(amax), clip, drop_p, *_seed_args(seed), ldp, dS.data_ptr(), dS.stride(-2), _rt(), _stream())
-        return dS, None, None, None, None, None
-
-
 def softmax_posbias_backward(dP, ldd, S, lds, lse, R, Lr, amax, clip, drop_p, seed, ldp_fwd, dS, ldo, table, pb_geom,
                              table_needs_grad):
     """dS (with the clamp mask) and the table gradient of the biased softmax.  The table gradient goes straight into the
     table's .grad when direct accumulation is on (returns None then), else into a new tensor that is returned."""
-    R_, grid, w = pb_geom
     tgt = _grad_target(table) if table_needs_grad else None
     buf = tgt if tgt is not None else _zeros((table.numel(),), table.device)
-    desc = _posbias_desc(table, R_, grid, w)
     L.call("sx_softmax_posbias_bwd", dP.data_ptr(), ldd, S.data_ptr(), lds, lse.data_ptr(), R, Lr, _ptr(amax), clip, drop_p,
-           *_seed_args(seed), ldp_fwd, dS.data_ptr(), ldo, _rt(), C.byref(desc), buf.data_ptr(),
+           *_seed_args(seed), ldp_fwd, dS.data_ptr(), ldo, _rt(), C.byref(_posbias_desc(table, *pb_geom)), buf.data_ptr(),
            *_part_args(dS.device), _stream())
     if tgt is not None or not table_needs_grad:
         return None
     return buf.view(table.shape)
 
 
-class _SoftmaxPosBias(torch.autograd.Function):
-    """P = dropout(softmax(clamp_if(S) + w * bias))  (segtran_shared.py:578-605 with pos_biases); S is the raw [B,M,N,N]
-    score tensor of a self-attention over the bias grid.  Backward: dS and the table gradient."""
+def softmax_backward(dP, S, lse, amax, clip, drop_p, seed, ldp, table=None, pb_geom=None, table_needs_grad=False):
+    """Backward of P = dropout(softmax(clamp_if(S) [+ w * bias])) on the saved raw scores S and row log-sum-exps lse;
+    P is recomputed from them, and the dropout mask is regenerated from `seed` and P's row pitch `ldp`.
+    table / pb_geom = (R, grid, w): the positional bias, if the softmax had one.
+    -> (dS, dT): dT is the table gradient, or None without a table, when it is not needed, or when it went straight into
+    the table's .grad (direct accumulation)."""
+    dP = _rowpad(dP)
+    Lr = S.shape[-1]
+    R = S.numel() // Lr
+    dS = _rowpad_empty(S.shape, S.device)
+    if table is None:
+        L.call("sx_softmax_bwd", dP.data_ptr(), dP.stride(-2), S.data_ptr(), S.stride(-2), lse.data_ptr(), R, Lr,
+               _ptr(amax), clip, drop_p, *_seed_args(seed), ldp, dS.data_ptr(), dS.stride(-2), _rt(), _stream())
+        return dS, None
+    return dS, softmax_posbias_backward(dP, dP.stride(-2), S, S.stride(-2), lse, R, Lr, amax, clip, drop_p, seed, ldp, dS,
+                                        dS.stride(-2), table, pb_geom, table_needs_grad)
+
+
+class _Softmax(torch.autograd.Function):
+    """P = dropout(softmax(clamp_if(S) [+ w * bias]))  (segtran_shared.py:578-605); output rounded for the P.V GEMM.
+    table / pb_geom (optional): the sliding-window positional bias of a self-attention over the bias grid, S its raw
+    [B,M,N,N] scores; backward then also gives the table gradient."""
 
     @staticmethod
     def forward(ctx, S, amax, clip, drop_p, seed, diag, table, pb_geom):
@@ -939,9 +925,12 @@ class _SoftmaxPosBias(torch.autograd.Function):
         R = S.numel() // Lr
         P = _rowpad_empty(S.shape, S.device)
         lse = torch.empty(R, device=S.device, dtype=torch.float32)
-        desc = _posbias_desc(table, *pb_geom)
-        L.call("sx_softmax_posbias_fwd", S.data_ptr(), R, Lr, ld, _ptr(amax), clip, drop_p, *_seed_args(seed), P.data_ptr(),
-               P.stride(-2), _rt(), lse.data_ptr(), _ptr(diag), C.byref(desc), _stream())
+        args = (S.data_ptr(), R, Lr, ld, _ptr(amax), clip, drop_p, *_seed_args(seed), P.data_ptr(), P.stride(-2), _rt(),
+                lse.data_ptr(), _ptr(diag))
+        if table is None:
+            L.call("sx_softmax_fwd", *args, _stream())
+        else:
+            L.call("sx_softmax_posbias_fwd", *args, C.byref(_posbias_desc(table, *pb_geom)), _stream())
         ctx.save_for_backward(S, lse, amax, table)
         ctx.meta = (clip, drop_p, seed, P.stride(-2), pb_geom)
         ctx.leaf = table
@@ -949,14 +938,9 @@ class _SoftmaxPosBias(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dP):
-        S, lse, amax, table = ctx.saved_tensors
+        S, lse, amax, _table = ctx.saved_tensors
         clip, drop_p, seed, ldp, pb_geom = ctx.meta
-        dP = _rowpad(dP)
-        Lr = S.shape[-1]
-        R = S.numel() // Lr
-        dS = _rowpad_empty(S.shape, S.device)
-        dT = softmax_posbias_backward(dP, dP.stride(-2), S, S.stride(-2), lse, R, Lr, amax, clip, drop_p, seed, ldp, dS,
-                                      dS.stride(-2), ctx.leaf, pb_geom, ctx.needs_input_grad[6])
+        dS, dT = softmax_backward(dP, S, lse, amax, clip, drop_p, seed, ldp, ctx.leaf, pb_geom, ctx.needs_input_grad[6])
         return dS, None, None, None, None, None, dT, None
 
 
@@ -1001,57 +985,23 @@ class _AttnPV(torch.autograd.Function):
                 gemm_nt(P.transpose(-1, -2), _head_cols(dU, B, U1, M, Fd, False),
                         out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3), round_out=False, tag=ctx.tag)
             return dP, dv, None, None, None, None
-        if ctx.needs_input_grad[0]:
-            # dP[b,m] (U1 x U2) = dU[b,m] (U1 x F) . V[b,m]^T  -> operand "B" = V[b,m] as [U2, F]
-            dP = _rowpad_empty((B, M, U1, U2), P.device)
-            gemm_nt(dU, v.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False, tag=ctx.tag)
-        if ctx.needs_input_grad[1]:
-            dv = torch.empty_like(v)
-            # dV[b,m] (U2 x F) = P[b,m]^T (U2 x U1) . dU[b,m] (U1 x F)
-            gemm_nt(P.transpose(-1, -2), dU.transpose(-1, -2), out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3),
-                    round_out=False, tag=ctx.tag)
+        dP, dv = _pv_grads(dU, P, v, M, Fd, ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.tag)
         return dP, dv, None, None, None, None
 
 
-class _AttnPVGelu(torch.autograd.Function):
-    """G[b,m] = dropout(gelu(P[b,m] V'[b,:,m] + bias)) — the P.V contraction with MMSharedMid's bias / erf-GELU /
-    dropout fused into its epilogue.  V' = V Wm^T is the value bank already pushed through the shared mid Linear
-    (re-association (P V) Wm^T = P (V Wm^T): A rows instead of N, see ExpandedFeatTrans.forward)."""
-
-    @staticmethod
-    def forward(ctx, P, v, M, bias, drop_p, seed):
-        B, _, U1, U2 = P.shape
-        Fd = v.shape[-1] // M
-        P = _rowpad(P)
-        vv = v.view(B, U2, M, Fd).permute(0, 2, 3, 1)
-        G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
-        H = torch.empty_like(G)
-        gemm_nt(P, vv, out=G, bias=bias, gelu=True, preact=H, drop_p=drop_p, seed=seed)
-        ctx.save_for_backward(P, v, H)
-        ctx.meta = (M, Fd, drop_p, bias is not None)
-        ctx.seed = seed
-        return G
-
-    @staticmethod
-    def backward(ctx, dG):
-        P, v, H = ctx.saved_tensors
-        M, Fd, drop_p, has_b = ctx.meta
-        B, _, U1, U2 = P.shape
-        dG = dG.contiguous()
-        dH = torch.empty_like(dG)
-        L.call("sx_gelu_bwd", dG.data_ptr(), H.data_ptr(), dG.numel(), drop_p, *_seed_args(ctx.seed), dH.data_ptr(), _rt(),
-               _stream())
-        dP = dv = db = None
-        if ctx.needs_input_grad[0]:
-            dP = _rowpad_empty((B, M, U1, U2), P.device)
-            gemm_nt(dH, v.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False)
-        if ctx.needs_input_grad[1]:
-            dv = torch.empty_like(v)
-            gemm_nt(P.transpose(-1, -2), dH.transpose(-1, -2), out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3),
-                    round_out=False)
-        if has_b and ctx.needs_input_grad[3]:
-            db = colsum(dH.view(-1, Fd))
-        return dP, dv, None, db, None, None
+def _pv_grads(dU, P, v, M, Fd, need_p, need_v, tag):
+    """Gradients of U[b,m] = P[b,m] V[b,:,m] (v [B,U2,M*F], dU [B,M,U1,F] contiguous):
+    dP[b,m] = dU[b,m] V[b,:,m]^T (row-padded like P) and dV[b,:,m] = P[b,m]^T dU[b,m]."""
+    B, _, U1, U2 = P.shape
+    dP = dv = None
+    if need_p:
+        dP = _rowpad_empty((B, M, U1, U2), P.device)
+        gemm_nt(dU, v.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False, tag=tag)
+    if need_v:
+        dv = torch.empty_like(v)
+        gemm_nt(P.transpose(-1, -2), dU.transpose(-1, -2), out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3),
+                round_out=False, tag=tag)
+    return dP, dv
 
 
 class _FoldedValueBank(torch.autograd.Function):
@@ -1075,14 +1025,14 @@ class _FoldedValueBank(torch.autograd.Function):
         if x3 and _PRECISION == "tf32":                               # single-pass backward: TF32-rounded operands
             Wf, Wvr, Wmr = round_tf32(Wf), round_tf32(Wv).view(M, 1, Fd, Cd), round_tf32(Wm)
         ctx.save_for_backward(a2, Wf, Wvr, Wmr)
-        ctx.meta = (B, A, Cd, Fd, M, Wv.shape)
+        ctx.meta = (B, A, Cd, Fd, M)
         ctx.leaves = (Wv, Wm)
         return Vp.view(B, A, M * Fd)
 
     @staticmethod
     def backward(ctx, dVp):
         a2, Wf, Wvr, Wmr = ctx.saved_tensors
-        B, A, Cd, Fd, M, wv_shape = ctx.meta
+        B, A, Cd, Fd, M = ctx.meta
         Wv, Wm = ctx.leaves
         d2 = dVp.reshape(B * A, M * Fd)
         if not d2.is_contiguous():
@@ -1093,18 +1043,9 @@ class _FoldedValueBank(torch.autograd.Function):
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             dWf = gemm_nt(d2.t(), a2.t(), round_out=False).view(M, 1, Fd, Cd)          # [m, o, c]
             if ctx.needs_input_grad[2]:                               # dWm[o,f] = sum_m dW'_m[o,:] . Wv_m[f,:]
-                tgt = _grad_target(Wm)
-                if tgt is not None:
-                    gemm_nt(dWf, Wvr, out=tgt.view(1, 1, Fd, Fd), reduce_z1=True, accumulate=True, round_out=False)
-                else:
-                    dWm = gemm_nt(dWf, Wvr, reduce_z1=True, round_out=False).view(Fd, Fd)
+                dWm = _param_grad(Wm, dWf, Wvr, (1, 1, Fd, Fd), reduce_z1=True)
             if ctx.needs_input_grad[1]:                               # dWv_m[f,c] = sum_o Wm[o,f] dW'_m[o,c]
-                tgt = _grad_target(Wv)
-                if tgt is not None:
-                    gemm_nt(Wmr.t().view(1, 1, Fd, Fd), dWf.transpose(-1, -2), out=tgt.view(M, 1, Fd, Cd), accumulate=True,
-                            round_out=False)
-                else:
-                    dWv = gemm_nt(Wmr.t().view(1, 1, Fd, Fd), dWf.transpose(-1, -2), round_out=False).view(wv_shape)
+                dWv = _param_grad(Wv, Wmr.t().view(1, 1, Fd, Fd), dWf.transpose(-1, -2), (M, 1, Fd, Cd))
         return da, dWv, dWm, None, None
 
 
@@ -1112,14 +1053,38 @@ def folded_value_bank(a, Wv, Wm, M, tag="small"):
     return _FoldedValueBank.apply(a, Wv, Wm, M, tag)
 
 
-def attn_pv_gelu(P, v, M, bias, drop_p=0.0, seed=0):
-    return _AttnPVGelu.apply(P, v, M, bias, drop_p, seed)
+def _group_linear_fwd(G, Wo, bo):
+    """Y[b,m] = G[b,m] Wo[m]^T + bo[m] for G [B,M,N,F] -> (Y, the TF32-rounded weights [M,F,F] that backward reads)."""
+    M, Fd = G.shape[1], G.shape[3]
+    Wr = round_tf32(Wo).reshape(M, Fd, Fd)
+    Y = torch.empty_like(G)
+    gemm_nt(G, Wr.unsqueeze(0), out=Y, bias=bo.reshape(1, M, Fd), round_out=False)
+    return Y, Wr
+
+
+def _group_linear_param_grads(dY, G, Wo, bo, need_w, need_b):
+    """(dWo, dbo) of _group_linear_fwd: dWo[m] = sum_b dY[b,m]^T G[b,m] and the column sums of dY (dY contiguous); a
+    gradient that goes straight into the parameter's .grad is returned as None."""
+    B, M, N, Fd = G.shape
+    dW = db = None
+    if need_w:
+        dW = _param_grad(Wo, dY.transpose(-1, -2), G.transpose(-1, -2), (1, M, Fd, Fd), reduce_z1=True)
+    if need_b:
+        tgt = _grad_target(bo)
+        buf = tgt if tgt is not None else _zeros((M * Fd,), G.device)
+        L.call("sx_colsum_batched", dY.data_ptr(), B, M * N * Fd, M, N * Fd, N, Fd, Fd, buf.data_ptr(),
+               *_part_args(dY.device), _stream())
+        db = None if tgt is not None else buf
+    return dW, db
 
 
 class _AttnPVGeluGroupLinear(torch.autograd.Function):
-    """Y[b,m] = dropout(gelu(P[b,m] V'[b,:,m] + bm)) Wo[m]^T + bo[m]: _AttnPVGelu followed by _GroupLinear as ONE autograd
-    node, so that backward can fuse gelu'(h) * dropout mask into the epilogue of the dG = dY Wo GEMM (SX_ACT_GELU_BWD)
-    instead of writing dG, re-reading it with the pre-activation and writing dH in a separate pass."""
+    """Y[b,m] = dropout(gelu(P[b,m] V'[b,:,m] + bm)) Wo[m]^T + bo[m]  (segtran_shared.py:447, :243-245, :267): the P.V'
+    contraction with MMSharedMid's bias / erf-GELU / dropout in its epilogue, then MMPrivateOutput's grouped Linear, as ONE
+    autograd node, so that backward can fuse gelu'(h) * dropout mask into the epilogue of the dG = dY Wo GEMM
+    (SX_ACT_GELU_BWD) instead of writing dG, re-reading it with the pre-activation and writing dH in a separate pass.
+    V' = V Wm^T is the value bank already pushed through the shared mid Linear (re-association (P V) Wm^T = P (V Wm^T):
+    A rows instead of N, see ExpandedFeatTrans.forward)."""
 
     @staticmethod
     def forward(ctx, P, v, M, bm, drop_p, seed, Wo, bo):
@@ -1128,53 +1093,32 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
         P = _rowpad(P)
         G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
         H = torch.empty_like(G)
-        gemm_nt(P, _bank_operand(v, B, U2, M, Fd), out=G, bias=bm, gelu=True, preact=H, drop_p=drop_p, seed=seed)
-        Wr = round_tf32(Wo).reshape(M, Fd, Fd)
-        Y = torch.empty_like(G)
-        gemm_nt(G, Wr.unsqueeze(0), out=Y, bias=bo.reshape(1, M, Fd), round_out=False)
+        gemm_nt(P, _head_cols(v, B, U2, M, Fd, _kmajor_copies()), out=G, bias=bm, gelu=True, preact=H, drop_p=drop_p,
+                seed=seed)
+        Y, Wr = _group_linear_fwd(G, Wo, bo)
         ctx.save_for_backward(P, v, H, G, Wr)
-        ctx.meta = (M, Fd, drop_p, bm is not None, Wo.shape)
-        ctx.seed = seed
+        ctx.meta = (M, Fd, drop_p, seed)
         ctx.leaves = (bm, Wo, bo)
         return Y
 
     @staticmethod
     def backward(ctx, dY):
         P, v, H, G, Wr = ctx.saved_tensors
-        M, Fd, drop_p, has_bm, wshape = ctx.meta
+        M, Fd, drop_p, seed = ctx.meta
         bm, Wo, bo = ctx.leaves
-        B, _, U1, U2 = P.shape
         dY = dY.contiguous()
-        dP = dv = dbm = dW = dbo = None
-        # dH = mask * (dY Wo) * gelu'(H), TF32-rounded for the two GEMMs that consume it
-        dH = torch.empty_like(H)
-        dbm_buf = None
-        if has_bm and ctx.needs_input_grad[3]:
+        dbm_buf = dbm = None
+        if bm is not None and ctx.needs_input_grad[3]:
             tgt = _grad_target(bm)
             dbm_buf = tgt if tgt is not None else _zeros((Fd,), dY.device)
             dbm = None if tgt is not None else dbm_buf
-        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=ctx.seed)
+        # dH = mask * (dY Wo) * gelu'(H), TF32-rounded for the two GEMMs that consume it
+        dH = torch.empty_like(H)
+        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=seed)
         if dbm_buf is not None:             # column sums of dH = the gradient of MMSharedMid's bias
             colsum(dH.view(-1, Fd), out=dbm_buf)
-        if ctx.needs_input_grad[6]:
-            tgt = _grad_target(Wo)
-            if tgt is not None:
-                gemm_nt(dY.transpose(-1, -2), G.transpose(-1, -2), out=tgt.view(1, M, Fd, Fd), reduce_z1=True,
-                        accumulate=True, round_out=False)
-            else:
-                dW = gemm_nt(dY.transpose(-1, -2), G.transpose(-1, -2), reduce_z1=True, round_out=False).view(wshape)
-        if ctx.needs_input_grad[7]:
-            tgt = _grad_target(bo)
-            dbo_buf = tgt if tgt is not None else _zeros((M * Fd,), G.device)
-            L.call("sx_colsum_batched", dY.data_ptr(), B, M * U1 * Fd, M, U1 * Fd, U1, Fd, Fd, dbo_buf.data_ptr(), *_part_args(dY.device), _stream())
-            dbo = None if tgt is not None else dbo_buf
-        if ctx.needs_input_grad[0]:
-            dP = _rowpad_empty((B, M, U1, U2), P.device)
-            gemm_nt(dH, v.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False)
-        if ctx.needs_input_grad[1]:
-            dv = torch.empty_like(v)
-            gemm_nt(P.transpose(-1, -2), dH.transpose(-1, -2), out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3),
-                    round_out=False)
+        dW, dbo = _group_linear_param_grads(dY, G, Wo, bo, ctx.needs_input_grad[6], ctx.needs_input_grad[7])
+        dP, dv = _pv_grads(dH, P, v, M, Fd, ctx.needs_input_grad[0], ctx.needs_input_grad[1], "big")
         return dP, dv, None, dbm, None, None, dW, dbo
 
 
@@ -1197,104 +1141,6 @@ def attn_fusion_enabled() -> bool:
     return _ATTN_FUSION and _PRECISION == "tf32"          # the 3-pass validation mode keeps the unfused fp32-grade products
 
 
-class _SqueezeOutFused(torch.autograd.Function):
-    """Y[b,m] = dropout(gelu(P[b,m] V'[b,:,m] + bm)) Wo[m]^T + bo[m]  with  P = dropout(softmax(min(Q K^T/sqrt(d), clip)))
-    — CrossAttFeatTrans.forward (segtran_shared.py:566-605) + ExpandedFeatTrans up to MMPrivateOutput's Linear
-    (:447, :243-245, :267) as ONE autograd node:
-      forward : sx_attn_probs_fwd (wgmma scores -> in-register softmax -> P)  ->  P.V' GEMM (bias/GELU/dropout epilogue)
-                -> grouped output Linear;
-      backward: dH GEMM (GELU'/dropout epilogue) -> bias-gradient column sums -> dP GEMM -> sx_softmax_bwd on the saved raw
-                scores (P recomputed from S and the row log-sum-exp, the row term sum_a P_a dP_a taken from the SAME dP values
-                it is subtracted from) -> dV', dQ, dK, dWo, dbo products.
-    A flash-attention style backward (row term from sum_f dU_f U_f in the dH epilogue, softmax backward in the dP GEMM
-    epilogue) was built and measured: its row term carries independent TF32 rounding, which the softmax Jacobian amplifies
-    (input-gradient error 1.3e-2 at cfg 1 / cfg 4 against 6e-4 for this form), so it is not used."""
-
-    @staticmethod
-    def forward(ctx, q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag, table=None, pb_geom=None):
-        B, U2 = k.shape[0], k.shape[1]
-        U1 = q.shape[1]
-        Fd = vp.shape[-1] // M
-        q = q.contiguous()
-        k = k.contiguous()
-        need_bwd = any(ctx.needs_input_grad)
-        pb = PosBias(table, pb_geom[0], pb_geom[1], pb_geom[2]) if table is not None else None
-        P, S, lse, _rowmax, stat = attn_probs_fused(q, k, M, clip, att_p, att_seed, diag, need_scores=need_bwd, posbias=pb)
-        G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
-        H = torch.empty_like(G)
-        gemm_nt(P, _bank_operand(vp, B, U2, M, Fd), out=G, bias=bm, gelu=True, preact=H, drop_p=hid_p, seed=hid_seed)
-        Wr = round_tf32(Wo).reshape(M, Fd, Fd)
-        Y = torch.empty_like(G)
-        gemm_nt(G, Wr.unsqueeze(0), out=Y, bias=bo.reshape(1, M, Fd), round_out=False)
-        ctx.save_for_backward(q, k, P, S, lse, stat, vp, H, G, Wr)
-        ctx.meta = (M, Fd, float(clip), att_p, hid_p, bm is not None, Wo.shape)
-        ctx.seeds = (att_seed, hid_seed)
-        ctx.leaves = (bm, Wo, bo)
-        ctx.pb = (table, pb_geom)
-        return Y
-
-    @staticmethod
-    def backward(ctx, dY):
-        q, k, P, S, lse, stat, vp, H, G, Wr = ctx.saved_tensors
-        M, Fd, clip, att_p, hid_p, has_bm, wshape = ctx.meta
-        att_seed, hid_seed = ctx.seeds
-        bm, Wo, bo = ctx.leaves
-        table, pb_geom = ctx.pb
-        dT = None
-        B, _, U1, U2 = P.shape
-        Bq, d = q.shape[0], q.shape[-1] // M
-        dY = dY.contiguous()
-        dq = dk = dvp = dbm = dW = dbo = None
-        # dH = mask * (dY Wo) * gelu'(H), then the column sums of dH (MMSharedMid's bias gradient)
-        dH = torch.empty_like(H)
-        dbm_buf = None
-        if has_bm and ctx.needs_input_grad[7]:
-            tgt = _grad_target(bm)
-            dbm_buf = tgt if tgt is not None else _zeros((Fd,), dY.device)
-            dbm = None if tgt is not None else dbm_buf
-        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=hid_p, seed=hid_seed)
-        if dbm_buf is not None:
-            colsum(dH.view(-1, Fd), out=dbm_buf)
-        if ctx.needs_input_grad[10]:
-            tgt = _grad_target(Wo)
-            if tgt is not None:
-                gemm_nt(dY.transpose(-1, -2), G.transpose(-1, -2), out=tgt.view(1, M, Fd, Fd), reduce_z1=True,
-                        accumulate=True, round_out=False)
-            else:
-                dW = gemm_nt(dY.transpose(-1, -2), G.transpose(-1, -2), reduce_z1=True, round_out=False).view(wshape)
-        if ctx.needs_input_grad[11]:
-            tgt = _grad_target(bo)
-            dbo_buf = tgt if tgt is not None else _zeros((M * Fd,), G.device)
-            L.call("sx_colsum_batched", dY.data_ptr(), B, M * U1 * Fd, M, U1 * Fd, U1, Fd, Fd, dbo_buf.data_ptr(), *_part_args(dY.device), _stream())
-            dbo = None if tgt is not None else dbo_buf
-        if ctx.needs_input_grad[2]:
-            dvp = torch.empty_like(vp)
-            gemm_nt(P.transpose(-1, -2), dH.transpose(-1, -2), out=dvp.view(B, U2, M, Fd).permute(0, 2, 1, 3),
-                    round_out=False)
-        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1] or (table is not None and ctx.needs_input_grad[13]):
-            dP = torch.empty_strided(P.size(), P.stride(), device=P.device, dtype=torch.float32)
-            gemm_nt(dH, vp.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False)
-            dS = torch.empty_strided(P.size(), P.stride(), device=P.device, dtype=torch.float32)
-            ld = P.stride(-2)
-            if table is not None:
-                dT = softmax_posbias_backward(dP, ld, S, ld, lse, B * M * U1, U2, stat[2:], clip, att_p, att_seed, ld, dS,
-                                              ld, table, pb_geom, ctx.needs_input_grad[13])
-            else:
-                L.call("sx_softmax_bwd", dP.data_ptr(), ld, S.data_ptr(), ld, lse.data_ptr(), B * M * U1, U2,
-                       stat[2:].data_ptr(), clip, att_p, *_seed_args(att_seed), ld, dS.data_ptr(), ld, _rt(), _stream())
-            scale = 1.0 / math.sqrt(d)
-            if ctx.needs_input_grad[0]:
-                bcast = Bq == 1 and B > 1
-                dq = _zeros_like(q) if bcast else torch.empty_like(q)
-                gemm_nt(dS, _bank_operand(k, B, U2, M, d), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3),
-                        alpha=scale, round_out=False, reduce_z1=bcast, split_k=1)
-            if ctx.needs_input_grad[1]:
-                dk = torch.empty_like(k)
-                gemm_nt(dS.transpose(-1, -2), q.view(Bq, U1, M, d).permute(0, 2, 3, 1),
-                        out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False)
-        return dq, dk, dvp, None, None, None, None, dbm, None, None, dW, dbo, None, dT, None
-
-
 def _pb_args(posbias):
     if posbias is None:
         return None, None
@@ -1302,8 +1148,14 @@ def _pb_args(posbias):
 
 
 def squeeze_out_fused(q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag, posbias=None):
-    """posbias (PosBias): sliding-window positional bias inside the softmax; its table receives a gradient."""
-    return _SqueezeOutFused.apply(q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag, *_pb_args(posbias))
+    """Y[b,m] = dropout(gelu(P[b,m] V'[b,:,m] + bm)) Wo[m]^T + bo[m]  with  P = dropout(softmax(min(Q K^T/sqrt(d), clip)))
+    — CrossAttFeatTrans.forward (segtran_shared.py:566-605) + ExpandedFeatTrans up to MMPrivateOutput's Linear: the fused
+    probabilities (_AttnProbs: scores, softmax and dropout in sx_attn_probs_fwd) feed attn_pv_gelu_group_linear.  The
+    attractor keys are small against dS, so dQ = dS K reads a K-major copy of them (DESIGN §4.3 on the backward's form).
+    posbias (PosBias): sliding-window positional bias inside the softmax; its table receives a gradient."""
+    P = _AttnProbs.apply(q.contiguous(), k.contiguous(), M, 1.0 / math.sqrt(q.shape[-1] // M), float(clip), att_p,
+                         att_seed, diag, *_pb_args(posbias), True)
+    return attn_pv_gelu_group_linear(P, vp, M, bm, hid_p, hid_seed, Wo, bo)
 
 
 class _LayerNorm(torch.autograd.Function):
@@ -1342,12 +1194,8 @@ class _GroupLinear(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, G, Wo, bo):
-        B, M, N, Fd = G.shape
-        Wr = round_tf32(Wo).reshape(M, Fd, Fd)
-        Y = torch.empty_like(G)
-        gemm_nt(G, Wr.unsqueeze(0), out=Y, bias=bo.reshape(1, M, Fd), round_out=False)
+        Y, Wr = _group_linear_fwd(G, Wo, bo)
         ctx.save_for_backward(G, Wr)
-        ctx.wshape = Wo.shape
         ctx.leaves = (Wo, bo)
         return Y
 
@@ -1356,24 +1204,10 @@ class _GroupLinear(torch.autograd.Function):
         G, Wr = ctx.saved_tensors
         B, M, N, Fd = G.shape
         dY = dY.contiguous()
-        dG = dW = db = None
+        dG = None
         if ctx.needs_input_grad[0]:
             dG = gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), round_out=False)
-        Wo, bo = ctx.leaves
-        if ctx.needs_input_grad[1]:
-            tgt = _grad_target(Wo)
-            if tgt is not None:
-                gemm_nt(dY.transpose(-1, -2), G.transpose(-1, -2), out=tgt.view(1, M, Fd, Fd), reduce_z1=True,
-                        accumulate=True, round_out=False)
-            else:
-                dW = gemm_nt(dY.transpose(-1, -2), G.transpose(-1, -2), reduce_z1=True, round_out=False)
-                dW = dW.view(ctx.wshape)
-        if ctx.needs_input_grad[2]:
-            tgt = _grad_target(bo)
-            db = tgt if tgt is not None else _zeros((M * Fd,), G.device)
-            L.call("sx_colsum_batched", dY.data_ptr(), B, M * N * Fd, M, N * Fd, N, Fd, Fd, db.data_ptr(), *_part_args(dY.device), _stream())
-            if tgt is not None:
-                db = None
+        dW, db = _group_linear_param_grads(dY, G, *ctx.leaves, ctx.needs_input_grad[1], ctx.needs_input_grad[2])
         return dG, dW, db
 
 
@@ -1572,7 +1406,7 @@ def attn_scores(q, k, M, amax=None, row_bias=None, tag="big", alpha=None):
 
 def softmax(S, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None):
     """diag: optional device float[2] updated in place: [0] = max(diag[0], *amax), [1] += (*amax > clip)."""
-    return _Softmax.apply(S, amax, clip, drop_p, seed, diag)
+    return _Softmax.apply(S, amax, clip, drop_p, seed, diag, None, None)
 
 
 def softmax_posbias(S, posbias, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None):
@@ -1580,7 +1414,7 @@ def softmax_posbias(S, posbias, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=
     if S.shape[-1] != posbias.num_tokens or S.shape[-2] != posbias.num_tokens:
         raise L.SxError("softmax_posbias: scores %s do not match the %s bias grid" % (tuple(S.shape), posbias.grid))
     table, geom = _pb_args(posbias)
-    return _SoftmaxPosBias.apply(S, amax, clip, drop_p, seed, diag, table, geom)
+    return _Softmax.apply(S, amax, clip, drop_p, seed, diag, table, geom)
 
 
 def attn_pv(P, v, M, tag="big", round_out=True, heads=False):
@@ -1832,45 +1666,34 @@ def resize_tokens_into(us, grid, grids_in, windows, Fd, round_out=True):
 
 class _AttnProbs(torch.autograd.Function):
     """P = dropout(softmax(clamp_if(alpha Q K^T) [+ w bias])) per mode as one node over the fused kernel
-    (attn_probs_fused): backward = softmax backward on the saved raw scores (sx_softmax_bwd / softmax_posbias_backward,
-    with the table gradient) -> dQ, dK products."""
+    (attn_probs_fused): backward = softmax backward on the saved raw scores (softmax_backward, with the table gradient)
+    -> dQ, dK products.  kmajor_dq: dQ reads a K-major copy of the keys (when the copies are on, see _kmajor_copies)."""
 
     @staticmethod
-    def forward(ctx, q, k, M, alpha, clip, drop_p, seed, diag, table, pb_geom):
+    def forward(ctx, q, k, M, alpha, clip, drop_p, seed, diag, table, pb_geom, kmajor_dq):
         pb = PosBias(table, *pb_geom) if table is not None else None
         need_bwd = any(ctx.needs_input_grad)
         P, S, lse, _rowmax, stat = attn_probs_fused(q, k, M, clip, drop_p, seed, diag, need_scores=need_bwd, posbias=pb,
                                                     alpha=alpha)
         ctx.save_for_backward(q, k, S, lse, stat)
-        ctx.meta = (M, alpha, clip, drop_p, P.stride(-2), pb_geom)
-        ctx.seed = seed
+        ctx.meta = (M, alpha, clip, drop_p, seed, P.stride(-2), pb_geom, kmajor_dq)
         ctx.leaf = table
         return P
 
     @staticmethod
     def backward(ctx, dP):
         q, k, S, lse, stat = ctx.saved_tensors
-        M, alpha, clip, drop_p, ldp, pb_geom = ctx.meta
-        table = ctx.leaf
-        B, _, U1, U2 = S.shape
-        dP = _rowpad(dP)
-        dS = _rowpad_empty(S.shape, S.device)
-        dT = None
-        if table is not None:
-            dT = softmax_posbias_backward(dP, dP.stride(-2), S, S.stride(-2), lse, B * M * U1, U2, stat[2:], clip, drop_p,
-                                          ctx.seed, ldp, dS, dS.stride(-2), table, pb_geom, ctx.needs_input_grad[8])
-        else:
-            L.call("sx_softmax_bwd", dP.data_ptr(), dP.stride(-2), S.data_ptr(), S.stride(-2), lse.data_ptr(), B * M * U1, U2,
-                   stat[2:].data_ptr(), clip, drop_p, *_seed_args(ctx.seed), ldp, dS.data_ptr(), dS.stride(-2),
-                   _rt(), _stream())
-        dq, dk = _score_grads(dS, q, k, M, alpha, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
-        return dq, dk, None, None, None, None, None, None, dT, None
+        M, alpha, clip, drop_p, seed, ldp, pb_geom, kmajor_dq = ctx.meta
+        dS, dT = softmax_backward(dP, S, lse, stat[2:], clip, drop_p, seed, ldp, ctx.leaf, pb_geom, ctx.needs_input_grad[8])
+        dq, dk = _score_grads(dS, q, k, M, alpha, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
+                              kmajor_k=kmajor_dq and _kmajor_copies())
+        return dq, dk, None, None, None, None, None, None, dT, None, None
 
 
 def attn_probs(q, k, M, alpha, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None):
     """Differentiable fused attention probabilities (see _AttnProbs); q, k [B, U, M*d] contiguous, TF32-rounded."""
     return _AttnProbs.apply(q.contiguous(), k.contiguous(), M, float(alpha), float(clip), drop_p, seed, diag,
-                            *_pb_args(posbias))
+                            *_pb_args(posbias), False)
 
 
 def _sgemm(A, B, M, N, K, sa, sb, out=None, alpha=1.0, accumulate=False, Z=1, zs=(0, 0, 0)):
@@ -2007,14 +1830,14 @@ class _Conv1x1Add(torch.autograd.Function):
         gemm_nt(Wr.view(1, 1, Cout, Cin), xr.view(B, 1, Cin, V).transpose(-1, -2), out=y, bias=b, bias_mode=L.SX_BIAS_M,
                 addend=ad, round_out=False)
         ctx.save_for_backward(xr, Wr)
-        ctx.meta = (W.shape, b is not None, addend is not None)
+        ctx.meta = (b is not None, addend is not None)
         ctx.leaves = (W, b)
         return y.view(B, Cout, V)
 
     @staticmethod
     def backward(ctx, dy):
         xr, Wr = ctx.saved_tensors
-        wshape, has_b, has_add = ctx.meta
+        has_b, has_add = ctx.meta
         W, b = ctx.leaves
         B, Cin, V = xr.shape
         Cout = Wr.shape[0]
@@ -2024,12 +1847,7 @@ class _Conv1x1Add(torch.autograd.Function):
             dx = gemm_nt(Wr.t().view(1, 1, Cin, Cout), dy.view(B, 1, Cout, V).transpose(-1, -2), round_out=False)
             dx = dx.view(B, Cin, V)
         if ctx.needs_input_grad[1]:
-            tgt = _grad_target(W)
-            if tgt is not None:
-                gemm_nt(dy.view(B, 1, Cout, V), xr.view(B, 1, Cin, V), out=tgt.view(1, 1, Cout, Cin), reduce_z1=True,
-                        accumulate=True, round_out=False)
-            else:
-                dW = gemm_nt(dy.view(B, 1, Cout, V), xr.view(B, 1, Cin, V), reduce_z1=True, round_out=False).view(wshape)
+            dW = _param_grad(W, dy.view(B, 1, Cout, V), xr.view(B, 1, Cin, V), (1, 1, Cout, Cin), reduce_z1=True)
         if has_b and ctx.needs_input_grad[2]:
             tgt = _grad_target(b)
             buf = tgt if tgt is not None else _zeros((Cout,), dy.device)

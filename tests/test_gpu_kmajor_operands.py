@@ -9,6 +9,7 @@ batch 1 instead of 4: majorness does not depend on the batch), that
       the weight-space value-bank fold), and the two launches that made the step slow are gone;
   (b) the step computes the same bits with the copies on and off.
 """
+import math
 import sys
 
 import pytest
@@ -20,12 +21,11 @@ pytestmark = pytest.mark.gpu
 INHERENT = {
     "dy2.t(), x2.t()": "Linear weight gradient dY^T X (token rows)",
     "dY.transpose(-1, -2), G.transpose(-1, -2)": "grouped output Linear weight gradient dY^T G (token rows)",
-    "P.transpose(-1, -2), dH.transpose(-1, -2)": "dV' = P^T dH (token contraction)",
-    "dS.transpose(-1, -2), q.view": "dK = dS^T Q (token contraction)",
-    "gemm_nt(dS, k.view": "in-squeeze dQ = dS K with the token keys",
+    "dS.transpose(-1, -2), _head_cols(q,": "dK = dS^T Q (token contraction)",
+    "gemm_nt(dS, _head_cols(k,": "in-squeeze dQ = dS K with the token keys",
     "gemm_nt(P, vv,": "in-squeeze P1 h with the token values",
     "gemm_nt(dU, v.view": "in-squeeze backward dP1 = dU h^T",
-    "P.transpose(-1, -2), dU.transpose(-1, -2)": "in-squeeze backward dh = P1^T dU",
+    "P.transpose(-1, -2), dU.transpose(-1, -2)": "dV' = P^T dH and the in-squeeze backward dh = P1^T dU (token contractions)",
     "Wvr.transpose(-1, -2)": "weight-space value-bank fold W' = Wm Wv",
     "d2.t(), a2.t()": "value-bank fold weight gradient (attractor rows)",
     "Wmr.t().view(1, 1, Fd, Fd)": "value-bank fold backward, weight space",
@@ -54,7 +54,7 @@ class _GemmRecorder:
             g = cargs[0]._obj
             f = sys._getframe(1)
             while f is not None and (not f.f_code.co_filename.endswith("ops.py") or
-                                     f.f_code.co_name in ("gemm_nt", "_gemm_nt_1", "call")):
+                                     f.f_code.co_name in ("gemm_nt", "_gemm_nt_1", "_param_grad", "call")):
                 f = f.f_back
             site = (f.f_code.co_qualname, _call_text(f)) if f is not None else ("?", "?")
             self.launches.append(("%dx%dx%d z%d" % (g.M, g.N, g.K, g.Z0 * g.Z1), g.op_dtype, g.A.major, g.B.major) + site)
@@ -94,7 +94,7 @@ def _restore():
     ops.set_precision("tf32")
 
 
-def test_cfg4_step_reads_mn_major_tf32_operands_only_in_token_contractions():
+def test_cfg4_step_reads_mn_major_tf32_operands_only_in_token_contractions_and_squeeze_out_dq_copies_keys():
     from segtran_b200 import _lib as L
     from segtran_b200 import ops
     ops.set_kmajor_copies(True)
@@ -113,6 +113,13 @@ def test_cfg4_step_reads_mn_major_tf32_operands_only_in_token_contractions():
     # the squeeze-out's P.V' and dH = dY Wo ([B*modes] x 2744 x 1024 x 1024) now read both operands K-major
     big = [x for x in tf32 if x[0] == "2744x1024x1024 z4"]
     assert len(big) >= 4 and all(x[2] == x[3] == L.SX_MAJOR_K for x in big), big
+    # the squeeze-out's dQ = dS K (tokens x key width x attractors, one batch per mode) shares its call site with the
+    # in-squeeze dQ, which reads the token keys MN-major; it reads a K-major copy of the attractor keys
+    import bench
+    c = bench.CONFIGS[4]
+    dq = [x for x in tf32 if x[0] == "%dx%dx%d z%d" % (math.prod(c["grid"]), c["dims"][0] // c["modes"], c["attractors"],
+                                                        c["modes"])]
+    assert dq and all(x[2] == x[3] == L.SX_MAJOR_K for x in dq), dq
 
 
 def test_cfg4_step_is_bit_identical_with_and_without_kmajor_copies():

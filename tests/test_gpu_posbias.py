@@ -379,7 +379,8 @@ def test_clamp_then_bias_matches_reference_fixture():
 @pytest.mark.parametrize("grid,B", [((5, 6, 7), 2), ((6, 7), 1)])
 def test_fused_dropout_mask_and_table_gradient(grid, B):
     """The fused forward's dropout mask is the one the biased softmax backward regenerates, and the table gradient of the
-    fused path (the backward _SqueezeOutFused runs) matches float64 autograd of the restatement."""
+    fused path (the backward ops.softmax_backward runs, through softmax_posbias_backward, on the saved raw scores)
+    matches float64 autograd of the restatement."""
     torch.manual_seed(6)
     R, w, M, d, p = 2, 0.7, 4, 16, 0.3
     N = math.prod(grid)

@@ -49,15 +49,15 @@ def cases():
            (("dx_tok", B * U1, 1024, 1024), ("dx_attr", B * U2, 1024, 1024), ("dx_ffn", B * U2, 4096, 1024))}
 
     def pv():
-        ops.gemm_nt(P, ops._bank_operand(vp, B, U2, M, FD), out=G, bias=bm, gelu=True, preact=H, drop_p=0.2, seed=7)
+        ops.gemm_nt(P, ops._head_cols(vp, B, U2, M, FD, ops._kmajor_copies()), out=G, bias=bm, gelu=True, preact=H, drop_p=0.2, seed=7)
 
     def dh():
         ops.gemm_nt(dY, ops._weight_t(Wr, M, FD, FD).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=0.2, seed=7)
         ops.colsum(dH.view(-1, FD), out=dbm)
 
     def dqf():
-        ops.gemm_nt(P, ops._bank_operand(k, B, U2, M, D), out=dq.view(B, U1, M, D).permute(0, 2, 1, 3), alpha=0.0625,
-                    round_out=False, split_k=1)
+        ops.gemm_nt(P, ops._head_cols(k, B, U2, M, D, ops._kmajor_copies()), out=dq.view(B, U1, M, D).permute(0, 2, 1, 3),
+                    alpha=0.0625, round_out=False, split_k=1)
 
     out = {"pv": pv, "dH": dh, "dQ": dqf}
     for name, (dy, W) in lin.items():
