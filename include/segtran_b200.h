@@ -469,6 +469,27 @@ int sx_sw_accumulate(const float* scores, int32_t K, int32_t dx, int32_t dy, int
 int sx_sw_finalize(float* preds, const float* cnt, int32_t K, int64_t V, int32_t brats, float* hard, void* stream);
 
 /* -------------------------------------------------------------------------------------------
+ * 2-D sliding-window inference and per-image evaluation (csrc/sx_eval2d.cu; code/test_util2d.py:169-265, harden_segmap2d
+ * of dataloaders/datasets2d.py:178-196, calc_vcdr of utils/losses.py:76-127).  Bilinear resizes use align_corners=False.
+ * sx_sw2d_accumulate: for one window at (xs, ys) of the [B][K][H2][W2] accumulator, preds += sigmoid(scores bilinearly
+ *   resized from [B][K][h][w] to dx x dy) and the shared [H2][W2] cnt += 1; the resized scores are never written.
+ * sx_sw2d_finalize: soft = preds / cnt cropped to [B][K][H][W] at (hl, wl); hard (int32, same shape): class k >= 1 is
+ *   soft >= 0.5, class 0 is "no class >= 1 fired".
+ * sx_eval2d_counts: per image b, the [K][h][w] soft prediction bilinearly resized to the [K][Hg][Wg] ground truth and
+ *   hardened at 0.5, against gt >= 0.5: counts[b * (3(K-1) + 9) + ...] (int32, zeroed by the caller; accumulated) =
+ *   for c = 1..K-1 |P and G|, |P|, |G| at 3(c-1) + {0,1,2}; then at 3(K-1) + {0..7}, for the prediction then the ground
+ *   truth and for class 1 then class 2, (last occupied row + 1) and (Hg - first occupied row), 0 when none; then the
+ *   number of ground-truth values of classes >= 1 other than 0 and 1.  pred may be NULL (ground-truth part only).
+ *   2 <= K <= 8.  Integer atomics only: the counts do not depend on scheduling.
+ * ------------------------------------------------------------------------------------------- */
+int sx_sw2d_accumulate(const float* scores, int32_t B, int32_t K, int32_t h, int32_t w, int32_t dx, int32_t dy, float* preds,
+                       float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, void* stream);
+int sx_sw2d_finalize(const float* preds, const float* cnt, int32_t B, int32_t K, int32_t H2, int32_t W2, int32_t hl,
+                     int32_t wl, int32_t H, int32_t W, float* soft, int32_t* hard, void* stream);
+int sx_eval2d_counts(const float* pred, int32_t B, int32_t K, int32_t h, int32_t w, const float* gt, int32_t Hg, int32_t Wg,
+                     int32_t* counts, void* stream);
+
+/* -------------------------------------------------------------------------------------------
  * Evaluation metrics of a case (csrc/sx_metrics.cu; code/test_util3d.py:186-215 calculate_metric_percase and medpy 0.4's
  * dc / jc / asd / assd / hd / hd95 with unit voxel spacing and connectivity 1).  The classes of a case are the leading
  * index of [K][n0][n1][n2] uint8 masks (non-zero = foreground, n2 contiguous; a 2-D mask has n0 = 1), so a case costs

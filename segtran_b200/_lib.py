@@ -106,6 +106,9 @@ _PROTOS = {
     "sx_convert": [_P, _I, _L, _P, _I, _I, _P],
     "sx_sw_accumulate": [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "sx_sw_finalize": [_P, _P, _I, _L, _I, _P, _P],
+    "sx_sw2d_accumulate": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P],
+    "sx_sw2d_finalize": [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P],
+    "sx_eval2d_counts": [_P, _I, _I, _I, _I, _P, _I, _I, _P, _P],
     "sx_mask_counts": [_P, _P, _I, _L, _P, _L, _P],
     "sx_surface": [_P, _I, _I, _I, _I, _I, _P, _P],
     "sx_edt_sq": [_P, _I, _I, _I, _I, _P, _P],

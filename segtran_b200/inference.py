@@ -2,7 +2,8 @@
 ``test_util3d.test_single_case`` (code/test_util3d.py:93-184) — same signature, same window enumeration, same padding —
 with the per-patch "sigmoid -> accumulate -> count" update and the final "average -> BraTS consistency -> threshold"
 running as two library kernels (csrc/sx_infer.cu) and the two tri-linear resizes as the library's per-axis kernels.
-No CPU fallback: the volume must live on the GPU."""
+``test_single_batch`` is the 2-D counterpart for ``test_util2d.test_single_batch`` (csrc/sx_eval2d.cu), with the score
+upsample folded into the accumulating kernel.  No CPU fallback: the images must live on the GPU."""
 from __future__ import annotations
 
 import math
@@ -15,7 +16,8 @@ from . import ops
 
 
 def _resize(x, size):
-    """F.interpolate(x, size, mode='trilinear', align_corners=False) via the library's per-axis kernels (no-op if equal)."""
+    """F.interpolate(x, size, mode='bilinear' / 'trilinear', align_corners=False) via the library's per-axis kernels
+    (no-op if equal)."""
     if tuple(x.shape[2:]) == tuple(size):
         return x
     return ops.resize_linear(x.float(), tuple(int(s) for s in size))
@@ -73,4 +75,54 @@ def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, 
         sl = (slice(hl_pad, hl_pad + H), slice(wl_pad, wl_pad + W), slice(dl_pad, dl_pad + D))
         preds_hard = (preds_hard[(slice(None),) + sl] if brats else preds_hard[sl]).clone()
         preds_soft = preds_soft[(slice(None),) + sl].clone()
+    return preds_hard, preds_soft
+
+
+def test_single_batch(net, image_batch, orig_input_size, patch_size, stride, task_name, num_classes, model_type):
+    """image_batch [B,C,H,W] (CUDA) -> (preds_hard int32 [B,K,H,W], preds_soft fp32 [B,K,H,W]), exactly as the reference's
+    test_util2d.test_single_batch (code/test_util2d.py:151-225): zero-pad to orig_input_size, one window per launch in the
+    reference's order, each window's scores upsampled, passed through the sigmoid and accumulated by one kernel
+    (csrc/sx_eval2d.cu), then average, harden_segmap2d and the crop by another.  task_name is unused, as in the reference."""
+    ops._req_cuda(image_batch)
+    B, C, H, W = image_batch.shape
+    dx, dy = orig_input_size
+    h_pad, w_pad = max(dx - H, 0), max(dy - W, 0)
+    add_pad = (h_pad + w_pad) > 0
+    hl_pad, hr_pad = h_pad // 2, h_pad - h_pad // 2
+    wl_pad, wr_pad = w_pad // 2, w_pad - w_pad // 2
+    if add_pad:
+        image_batch = F.pad(image_batch, (wl_pad, wr_pad, hl_pad, hr_pad), mode='constant', value=0)
+    H2, W2 = image_batch.shape[2:]
+    sx = math.ceil((H2 - dx) / stride[0]) + 1
+    sy = math.ceil((W2 - dy) / stride[1]) + 1
+    K = int(num_classes)
+    dev = image_batch.device
+    preds = torch.zeros((B, K, H2, W2), device=dev, dtype=torch.float32)
+    cnt = torch.zeros((H2, W2), device=dev, dtype=torch.float32)
+    st = ops._stream
+
+    for x in range(sx):
+        xs = min(stride[0] * x, H2 - dx)
+        for y in range(sy):
+            ys = min(stride[1] * y, W2 - dy)
+            test_patch = _resize(image_batch[:, :, xs:xs + dx, ys:ys + dy], patch_size)
+            with torch.no_grad():
+                scores_raw = net(test_patch)
+            if model_type == 'pranet':                      # lateral_map_2 lacks the background channel: prepend zeros
+                scores_raw0 = scores_raw[3]
+                scores_raw = torch.cat([torch.zeros_like(scores_raw0[:, [0]]), scores_raw0], dim=1)
+            if model_type == 'nnunet':
+                scores_raw = scores_raw[0]
+            scores_raw = scores_raw.float().contiguous()
+            if scores_raw.dim() != 4 or scores_raw.shape[0] != B or scores_raw.shape[1] != K:
+                raise ValueError("test_single_batch: the net returned scores of shape %s, expected [%d, %d, h, w]"
+                                 % (tuple(scores_raw.shape), B, K))
+            h, w = scores_raw.shape[2:]
+            L.call("sx_sw2d_accumulate", scores_raw.data_ptr(), B, K, h, w, dx, dy, preds.data_ptr(), cnt.data_ptr(),
+                   H2, W2, xs, ys, st())
+
+    preds_soft = torch.empty((B, K, H, W), device=dev, dtype=torch.float32)
+    preds_hard = torch.empty((B, K, H, W), device=dev, dtype=torch.int32)
+    L.call("sx_sw2d_finalize", preds.data_ptr(), cnt.data_ptr(), B, K, H2, W2, hl_pad, wl_pad, H, W, preds_soft.data_ptr(),
+           preds_hard.data_ptr(), st())
     return preds_hard, preds_soft

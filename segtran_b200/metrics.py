@@ -1,10 +1,12 @@
 """Evaluation metrics on the GPU: a drop-in for the reference's ``test_util3d.calculate_metric_percase``
 (code/test_util3d.py:186-215) and medpy 0.4's ``dc, jc, hd, hd95, asd, assd`` (medpy/metric/binary.py) on CUDA tensors,
-with unit voxel spacing and connectivity 1.
+with unit voxel spacing and connectivity 1; and for the 2-D evaluation, ``test_util2d.calc_batch_metric`` and the
+unbatched ``utils/losses.calc_vcdr`` (per-image Dice and vertical cup-to-disc ratio, csrc/sx_eval2d.cu).
 
 Every distance is sqrt of an exact integer squared distance, so the library's kernels (csrc/sx_metrics.cu) compute
 the same dc, jc, hd and hd95 as medpy bit for bit, and asd to the last bits of an fp64 sum in another order.  All
-functions go through ``_case_metrics``: one fixed sequence of launches for all classes of a case, one device-to-host copy.
+medpy-style functions go through ``_case_metrics``: one fixed sequence of launches for all classes of a case, one
+device-to-host copy.  The 2-D functions go through ``_eval2d_counts``: one launch per batch, one device-to-host copy.
 No CPU fallback: the masks must live on the GPU.
 """
 from __future__ import annotations
@@ -167,3 +169,116 @@ def calculate_metric_percase(allcls_pred, allcls_gt, num_classes, hd95=False):
             valid[i, 3] = 0
         metric[i] = [dice, jac, hdv, asdv]
     return metric, valid
+
+
+# ------------------------------------------------------------------------------------------------
+# 2-D per-image evaluation: drop-ins for test_util2d.calc_batch_metric / calc_dice (code/test_util2d.py:229-265) and the
+# unbatched branch of utils/losses.calc_vcdr (:76-127), from the integer counts of sx_eval2d_counts (csrc/sx_eval2d.cu)
+# ------------------------------------------------------------------------------------------------
+_ROWS = 8                     # row slots per image: {pred, gt} x {disc, cup} x {last row + 1, H - first row}
+
+
+def _eval2d_ld(K: int) -> int:
+    return 3 * (K - 1) + _ROWS + 1
+
+
+def _eval2d_counts(preds, gts, K: int) -> np.ndarray:
+    """preds: a [B,K',h,w] CUDA tensor or a list of [K',h,w] ones (None: ground-truth part only); gts likewise, with
+    K', h, w free per image in a list.  -> int64 [B, 3(K-1) + 9] counts of the first K classes, one device-to-host copy."""
+    B = len(gts)
+    if preds is not None and len(preds) != B:
+        raise ValueError("calc_batch_metric: %d predictions for %d ground truths" % (len(preds), B))
+    if B == 0:
+        return np.zeros((0, _eval2d_ld(K)), dtype=np.int64)
+    if torch.is_tensor(gts) and (preds is None or torch.is_tensor(preds)):
+        groups = [(preds, gts)]                                     # one shape: the whole batch in one launch
+    else:                                                           # images of different sizes: one launch each
+        groups = [(None if preds is None else preds[b].unsqueeze(0), gts[b].unsqueeze(0)) for b in range(B)]
+    for p, g in groups:
+        ops._req_cuda(p, g)
+        if g.dim() != 4 or g.shape[1] < K or (p is not None and (p.dim() != 4 or p.shape[1] < K)):
+            raise ValueError("calc_batch_metric: need [C,H,W] maps of at least %d classes, got %s and %s"
+                             % (K, None if p is None else tuple(p.shape[1:]), tuple(g.shape[1:])))
+    counts = torch.zeros((B, _eval2d_ld(K)), device=groups[0][1].device, dtype=torch.int32)
+    st = ops._stream()
+    b0 = 0
+    for p, g in groups:
+        g = g[:, :K].float().contiguous()
+        h = w = 0
+        if p is not None:
+            p = p[:, :K].float().contiguous()
+            h, w = p.shape[2:]
+        n = g.shape[0]
+        L.call("sx_eval2d_counts", ops._ptr(p), n, K, h, w, g.data_ptr(), g.shape[2], g.shape[3], counts[b0].data_ptr(),
+               st)
+        b0 += n
+    return counts.cpu().numpy().astype(np.int64)
+
+
+def _vcdr(rows: np.ndarray, H: int) -> np.float32:
+    """calc_vcdr (losses.py:102-127) of one mask from its four row slots [disc last+1, disc H-first, cup last+1,
+    cup H-first]: fp32 cup_len / (disc_len + 1e-4) with len = last - first - 1; -1 without a disc, 0 without a cup."""
+    if rows[0] == 0:
+        return np.float32(-1.)
+    disc_len = int(rows[0] - 1) - int(H - rows[1]) - 1
+    if rows[2] == 0:
+        return np.float32(0.)
+    cup_len = int(rows[2] - 1) - int(H - rows[3]) - 1
+    return np.float32(cup_len) / (np.float32(disc_len) + np.float32(1e-4))
+
+
+def _batch_values(counts: np.ndarray, K: int, heights, do_calc_vcdr_error: bool) -> np.ndarray:
+    """calc_batch_metric's array from the counts of sx_eval2d_counts, in the reference's fp32 operation order.
+    heights: the ground-truth height of each image."""
+    B = counts.shape[0]
+    nc = K - 1
+    bad = counts[:, 3 * nc + _ROWS]
+    if bad.any():
+        raise ValueError("calc_batch_metric: the ground truth must be binary (0/1); %d values of classes 1..%d are not"
+                         % (int(bad.sum()), nc))
+    out = np.zeros((B, nc + int(bool(do_calc_vcdr_error))))
+    eps = np.float32(1e-5)
+    for b in range(B):
+        for c in range(nc):
+            inter, p, g = (np.float32(v) for v in counts[b, 3 * c:3 * c + 3])
+            out[b, c] = (np.float32(2) * inter + eps) / ((p + g) + eps)          # calc_dice, test_util2d.py:229-236
+        if do_calc_vcdr_error:
+            r = counts[b, 3 * nc:3 * nc + _ROWS]
+            out[b, nc] = np.abs(_vcdr(r[4:], heights[b]) - _vcdr(r[:4], heights[b]))
+    return out
+
+
+def _require_vcdr_classes(K: int):
+    if K < 3:
+        raise ValueError("vCDR needs the disc (class 1) and cup (class 2) channels: num_classes >= 3, got %d" % K)
+
+
+def calc_batch_metric(BC_pred_soft, BC_gt, num_classes, do_calc_vcdr_error=False):
+    """Drop-in for test_util2d.calc_batch_metric: per image, the soft prediction bilinearly resized to its ground truth's
+    size and hardened at 0.5 (harden_segmap2d), the Dice of each class 1..K-1 ((2|P and G| + 1e-5) / (|P| + |G| + 1e-5)
+    in fp32) and, with do_calc_vcdr_error, |vCDR(gt) - vCDR(pred)|.  BC_pred_soft / BC_gt: [B,K,h,w] / [B,K,H,W] CUDA
+    tensors, or lists of [K,h,w] / [K,H,W] ones of per-image sizes.  The ground truth must be binary (every
+    mask_prepred_mapping_func gives 0/1): ValueError otherwise.  One kernel launch per batch (per image for lists) and one
+    device-to-host copy.  -> float64 numpy [B, K-1+do_calc_vcdr_error], bit-identical to the reference for the same
+    hard masks."""
+    K = int(num_classes)
+    if do_calc_vcdr_error:
+        _require_vcdr_classes(K)
+    if K < 2:
+        raise ValueError("calc_batch_metric: num_classes must be >= 2, got %d" % K)
+    counts = _eval2d_counts(BC_pred_soft, BC_gt, K)
+    heights = [int(g.shape[-2]) for g in BC_gt]
+    return _batch_values(counts, K, heights, do_calc_vcdr_error)
+
+
+def calc_vcdr(mask):
+    """Drop-in for utils/losses.calc_vcdr on one [C,H,W] mask (C >= 3; classes 1: disc, 2: cup; occupied = >= 0.5):
+    the vertical cup-to-disc ratio as a 0-dim fp32 tensor on the mask's device (-1 without a disc, 0 without a cup)."""
+    ops._req_cuda(mask)
+    if mask.dim() != 3:
+        raise ValueError("calc_vcdr: one [C,H,W] mask expected (the batched form is not implemented), got %s"
+                         % (tuple(mask.shape),))
+    _require_vcdr_classes(mask.shape[0])
+    counts = _eval2d_counts(None, mask[:3].unsqueeze(0), 3)
+    rows = counts[0, 6:6 + _ROWS]
+    return torch.tensor(_vcdr(rows[4:], int(mask.shape[1])), device=mask.device)
