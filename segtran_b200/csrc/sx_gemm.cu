@@ -2,7 +2,8 @@
 //
 //   C[z][m][n] = epilogue(alpha * sum_k A[z][m][k] * B[z][n][k])
 //
-// Persistent, warp-specialised kernel, one CTA per SM, 128 x 128 output tiles:
+// Persistent, warp-specialised kernel, one CTA per SM, 128 x 128 output tiles, or 128 x 256 for large TF32 products with
+// both operands K-major (see sx_gemm() for the rule):
 //   warpgroup 0    : warp 0: TMA producer (one elected thread: cp.async.bulk.tensor 4-D boxes, 128-byte swizzle);
 //                    warps 1-3: transposers (tf32 MN-major operands only, see below)
 //   warpgroups 1-2 : consumers, 64 tile rows each: wgmma.mma_async with the fp32 accumulators in registers, then the
@@ -12,6 +13,9 @@
 // tf32 wgmma reads K-major operands only, so TMA lands an MN-major tf32 tile in a raw ring and the transposer warps
 // rewrite it into the K-major stage the consumers read.  The consumers run the same loop for every majorness.
 // Operand arithmetic: tf32 on fp32 storage (parity-grade) or bf16 storage (fast).
+// A 128 x 256 tile (each consumer issues m64n256k8 into 128 accumulators) moves 25 % fewer operand bytes from L2 into
+// shared memory per FLOP than a 128 x 128 tile.  Every output element still sees the same k-blocks in the same order and
+// the same k8 steps, so both tile widths give bit-identical results.
 //
 // Replaces in the reference: nn.Linear / torch.matmul / grouped Conv1d call sites on the hot path,
 // code/networks/segtran_shared.py:243, :267, :414, :447, :559-560, :566 (and their autograd backward).
@@ -26,20 +30,25 @@ using namespace sxtc;
 
 constexpr int NUM_THREADS = 384;          // warpgroup 0: TMA + transposers; warpgroups 1-2: MMA + epilogue
 constexpr int STAGES = 4;                 // K-major operand ring (what wgmma reads)
-constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;     // 32 KB
 constexpr int XPOSE_WARPS = 3;            // warps 1-3 of warpgroup 0
+constexpr int BN_WIDE = 256;              // tile cols of the wide instantiation (tf32, both operands K-major)
 
 // Shared-memory plan of one instantiation.  A tf32 MN-major operand goes through a raw ring (as TMA lands it) before
-// the transposers write its K-major copy into the stage; everything else lands in the stage directly.
-template <int ES, bool A_MN, bool B_MN>
+// the transposers write its K-major copy into the stage; everything else lands in the stage directly.  BN_T = 256 (the
+// wide tile) has K-major tf32 operands only: 16 KB of A + 32 KB of B per stage, no raw ring.
+template <int ES, bool A_MN, bool B_MN, int BN_T>
 struct Plan {
+  static_assert(BN_T == BN || (BN_T == BN_WIDE && ES == 4 && !A_MN && !B_MN),
+                "sx_gemm: the 256-column tile is instantiated for K-major tf32 operands only");
+  static constexpr int B_BYTES = BN_T * BKB;                          // B operand tile per stage: 16 / 32 KB
+  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_BYTES;         // 32 / 48 KB
   static constexpr bool XA = ES == 4 && A_MN, XB = ES == 4 && B_MN;
   static constexpr bool XPOSE = XA || XB;
   static constexpr int RAW_BYTES = (XA ? A_STAGE_BYTES : 0) + (XB ? B_STAGE_BYTES : 0);      // per raw slot
   static constexpr int RAW_SLOTS = !XPOSE ? 0 : (XA && XB ? 3 : 4);
   static constexpr int DIRECT_BYTES = STAGE_BYTES - RAW_BYTES;   // per stage, loaded by TMA straight into the stage
   static constexpr int SMEM = STAGES * STAGE_BYTES + RAW_SLOTS * RAW_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  static_assert(SMEM <= 227 * 1024, "sx_gemm: shared memory plan exceeds 227 KB");
+  static_assert(SMEM <= 227 * 1024, "sx_gemm: shared memory plan exceeds 227 KB");   // wide: 4 x 48 KB + 1.25 KB
   // the transposers address B at A's offset + A_STAGE_BYTES in both the raw slot and the stage, and move 256 4 x 4
   // blocks (4 boxes of 32 x 32) per operand: both hold only for 128 x 128 tf32 operand tiles
   static_assert(!XPOSE || (A_STAGE_BYTES == 16384 && B_STAGE_BYTES == 16384 && BM == 128 && BN == 128),
@@ -101,11 +110,13 @@ __device__ __forceinline__ void xpose_store(uint32_t dst, int b, const float4 (&
   st(3, v[0].w, v[1].w, v[2].w, v[3].w);
 }
 
-template <int ES, bool A_MN, bool B_MN>
+template <int ES, bool A_MN, bool B_MN, int BN_T>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using PL = Plan<ES, A_MN, B_MN>;
+  using PL = Plan<ES, A_MN, B_MN, BN_T>;
   constexpr bool kTF32 = (ES == 4);
+  constexpr bool WIDE = BN_T == BN_WIDE;
+  constexpr int STAGE_BYTES = PL::STAGE_BYTES;
   constexpr bool XA = PL::XA, XB = PL::XB;
   constexpr int BK = BKB / ES;                 // elements of K per stage: 64 (bf16) / 32 (tf32)
   constexpr int MN_BOX = BKB / ES;             // contiguous MN elements per MN-major box: 64 / 32
@@ -151,7 +162,9 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   auto split_kbs = [&](int ks) { return min(p.num_kb, (ks + 1) * p.kb_per_split) - ks * p.kb_per_split; };
 
   if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");   // the producers hand their registers over
+    // the producers hand their registers over (the wide tile has no transposers: its producer keeps only 40)
+    if constexpr (WIDE) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    else asm volatile("setmaxnreg.dec.sync.aligned.u32 56;" ::: "memory");
     if (warp == 0) {
       // ===================== TMA producer =====================
       if (sx::elect_one()) {
@@ -165,7 +178,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           decode(t, z0, z1, mb, nb, ks);
           const int kb0 = ks * p.kb_per_split;
           const int az0 = p.a_uses_z0 ? z0 : 0, bz0 = p.b_uses_z0 ? z0 : 0;
-          const int m0 = mb * BM, n0 = nb * BN;
+          const int m0 = mb * BM, n0 = nb * BN_T;
           const int nkb = split_kbs(ks);
           for (int q = 0; q < p.z1_loop * nkb; ++q) {
             const int kb = kb0 + q % nkb, zc = p.z1_loop > 1 ? q / nkb : z1;
@@ -183,7 +196,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               }
               if constexpr (XB) {
 #pragma unroll
-                for (int j = 0; j < BN / MN_BOX; ++j)
+                for (int j = 0; j < BN_T / MN_BOX; ++j)
                   sx::tma_load_4d(rb + j * MN_BOX_BYTES, &tmB, &raw_full[rs], n0 + j * MN_BOX, k0, bz0, bz1, pol);
               }
               if (++rs == PL::RAW_SLOTS) { rs = 0; rphase ^= 1; }
@@ -207,7 +220,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                   sx::tma_load_4d(sb, &tmB, &full_bar[stage], k0, n0, bz0, bz1, pol);
                 } else {
 #pragma unroll
-                  for (int j = 0; j < BN / MN_BOX; ++j)
+                  for (int j = 0; j < BN_T / MN_BOX; ++j)
                     sx::tma_load_4d(sb + j * MN_BOX_BYTES, &tmB, &full_bar[stage], n0 + j * MN_BOX, k0, bz0, bz1, pol);
                 }
               }
@@ -251,14 +264,14 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     return;
   }
 
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 224;" ::: "memory");
+  if constexpr (WIDE) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");    // 128 x 40 + 256 x 232
+  else asm volatile("setmaxnreg.inc.sync.aligned.u32 224;" ::: "memory");
   // ===================== consumers: MMA + epilogue =====================
   const int cw = wg - 1;                        // tile rows 64 cw .. 64 cw + 63
   const int wtid = threadIdx.x & 127;           // thread within the warpgroup
   const int wq = warp & 3;                      // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of those
   const int tr = lane >> 2;                     // row within an 8-row group
   const int tc = (lane & 3) * 2;                // first column of this thread's pair within an 8-column group
-  float tmax = -3.0e38f;
   int stage = 0;
   uint32_t phase = 0;
 
@@ -335,7 +348,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const unsigned long long drop_seed = p.drop_p > 0.f ? p.drop_seed + (p.drop_seed_dev ? *p.drop_seed_dev : 0ull) : 0ull;
   const uint32_t drop_mul_t = sx::drop_mul((tc >> 1) & 1), drop_key_t = sx::drop_key(drop_seed, (tc >> 1) & 1);
 
-  float acc[64];
+  float acc[BN_T / 2];                          // 64 rows x BN_T cols over 128 threads
   for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
     int z0, z1, mb, nb, ks;
     decode(t, z0, z1, mb, nb, ks);
@@ -353,7 +366,8 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int kk = 0; kk < KSTEPS; ++kk) {
         const uint64_t da = desc_a(sa, kk, A_MN && !kTF32), db = desc_b(sb, kk, B_MN && !kTF32);
         const uint32_t accum = (q > 0 || kk > 0) ? 1u : 0u;
-        if constexpr (kTF32) sx::wgmma_tf32(acc, da, db, accum);
+        if constexpr (WIDE) sx::wgmma_tf32_n256(acc, da, db, accum);
+        else if constexpr (kTF32) sx::wgmma_tf32(acc, da, db, accum);
         else sx::wgmma_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, accum);
       }
       sx::wgmma_commit();
@@ -372,6 +386,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const float* bias = p.bias ? p.bias + (long long)z1 * p.bias_sz1 + (long long)z0 * p.bias_sz0 : nullptr;
     const bool add_bias = (bias != nullptr) && (ks == 0);
     const int row0 = mb * BM + cw * 64 + wq * 16;
+    float tmax = -3.0e38f;                                // running max of this tile's outputs (p.amax)
     float bias_m[2] = {0.f, 0.f};                         // [h]
     if (add_bias && p.bias_mode == SX_BIAS_M) {
 #pragma unroll
@@ -380,13 +395,17 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         bias_m[h] = r < p.M ? bias[r] : 0.f;
       }
     }
-#pragma unroll
-    for (int c = 0; c < BN / 32; ++c) {
-      const int col0 = nb * BN + c * 32;
+    // the wide tile runs its 8 column chunks as a rolled loop (unrolled, the 128 accumulators plus the interleaved
+    // epilogues of several chunks exceed the consumer's registers): it always takes acc[0..15], then moves the
+    // remaining chunks forward
+    constexpr int EPI_UNROLL = WIDE ? 1 : BN_T / 32;
+#pragma unroll EPI_UNROLL
+    for (int c = 0; c < BN_T / 32; ++c) {
+      const int col0 = nb * BN_T + c * 32;
       if (col0 >= p.N) break;                   // warp-uniform
       float f[16];
 #pragma unroll
-      for (int i = 0; i < 16; ++i) f[i] = acc[16 * c + i] * p.alpha + bias_m[(i >> 1) & 1];
+      for (int i = 0; i < 16; ++i) f[i] = acc[(WIDE ? 0 : 16 * c) + i] * p.alpha + bias_m[(i >> 1) & 1];
       if (p.addend) {
         float g[16];
         load_frag(p.addend, g, zoff, row0, col0);
@@ -466,7 +485,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 if (col0 + 8 * j + tc + e < p.N) tmax = fmaxf(tmax, f[4 * j + 2 * h + e]);
           }
       }
-      if (p.split_k > 1) {
+      if (!WIDE && p.split_k > 1) {           // (the wide tile never splits)
         // this split's partial tile (local row-major 128 x 128), summed over the splits in order by split_reduce_kernel
         float* pt = p.part + ((((long long)z1 * p.Z0 + z0) * p.tiles_m + mb) * p.tiles_n + nb) * p.split_k * (BM * BN) +
                     (long long)ks * (BM * BN);
@@ -479,11 +498,17 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       } else {
         store_frag(p.C, f, zoff, row0, col0, p.accumulate != 0);
       }
+      if constexpr (WIDE) {
+#pragma unroll
+        for (int i = 0; i < BN_T / 2 - 16; ++i) acc[i] = acc[i + 16];
+      }
     }
-  }
-  if (p.amax) {
-    tmax = sx::warp_max(tmax);
-    if (lane == 0 && tmax > -3.0e38f) sx::atomic_max_float(p.amax, tmax);
+    // reduced per tile: a running max held across the whole persistent loop keeps ptxas from giving the consumers
+    // setmaxnreg's registers (the wide tile's 128 accumulators then spill)
+    if (p.amax) {
+      tmax = sx::warp_max(tmax);
+      if (lane == 0 && tmax > -3.0e38f) sx::atomic_max_float(p.amax, tmax);
+    }
   }
 }
 
@@ -509,11 +534,12 @@ __global__ void split_reduce_kernel(const GemmParams p) {
 // host side
 // ------------------------------------------------------------------------------------------------
 long long g_max_ctas = -1;         // cap on the persistent grid (tests drive the multi-tile-per-CTA schedule with it)
+int g_wide_tiles = -1;             // 128 x 256 tiles: -1 by shape, 0 never, 1 wherever legal (tests compare the two widths)
 
-template <int ES, bool A_MN, bool B_MN>
+template <int ES, bool A_MN, bool B_MN, int BN_T = BN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int grid, cudaStream_t st) {
-  auto kern = sx_gemm_kernel<ES, A_MN, B_MN>;
-  constexpr int bytes = Plan<ES, A_MN, B_MN>::SMEM;
+  auto kern = sx_gemm_kernel<ES, A_MN, B_MN, BN_T>;
+  constexpr int bytes = Plan<ES, A_MN, B_MN, BN_T>::SMEM;
   SX_CHECK_CUDA(set_max_smem_once(kern, bytes));         // per device (a process may drive several GPUs)
   kern<<<grid, NUM_THREADS, bytes, st>>>(ta, tb, p);
   SX_CHECK_CUDA(cudaGetLastError());
@@ -530,6 +556,7 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, in
 extern "C" int sx_gemm_debug_set(const char* key, int64_t value) {
   std::string k(key);
   if (k == "max_ctas") g_max_ctas = value;
+  else if (k == "wide_tiles") g_wide_tiles = value < 0 ? -1 : (value ? 1 : 0);
   else {
     sx_set_error("sx_gemm_debug_set: unknown key %s", key);
     return -1;
@@ -577,6 +604,15 @@ extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
   SX_REQUIRE(!a->round_tf32 || (!a->accumulate && p.split_k == 1),
              "sx_gemm: round_tf32 cannot be combined with accumulate / split_k > 1 (a sum of rounded partials is not a TF32 "
              "value): round the finished output instead");
+  // 128 x 256 tiles (fewer operand bytes per FLOP) for tf32 products with both operands K-major and no split, when N
+  // spans more than one narrow tile and the narrow tiles would take more than one wave.  (H100 SXM at 700 W, plain
+  // products: 2744x1024x1024 z16 1.27x faster at 1408 wide tiles, 4096x1024x1024 1.42x at 128; 2744x512x1024 z4,
+  // 176 wide tiles = 1.3 waves, 1.01x.)
+  const bool amn = a->A.major == SX_MAJOR_MN, bmn = a->B.major == SX_MAJOR_MN;
+  const bool wide_legal = es == 4 && !amn && !bmn && p.split_k == 1;
+  const long long wide_tt = (long long)p.tiles_m * sx_ceil_div(a->N, BN_WIDE) * a->Z0 * p.Z1;
+  const bool wide = wide_legal && (g_wide_tiles == 1 || (g_wide_tiles < 0 && a->N > BN && 2 * wide_tt > sms));
+  if (wide) p.tiles_n = sx_ceil_div(a->N, BN_WIDE);
   const long long tt = (long long)p.tiles_m * p.tiles_n * p.split_k * a->Z0 * p.Z1;
   SX_REQUIRE(tt < (1ll << 30), "sx_gemm: too many tiles");
   p.total_tiles = (int)tt;
@@ -606,14 +642,14 @@ extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
   CUtensorMap ta, tb;
   int rc = make_map(&ta, a->A, es, a->M, a->K, a->Z0, a->Z1, BM, "A");
   if (rc) return rc;
-  rc = make_map(&tb, a->B, es, a->N, a->K, a->Z0, a->Z1, BN, "B");
+  rc = make_map(&tb, a->B, es, a->N, a->K, a->Z0, a->Z1, wide ? BN_WIDE : BN, "B");
   if (rc) return rc;
 
   int grid = p.total_tiles < sms ? p.total_tiles : sms;
   if (g_max_ctas > 0 && grid > g_max_ctas) grid = (int)g_max_ctas;
   p.part = a->part;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const bool amn = a->A.major == SX_MAJOR_MN, bmn = a->B.major == SX_MAJOR_MN;
+  if (wide) return launch<4, false, false, BN_WIDE>(ta, tb, p, grid, st);
   if (es == 4) {
     if (!amn && !bmn) return launch<4, false, false>(ta, tb, p, grid, st);
     if (!amn && bmn) return launch<4, false, true>(ta, tb, p, grid, st);

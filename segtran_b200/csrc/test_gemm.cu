@@ -1,10 +1,12 @@
 // Stand-alone bring-up / regression driver for sx_gemm (no Python, no torch).
-//   ./test_gemm [key=value ...]     keys: the sx_gemm_debug_set knobs, plus perf=1 only=<substr>
+//   ./test_gemm [key=value ...]     keys: the sx_gemm_debug_set knobs, plus perf=1 only=<substr> widesweep=1
+// (wide_tiles=1 runs every K-major tf32 case on the 128 x 256 tile; widesweep=1 times narrow against wide tiles)
 // Every case is checked against a double-precision host product of the (pre-rounded) operands.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
 #include <vector>
 
@@ -248,8 +250,67 @@ static void perf_epi(const char* name, int bias, int pre, int gelu, float drop, 
   if (dP) cudaFree(dP);
 }
 
+// narrow (128 x 128) against wide (128 x 256) tiles on one K-major tf32 product, alternating, `rounds` times each;
+// epi: 0 none, 1 GELU + dropout + pre-activation store, 2 GELU' (reads the pre-activation) + dropout
+static void perf_wide(int M, int N, int K, int Z, int epi, int rounds) {
+  float *dA, *dB, *dC, *dP = nullptr, *dbias;
+  cudaMalloc(&dA, (size_t)M * K * Z * 4); cudaMalloc(&dB, (size_t)N * K * Z * 4); cudaMalloc(&dC, (size_t)M * N * Z * 4);
+  cudaMalloc(&dbias, N * 4);
+  fill_rand_kernel<<<1024, 256>>>(dA, (size_t)M * K * Z, 1u, 1.f);
+  fill_rand_kernel<<<1024, 256>>>(dB, (size_t)N * K * Z, 2u, 1.f);
+  fill_rand_kernel<<<4, 256>>>(dbias, N, 3u, 0.1f);
+  if (epi) {
+    cudaMalloc(&dP, (size_t)M * N * Z * 4);
+    fill_rand_kernel<<<1024, 256>>>(dP, (size_t)M * N * Z, 4u, 2.f);
+  }
+  sx_gemm_args g;
+  memset(&g, 0, sizeof(g));
+  g.op_dtype = SX_OP_TF32; g.M = M; g.N = N; g.K = K; g.Z0 = Z; g.Z1 = 1;
+  g.A.ptr = dA; g.A.major = SX_MAJOR_K; g.A.ld = K; g.A.stride_z0 = Z > 1 ? (long long)M * K : 0;
+  g.B.ptr = dB; g.B.major = SX_MAJOR_K; g.B.ld = K; g.B.stride_z0 = Z > 1 ? (long long)N * K : 0;
+  g.C = dC; g.c_dtype = SX_F32; g.ldc = N; g.c_stride_z0 = (long long)M * N; g.alpha = 1.f; g.split_k = 1;
+  g.round_tf32 = 1;
+  if (epi == 1) { g.bias = dbias; g.bias_mode = SX_BIAS_N; g.act = SX_ACT_GELU; g.preact = dP; }
+  if (epi == 2) { g.act = SX_ACT_GELU_BWD; g.preact = dP; }
+  if (epi) { g.drop_p = 0.2f; g.drop_seed = 77; }
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  const int iters = 20;
+  std::vector<float> t[2];
+  for (int w = 0; w < 2; ++w) {
+    sx_gemm_debug_set("wide_tiles", w);
+    for (int i = 0; i < 3; ++i) sx_gemm(&g, nullptr);
+  }
+  for (int r = 0; r < rounds; ++r)
+    for (int w = 0; w < 2; ++w) {
+      sx_gemm_debug_set("wide_tiles", w);
+      cudaDeviceSynchronize();
+      cudaEventRecord(e0);
+      for (int i = 0; i < iters; ++i) sx_gemm(&g, nullptr);
+      cudaEventRecord(e1);
+      cudaEventSynchronize(e1);
+      float ms = 0;
+      cudaEventElapsedTime(&ms, e0, e1);
+      t[w].push_back(ms / iters);
+    }
+  sx_gemm_debug_set("wide_tiles", -1);
+  const double fl = 2.0 * M * N * K * Z;
+  const int tiles_n = (N + 127) / 128, tiles_w = (N + 255) / 256, tm = (M + 127) / 128;
+  for (int w = 0; w < 2; ++w) {
+    std::sort(t[w].begin(), t[w].end());
+    const float med = t[w][t[w].size() / 2];
+    printf("WIDE %-6s M=%d N=%d K=%d Z=%d epi=%d tiles=%d : median %.4f ms (min %.4f max %.4f)  %.1f TFLOP/s\n",
+           w ? "wide" : "narrow", M, N, K, Z, epi, tm * (w ? tiles_w : tiles_n) * Z, med, t[w].front(), t[w].back(),
+           fl / (med * 1e-3) / 1e12);
+  }
+  printf("WIDE speedup M=%d N=%d K=%d Z=%d epi=%d : %.3fx  (%s)\n", M, N, K, Z, epi,
+         t[0][t[0].size() / 2] / t[1][t[1].size() / 2], cudaGetErrorString(cudaGetLastError()));
+  cudaFree(dA); cudaFree(dB); cudaFree(dC); cudaFree(dbias);
+  if (dP) cudaFree(dP);
+}
+
 int main(int argc, char** argv) {
-  bool do_perf = false, ksweep = false, episweep = false;
+  bool do_perf = false, ksweep = false, episweep = false, widesweep = false;
   std::string only;
   for (int i = 1; i < argc; ++i) {
     char* eq = strchr(argv[i], '=');
@@ -258,6 +319,7 @@ int main(int argc, char** argv) {
     if (k == "perf") { do_perf = atoi(eq + 1) != 0; continue; }
     if (k == "ksweep") { ksweep = atoi(eq + 1) != 0; continue; }
     if (k == "episweep") { episweep = atoi(eq + 1) != 0; continue; }
+    if (k == "widesweep") { widesweep = atoi(eq + 1) != 0; continue; }
     if (k == "only") { only = eq + 1; continue; }
     if (sx_gemm_debug_set(k.c_str(), atoll(eq + 1)) != 0) { printf("bad knob %s\n", k.c_str()); return 3; }
     printf("knob %s=%lld\n", k.c_str(), atoll(eq + 1));
@@ -295,6 +357,11 @@ int main(int argc, char** argv) {
       {"tf32_round_amax",          T, K_, K_, 300, 520, 200, 1, 1, 0, 1, 1, 0, 0, 1, 0, 1, 0.25f},
       {"bf16_out_bf16_gelu",       H, K_, K_, 300, 520, 200, 1, 1, 0, 1, 1, 1, 1, 0, 1, 0, 1.f},
       {"tf32_many_tiles",          T, K_, K_, 1300, 2100, 96, 2, 1, 0, 1, 0, 0, 0, 0, 0, 0, 1.f},
+      // ragged N against the 256-column tile (K-major tf32: the wide path under wide_tiles=1)
+      {"tf32_kk_n136",             T, K_, K_, 300, 136, 200, 1, 1, 0, 1, 0, 0, 0, 0, 0, 0, 1.f},
+      {"tf32_kk_n1000_bias_gelu",  T, K_, K_, 330, 1000, 96, 2, 1, 0, 1, 1, 1, 0, 0, 1, 0, 1.f},
+      {"tf32_kk_bcastB_batched",   T, K_, K_, 150, 300, 100, 3, 2, 1, 1, 0, 0, 0, 0, 0, 0, 1.f},
+      {"tf32_kk_bias_m_round_amax",T, K_, K_, 260, 600, 64, 1, 1, 0, 1, 2, 0, 0, 1, 0, 1, 0.5f},
   };
   int fails = 0, ran = 0;
   for (auto& c : cases) {
@@ -315,6 +382,20 @@ int main(int argc, char** argv) {
     perf_epi("bias+round+gelu+dropout", 1, 0, 1, 0.2f, 1);
     perf_epi("all (preact+gelu+dropout)", 1, 1, 1, 0.2f, 1);
     return 0;
+  }
+  if (widesweep) {
+    // the cfg-4 step's K-major tf32 products, then tile counts around the selection threshold (2 x 132 wide tiles)
+    perf_wide(2744, 1024, 1024, 16, 0, 5);
+    perf_wide(2744, 1024, 1024, 16, 1, 5);
+    perf_wide(2744, 1024, 1024, 16, 2, 5);
+    perf_wide(10976, 1024, 1024, 1, 0, 5);
+    perf_wide(10976, 1024, 1024, 1, 1, 5);
+    perf_wide(4096, 1024, 1024, 1, 0, 5);       // 128 wide tiles (~1 wave)
+    perf_wide(8192, 1024, 1024, 1, 0, 5);       // 256 wide tiles (~2 waves)
+    perf_wide(2744, 512, 1024, 4, 0, 5);        // 176 wide tiles
+    perf_wide(2744, 1024, 256, 16, 0, 5);
+    perf_wide(8192, 8192, 8192, 1, 0, 3);
+    return fails ? 1 : 0;
   }
   if (ksweep) {
     const int Ks[] = {128, 256, 512, 1024, 2048, 4096};
