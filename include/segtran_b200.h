@@ -345,12 +345,24 @@ int sx_head_contract_bwd_data(const float* dL, const float* W, int32_t B, int32_
                               float* dcurr, void* stream);
 int sx_head_contract_bwd_weight(const float* dL, const float* curr, int32_t B, int32_t Cf, int64_t V, int32_t K,
                                 float* dW, float* part, int64_t part_floats, void* stream);
-/* class scores of the fused tokens, exact fp32: out[b,k,n] = sum_f W[k,f] vf[b,n,f]   (Wc . vfeat_fused) */
+/* class scores of the fused tokens, exact fp32: out[b,k,n] = sum_f W[k,f] vf[b,n,f]   (Wc . vfeat_fused), K <= 32 rows
+ * (the collapsed head's classes, or the direct head's 4 sub-pixel rows per class); vf is read once for all rows */
 int sx_token_scores(const float* vf, const float* W, int32_t B, int32_t N, int32_t F, int32_t K, float* out,
                     void* stream);
-/* and its data gradient: dvf[b,n,f] = sum_k dt[b,k,n] W[k,f]   (F % 4 == 0) */
+/* and its data gradient: dvf[b,n,f] = sum_k dt[b,k,n] W[k,f]   (F % 4 == 0, K <= 32) */
 int sx_token_scores_bwd(const float* dt, const float* W, int32_t B, int32_t N, int32_t F, int32_t K, float* dvf,
                         void* stream);
+/* Direct class head (out_fpn_layers == in_fpn_layers; segtran2d.py:198-209, :421-437, segtran3d.py:234-245, :478-498):
+ * the 2x2(x1) stride-2 transposed conv of the tokens followed by bi/trilinear interpolation (align_corners=False) to
+ * the input size, without the upsampled score map.  S [B][4K][N]: sub-pixel scores, row 4k + 2a + c = output cell
+ * (2y+a, 2x+c) of class k (sx_token_scores with the transposed-conv weight as [4K, C]); token n = d*H2*W2 + y*W2 + x.
+ * fwd: out [B][K][H][W][D] = trilinear resampling of the virtual grid (2H2, 2W2, D2) to (H, W, D), + bias[k] (bias may
+ * be NULL).  2-D: D2 = D = 1, out [B][K][H][W].  bwd: dS [B][4K][N] = its adjoint in gather form (fixed summation order,
+ * no atomics).  The bias gradient is the row sum of dS per class (sx_rowsum): interpolation weights sum to one. */
+int sx_subpixel_resize_fwd(const float* S, const float* bias, int32_t B, int32_t K, int32_t D2, int32_t H2, int32_t W2,
+                           int32_t H, int32_t W, int32_t D, float* out, void* stream);
+int sx_subpixel_resize_bwd(const float* dout, int32_t B, int32_t K, int32_t D2, int32_t H2, int32_t W2, int32_t H,
+                           int32_t W, int32_t D, float* dS, void* stream);
 /* Out-FPN dropout head (--outdrop; segtran3d.py:372-396, :488-490; segtran2d.py:304-311, :427), which cannot be
  * collapsed: the dropout mask is per channel.  The dropped map X [B,F',D',HW] is never written:
  *   Ls[b,k,d',hw] = bc[k] + sum_f Wc[k,f] keep(b,f,d',hw) X[b,f,d',hw] / (1-p)

@@ -129,6 +129,8 @@ _PROTOS = {
     "sx_head_dropout_bwd": [C.POINTER(sx_head_dropout_args), _P, _P, _I, _P, _P],
     "sx_token_scores": [_P, _P, _I, _I, _I, _I, _P, _P],
     "sx_token_scores_bwd": [_P, _P, _I, _I, _I, _I, _P, _P],
+    "sx_subpixel_resize_fwd": [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P],
+    "sx_subpixel_resize_bwd": [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P],
     "sx_resize_axis_fwd": [_P, _L, _I, _I, _L, _P, _I, _P],
     "sx_resize_axis_bwd": [_P, _L, _I, _I, _L, _P, _P],
     "sx_resize_tokens_fwd": [_P, _L, _L, _L, _P, _L, _L, _L, _I, _I, _I, _I, C.POINTER(sx_resample_grid), _I, _P],

@@ -357,22 +357,24 @@ __global__ void resize_last_x2_bwd_kernel(const float* __restrict__ dy, unsigned
 }
 
 // ---- class scores of the fused tokens, exact fp32: out[b,k,n] = sum_f W[k,f] vf[b,n,f]; one warp per token ----
-template <bool V4>
+// KMAX: rows handled per pass (8 for the class rows of the collapsed head; 16 / 32 for the 4 sub-pixel rows per class
+// of the direct head), so a token row is read once for all of them
+template <bool V4, int KMAX>
 __global__ void token_scores_kernel(const float* __restrict__ vf, const float* __restrict__ W, long long T, int N,
                                     int F, int K, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   const long long t = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (t >= T) return;
   const float* x = vf + t * F;
-  float acc[MAXK];
+  float acc[KMAX];
 #pragma unroll
-  for (int k = 0; k < MAXK; ++k) acc[k] = 0.f;
+  for (int k = 0; k < KMAX; ++k) acc[k] = 0.f;
   if (V4) {                                 // F % 4 == 0, 16-byte aligned rows: 4 x 512 B of the token row in flight
 #pragma unroll 4
     for (int f = lane * 4; f < F; f += 128) {
       const float4 xv = *reinterpret_cast<const float4*>(x + f);
 #pragma unroll
-      for (int k = 0; k < MAXK; ++k)
+      for (int k = 0; k < KMAX; ++k)
         if (k < K) {
           const float4 w = __ldg(reinterpret_cast<const float4*>(W + (long long)k * F + f));
           acc[k] = fmaf(xv.x, w.x, fmaf(xv.y, w.y, fmaf(xv.z, w.z, fmaf(xv.w, w.w, acc[k]))));
@@ -382,13 +384,13 @@ __global__ void token_scores_kernel(const float* __restrict__ vf, const float* _
     for (int f = lane; f < F; f += 32) {
       const float xv = x[f];
 #pragma unroll
-      for (int k = 0; k < MAXK; ++k)
+      for (int k = 0; k < KMAX; ++k)
         if (k < K) acc[k] = fmaf(xv, __ldg(W + (long long)k * F + f), acc[k]);
     }
   }
   const long long b = t / N, n = t % N;
 #pragma unroll
-  for (int k = 0; k < MAXK; ++k)
+  for (int k = 0; k < KMAX; ++k)
     if (k < K) {
       const float s = sx::warp_sum(acc[k]);
       if (lane == 0) out[(b * K + k) * N + n] = s;
@@ -396,6 +398,7 @@ __global__ void token_scores_kernel(const float* __restrict__ vf, const float* _
 }
 
 // ---- its data gradient: dvf[b,n,f] = sum_k dt[b,k,n] W[k,f]; one thread per 4 channels, writes coalesced ----
+template <int KMAX>
 __global__ void token_scores_bwd_kernel(const float* __restrict__ dt, const float* __restrict__ W, long long T, int N,
                                         int F, int K, float* __restrict__ dvf) {
   const int F4 = F >> 2;
@@ -406,7 +409,7 @@ __global__ void token_scores_bwd_kernel(const float* __restrict__ dt, const floa
     const long long b = t / N, n = t - b * N;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-    for (int k = 0; k < MAXK; ++k)
+    for (int k = 0; k < KMAX; ++k)
       if (k < K) {
         const float d = __ldg(dt + (b * K + k) * N + n);
         const float4 w = __ldg(reinterpret_cast<const float4*>(W + (long long)k * F + f));
@@ -463,6 +466,90 @@ __global__ void sgemm_small_warp_kernel(const float* __restrict__ A, const float
   if (lane == 0) {
     float* c = C + z * scz + (long long)m * scm + (long long)n * scn;
     *c = accumulate ? *c + alpha * acc : alpha * acc;
+  }
+}
+
+// ---- direct class head (out_fpn_layers == in_fpn_layers): sub-pixel scores -> logits in their final layout ----
+// S [B][4K][N], row 4k + 2a + c = sub-pixel (a, c) of class k's 2x2 transposed-conv output, token n = d*H2*W2 + y*W2 + x.
+// The virtual grid V[b,k] (2H2, 2W2, D2) holds V[i,j,d] = S[b, 4k + 2(i%2) + j%2, d*H2*W2 + (i/2)*W2 + j/2]; the logits
+// [B][K][H][W][D] are its trilinear resampling to (H, W, D) (2-D: D2 = D = 1), plus bias[k].
+__device__ __forceinline__ long long subpixel_src(int i, int j, int d, int H2, int W2, long long N) {
+  return (long long)(((i & 1) << 1) | (j & 1)) * N + (long long)d * H2 * W2 + (long long)(i >> 1) * W2 + (j >> 1);
+}
+
+// one thread per logit; blockIdx.y = b*K + k; the innermost output axis is the fastest (coalesced writes)
+__global__ void subpixel_resize_fwd_kernel(const float* __restrict__ S, const float* __restrict__ bias, int K, int D2,
+                                           int H2, int W2, int H, int W, int D, float* __restrict__ out) {
+  const int bk = blockIdx.y, k = bk % K;
+  const long long N = (long long)D2 * H2 * W2;
+  const float* s = S + (long long)bk * 4 * N;
+  float* o = out + (long long)bk * H * W * D;
+  const float rh = (float)(2 * H2) / (float)H, rw = (float)(2 * W2) / (float)W, rd = (float)D2 / (float)D;
+  const float bv = bias ? bias[k] : 0.f;
+  const unsigned total = (unsigned)H * W * D;
+  for (unsigned idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
+    const int dd = (int)(idx % (unsigned)D);
+    const unsigned t = idx / (unsigned)D;
+    const int w = (int)(t % (unsigned)W), h = (int)(t / (unsigned)W);
+    int i0, i1, j0, j1, d0, d1;
+    float ti, tj, td;
+    sx::src_index(h, rh, 2 * H2, i0, i1, ti);
+    sx::src_index(w, rw, 2 * W2, j0, j1, tj);
+    sx::src_index(dd, rd, D2, d0, d1, td);
+    auto g = [&](int i, int j) {
+      return (1.f - td) * __ldg(s + subpixel_src(i, j, d0, H2, W2, N)) + td * __ldg(s + subpixel_src(i, j, d1, H2, W2, N));
+    };
+    const float v = (1.f - ti) * ((1.f - tj) * g(i0, j0) + tj * g(i0, j1)) + ti * ((1.f - tj) * g(i1, j0) + tj * g(i1, j1));
+    o[idx] = v + bv;
+  }
+}
+
+// weight of input cell i in output cell j of a 1-D linear resampling (both taps may be i at a clamped edge)
+__device__ __forceinline__ float tap_weight(int j, float ratio, int Lin, int i) {
+  int i0, i1;
+  float w1;
+  sx::src_index(j, ratio, Lin, i0, i1, w1);
+  return (i0 == i ? 1.f - w1 : 0.f) + (i1 == i ? w1 : 0.f);
+}
+
+// adjoint in gather form: one thread per virtual cell (i, j, d), d fastest; dS[b, 4k + s, n] = sum over the logits that
+// read the cell of weight * dout, in a fixed order (no atomics)
+__global__ void subpixel_resize_bwd_kernel(const float* __restrict__ dout, int D2, int H2, int W2, int H, int W, int D,
+                                           float* __restrict__ dS) {
+  const int bk = blockIdx.y;
+  const long long N = (long long)D2 * H2 * W2;
+  const float* g = dout + (long long)bk * H * W * D;
+  float* ds = dS + (long long)bk * 4 * N;
+  const int Li = 2 * H2, Lj = 2 * W2;
+  const float rh = (float)Li / (float)H, rw = (float)Lj / (float)W, rd = (float)D2 / (float)D;
+  const unsigned total = (unsigned)Li * Lj * D2;
+  for (unsigned idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
+    const int d = (int)(idx % (unsigned)D2);
+    const unsigned t = idx / (unsigned)D2;
+    const int j = (int)(t % (unsigned)Lj), i = (int)(t / (unsigned)Lj);
+    int hlo, hhi, wlo, whi, dlo, dhi;
+    sx::src_readers(i, (float)H / (float)Li, Li, H, hlo, hhi);
+    sx::src_readers(j, (float)W / (float)Lj, Lj, W, wlo, whi);
+    sx::src_readers(d, (float)D / (float)D2, D2, D, dlo, dhi);
+    float acc = 0.f;
+    for (int h = hlo; h <= hhi; ++h) {
+      const float wh = tap_weight(h, rh, Li, i);
+      if (wh == 0.f) continue;
+      float acc_h = 0.f;
+      for (int w = wlo; w <= whi; ++w) {
+        const float ww = tap_weight(w, rw, Lj, j);
+        if (ww == 0.f) continue;
+        const float* row = g + ((long long)h * W + w) * D;
+        float acc_w = 0.f;
+        for (int dd = dlo; dd <= dhi; ++dd) {
+          const float wd = tap_weight(dd, rd, D2, d);
+          if (wd != 0.f) acc_w = fmaf(wd, __ldg(row + dd), acc_w);
+        }
+        acc_h = fmaf(ww, acc_w, acc_h);
+      }
+      acc = fmaf(wh, acc_h, acc);
+    }
+    ds[subpixel_src(i, j, d, H2, W2, N)] = acc;
   }
 }
 
@@ -609,14 +696,29 @@ extern "C" int sx_sgemm_small(const float* A, const float* B, float* C, int32_t 
   return 0;
 }
 
+// rows per pass of the token-score kernels: the collapsed head's class rows (<= 8, unchanged), or the direct head's
+// 4 sub-pixel rows per class (<= 32)
+constexpr int MAXROWS = 32;
+
+template <int KMAX>
+static void token_scores_launch(const float* vf, const float* W, long long T, int N, int F, int K, float* out,
+                                cudaStream_t st) {
+  if (F % 4 == 0 && (reinterpret_cast<uintptr_t>(vf) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0)
+    token_scores_kernel<true, KMAX><<<sx_ceil_div(T, 8), 256, 0, st>>>(vf, W, T, N, F, K, out);
+  else
+    token_scores_kernel<false, KMAX><<<sx_ceil_div(T, 8), 256, 0, st>>>(vf, W, T, N, F, K, out);
+}
+
 extern "C" int sx_token_scores(const float* vf, const float* W, int32_t B, int32_t N, int32_t F, int32_t K, float* out,
                                void* stream) {
-  SX_REQUIRE(K >= 1 && K <= MAXK, "sx_token_scores: num_classes %d not in 1..%d", K, MAXK);
+  SX_REQUIRE(K >= 1 && K <= MAXROWS, "sx_token_scores: rows %d not in 1..%d", K, MAXROWS);
   const long long T = (long long)B * N;
-  if (F % 4 == 0 && (reinterpret_cast<uintptr_t>(vf) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0)
-    token_scores_kernel<true><<<sx_ceil_div(T, 8), 256, 0, ST(stream)>>>(vf, W, T, N, F, K, out);
+  if (K <= MAXK)
+    token_scores_launch<MAXK>(vf, W, T, N, F, K, out, ST(stream));
+  else if (K <= 16)
+    token_scores_launch<16>(vf, W, T, N, F, K, out, ST(stream));
   else
-    token_scores_kernel<false><<<sx_ceil_div(T, 8), 256, 0, ST(stream)>>>(vf, W, T, N, F, K, out);
+    token_scores_launch<MAXROWS>(vf, W, T, N, F, K, out, ST(stream));
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -624,12 +726,42 @@ extern "C" int sx_token_scores(const float* vf, const float* W, int32_t B, int32
 extern "C" int sx_token_scores_bwd(const float* dt, const float* W, int32_t B, int32_t N, int32_t F, int32_t K, float* dvf,
                                    void* stream) {
   SX_REQUIRE(dt && W && dvf && B >= 1 && N >= 1 && F >= 1, "sx_token_scores_bwd: bad arguments");
-  SX_REQUIRE(K >= 1 && K <= MAXK, "sx_token_scores_bwd: num_classes %d not in 1..%d", K, MAXK);
+  SX_REQUIRE(K >= 1 && K <= MAXROWS, "sx_token_scores_bwd: rows %d not in 1..%d", K, MAXROWS);
   SX_REQUIRE(F % 4 == 0 && (reinterpret_cast<uintptr_t>(dvf) & 15) == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0,
              "sx_token_scores_bwd: F must be a multiple of 4 and W/dvf 16-byte aligned");
   const long long T = (long long)B * N, total = T * (F / 4);
   const int grid = (int)std::min<long long>(sx_ceil_div(total, 256), sm_count_cached() * 16ll);
-  token_scores_bwd_kernel<<<grid, 256, 0, ST(stream)>>>(dt, W, T, N, F, K, dvf);
+  if (K <= MAXK)
+    token_scores_bwd_kernel<MAXK><<<grid, 256, 0, ST(stream)>>>(dt, W, T, N, F, K, dvf);
+  else if (K <= 16)
+    token_scores_bwd_kernel<16><<<grid, 256, 0, ST(stream)>>>(dt, W, T, N, F, K, dvf);
+  else
+    token_scores_bwd_kernel<MAXROWS><<<grid, 256, 0, ST(stream)>>>(dt, W, T, N, F, K, dvf);
+  SX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+static bool subpixel_shape_ok(int32_t B, int32_t K, int32_t D2, int32_t H2, int32_t W2, int32_t H, int32_t W, int32_t D) {
+  return B >= 1 && K >= 1 && (long long)B * K <= 65535 && D2 >= 1 && H2 >= 1 && W2 >= 1 && H >= 1 && W >= 1 && D >= 1 &&
+         (long long)H * W * D < (1ll << 31) && 4ll * H2 * W2 * D2 < (1ll << 31);
+}
+
+extern "C" int sx_subpixel_resize_fwd(const float* S, const float* bias, int32_t B, int32_t K, int32_t D2, int32_t H2,
+                                      int32_t W2, int32_t H, int32_t W, int32_t D, float* out, void* stream) {
+  SX_REQUIRE(S && out && subpixel_shape_ok(B, K, D2, H2, W2, H, W, D), "sx_subpixel_resize_fwd: bad arguments");
+  const long long per = (long long)H * W * D;
+  const int gx = (int)std::max<long long>(1, std::min<long long>(sx_ceil_div(per, 256),
+                                                                 sm_count_cached() * 16ll / (B * K) + 1));
+  subpixel_resize_fwd_kernel<<<dim3(gx, B * K), 256, 0, ST(stream)>>>(S, bias, K, D2, H2, W2, H, W, D, out);
+  SX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int sx_subpixel_resize_bwd(const float* dout, int32_t B, int32_t K, int32_t D2, int32_t H2, int32_t W2,
+                                      int32_t H, int32_t W, int32_t D, float* dS, void* stream) {
+  SX_REQUIRE(dout && dS && subpixel_shape_ok(B, K, D2, H2, W2, H, W, D), "sx_subpixel_resize_bwd: bad arguments");
+  const long long cells = 4ll * H2 * W2 * D2;
+  subpixel_resize_bwd_kernel<<<dim3(sx_ceil_div(cells, 128), B * K), 128, 0, ST(stream)>>>(dout, D2, H2, W2, H, W, D, dS);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

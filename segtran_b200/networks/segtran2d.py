@@ -2,7 +2,8 @@
 
 Backbone (ResNet / EfficientNet) and the in-/out-FPN pyramids stay stock PyTorch/cuDNN (out of the hot path);
 token flatten, the Squeeze-and-Expansion stack and the pixel-wise head (collapsed form; with --outdrop in training, the
-dropout head of csrc/sx_head_drop.cu) run on segtran_b200 kernels.
+dropout head of csrc/sx_head_drop.cu; with out_fpn_layers == in_fpn_layers, the direct ConvTranspose2d head of
+ops.direct_head) run on segtran_b200 kernels.
 The backbone is the reference's own class when this package is dropped into the reference tree
 (``resnet`` / ``efficientnet.model`` importable), or any module passed as ``backbone=``.
 """
@@ -131,26 +132,30 @@ class Segtran2d(SegtranInitWeights):
         self.out_fpn_use_bn, self.out_fpn_layers, self.out_fpn_scheme = \
             config.out_fpn_use_bn, config.out_fpn_layers, config.out_fpn_scheme
         self.out_fpn_do_dropout = config.out_fpn_do_dropout
-        if self.out_fpn_layers == self.in_fpn_layers:
-            raise NotImplementedError("segtran_b200: out_fpn_layers == in_fpn_layers (ConvTranspose2d head) is not "
-                                      "implemented; the drivers use in='34', out='1234'")
-        self.do_out_fpn = True
-        self.out_fpn12_conv = nn.Conv2d(d[1], d[2], 1)
-        self.out_fpn23_conv = nn.Conv2d(d[2], d[3], 1)
-        self.out_fpn34_conv = nn.Conv2d(d[3], d[4], 1)
-        last_out = self.out_fpn_layers[-len(self.in_fpn_layers)]
-        self.out_fpn_bridgeconv = nn.Conv2d(d[last_out], self.trans_out_dim, 1) if d[last_out] != self.trans_out_dim \
-            else nn.Identity()
-        if self.out_fpn_use_bn:
-            self.out_bn2b, self.out_bn3b, self.out_bn4b = nn.BatchNorm2d(d[2]), nn.BatchNorm2d(d[3]), nn.BatchNorm2d(d[4])
-            self.out_fpn_norms = [None, None, self.out_bn2b, self.out_bn3b, self.out_bn4b]
+        self.do_out_fpn = self.out_fpn_layers != self.in_fpn_layers
+        if self.do_out_fpn:
+            self.out_fpn12_conv = nn.Conv2d(d[1], d[2], 1)
+            self.out_fpn23_conv = nn.Conv2d(d[2], d[3], 1)
+            self.out_fpn34_conv = nn.Conv2d(d[3], d[4], 1)
+            last_out = self.out_fpn_layers[-len(self.in_fpn_layers)]
+            self.out_fpn_bridgeconv = nn.Conv2d(d[last_out], self.trans_out_dim, 1) \
+                if d[last_out] != self.trans_out_dim else nn.Identity()
+            if self.out_fpn_use_bn:
+                self.out_bn2b, self.out_bn3b, self.out_bn4b = \
+                    nn.BatchNorm2d(d[2]), nn.BatchNorm2d(d[3]), nn.BatchNorm2d(d[4])
+                self.out_fpn_norms = [None, None, self.out_bn2b, self.out_bn3b, self.out_bn4b]
+            else:
+                self.out_gn2b, self.out_gn3b, self.out_gn4b = \
+                    nn.GroupNorm(self.G, d[2]), nn.GroupNorm(self.G, d[3]), nn.GroupNorm(self.G, d[4])
+                self.out_fpn_norms = [None, None, self.out_gn2b, self.out_gn3b, self.out_gn4b]
+            self.out_fpn_convs = [None, self.out_fpn12_conv, self.out_fpn23_conv, self.out_fpn34_conv]
+            self.out_conv = nn.Conv2d(self.trans_out_dim, self.num_classes, 1)
+            self.out_fpn_dropout = nn.Dropout(config.hidden_dropout_prob)
         else:
-            self.out_gn2b, self.out_gn3b, self.out_gn4b = \
-                nn.GroupNorm(self.G, d[2]), nn.GroupNorm(self.G, d[3]), nn.GroupNorm(self.G, d[4])
-            self.out_fpn_norms = [None, None, self.out_gn2b, self.out_gn3b, self.out_gn4b]
-        self.out_fpn_convs = [None, self.out_fpn12_conv, self.out_fpn23_conv, self.out_fpn34_conv]
-        self.out_conv = nn.Conv2d(self.trans_out_dim, self.num_classes, 1)
-        self.out_fpn_dropout = nn.Dropout(config.hidden_dropout_prob)
+            # Class scores straight from the tokens.  The reference's 1x1-conv branch for in_fpn_layers '234' tests
+            # `'2' in self.in_fpn_layers` on a list of ints, which is never true, so '234' also gets the transposed conv
+            # (doubling a grid that is already at 1/4 resolution); that is reproduced here.  --outdrop has no map to drop.
+            self.out_conv = nn.ConvTranspose2d(self.trans_out_dim, self.num_classes, 2, 2)
 
         self.apply(self.init_weights)
         self.apply(self.tie_qk)
@@ -202,7 +207,8 @@ class Segtran2d(SegtranInitWeights):
     def hot_path(self, feat_fpn, curr_feat, vmask, out_size, B0=None, MOD=0):
         """The CUDA segment: token flatten -> Squeeze-and-Expansion stack -> scatter -> collapsed pixel-wise head
         (reference segtran2d.py:264-269, :362-436 minus the FPN pyramids).
-        feat_fpn [B,C0,H2,W2], curr_feat [B,Cf,H1,W1], vmask [B,N] or None, out_size = (H,W) -> logits."""
+        feat_fpn [B,C0,H2,W2], curr_feat [B,Cf,H1,W1] (ignored, may be None, without the out-FPN), vmask [B,N] or None,
+        out_size = (H,W) -> logits."""
         B, C0, H2, W2 = feat_fpn.shape
         B0 = B if B0 is None else B0
         H, W = out_size
@@ -223,7 +229,10 @@ class Segtran2d(SegtranInitWeights):
             self._pos_cache_key, self._pos_cache = key, idx
         voxels_pos = self._pos_cache.unsqueeze(0).expand(B0, -1, -1)
         fused = self.voxel_fusion(vfeat, voxels_pos, None if vmask is None else vmask.unsqueeze(2), grid)
-        ops.grad_ready(fused, list(self.out_fpn_bridgeconv.parameters()) + list(self.out_conv.parameters()))   # backward past the head
+        head_params = list(self.out_conv.parameters())
+        if self.do_out_fpn:
+            head_params += list(self.out_fpn_bridgeconv.parameters())
+        ops.grad_ready(fused, head_params)                            # backward past the head
         self.layers_attn_scores = self.voxel_fusion.layers_attn_scores
         for i in range(self.num_translayers):
             self.feature_maps.append(self.voxel_fusion.translayers[i].attention_scores)
@@ -231,6 +240,8 @@ class Segtran2d(SegtranInitWeights):
             lv = self.voxel_fusion.layers_vfeat[i]
             self.feature_maps.append(lv.detach().view(B0, H2, W2, self.translayer_dims[i + 1]).permute(0, 3, 1, 2))
         self.orig_feat_shape = grid
+        if not self.do_out_fpn:                               # ConvTranspose2d + bilinear: the direct head (curr_feat unused)
+            return ops.direct_head(fused, tuple(grid), self.out_conv.weight, self.out_conv.bias, (H, W))
         bridge = self.out_fpn_bridgeconv
         Wb, bb = (bridge.weight, bridge.bias) if isinstance(bridge, nn.Conv2d) else (None, None)
         if self.out_fpn_do_dropout and self.training:         # per-channel mask: the dropout head (sx_head_drop.cu)
@@ -256,7 +267,9 @@ class Segtran2d(SegtranInitWeights):
         else:
             feat_fpn = bc(cur)
         self.feature_maps.append(feat_fpn)
-        layers = self.out_fpn_layers[:-len(self.in_fpn_layers)]
-        curr_feat = self._pyramid(feats, layers, self.out_fpn_convs, self.out_fpn_norms, self.out_fpn_scheme,
-                                  self.out_fpn_layers[0])
+        curr_feat = None
+        if self.do_out_fpn:
+            layers = self.out_fpn_layers[:-len(self.in_fpn_layers)]
+            curr_feat = self._pyramid(feats, layers, self.out_fpn_convs, self.out_fpn_norms, self.out_fpn_scheme,
+                                      self.out_fpn_layers[0])
         return self.hot_path(feat_fpn, curr_feat, nonzero_mask.reshape(B, -1), (H, W), B0, MOD)

@@ -10,6 +10,8 @@ What runs where
     own parameters (checkpoint compatible) but are applied as one class-dimension contraction.  ``--upd conv``
     (``out_fpn_upsampleD``) is linear too and is folded into the class conv in weight space.  ``--outdrop`` in training
     runs the dropout head (csrc/sx_head_drop.cu), which never writes the dropped full-resolution map.
+    With out_fpn_layers == in_fpn_layers there is no out-FPN: ``out_conv3d`` is a ConvTranspose3d on the tokens, run
+    with the trilinear interpolation as ``ops.direct_head``.
 """
 from __future__ import annotations
 
@@ -157,32 +159,36 @@ class Segtran3d(SegtranInitWeights):
         self.out_fpn_use_bn, self.out_fpn_layers, self.out_fpn_scheme = \
             config.out_fpn_use_bn, config.out_fpn_layers, config.out_fpn_scheme
         self.out_fpn_do_dropout = config.out_fpn_do_dropout
-        if self.out_fpn_layers == self.in_fpn_layers:
-            raise NotImplementedError("segtran_b200: out_fpn_layers == in_fpn_layers (ConvTranspose3d head) is not "
-                                      "implemented; the drivers use in='34', out='1234'")
-        self.do_out_fpn = True
-        last_out = self.out_fpn_layers[-len(self.in_fpn_layers)]
-        self.out_fpn_out_dim = self.trans_out_dim
-        self.out_fpn12_conv3d = nn.Conv3d(d[1], d[2], 1)
-        self.out_fpn23_conv3d = nn.Conv3d(d[2], d[3], 1)
-        self.out_fpn34_conv3d = nn.Conv3d(d[3], d[4], 1)
-        self.out_fpn_bridgeconv3d = nn.Conv3d(d[last_out], self.trans_out_dim, 1)
-        if self.out_fpn_upsampleD_scheme == 'conv':
-            # created here, before the norms, as the reference does: seeded construction draws the same weights
-            self.out_feat_dim = self.out_fpn_out_dim // self.D_pool_K
-            self.out_fpn_upsampleD = nn.Conv3d(self.out_fpn_out_dim, self.out_feat_dim * self.D_pool_K, 1)
+        self.do_out_fpn = self.out_fpn_layers != self.in_fpn_layers
+        if self.do_out_fpn:
+            last_out = self.out_fpn_layers[-len(self.in_fpn_layers)]
+            self.out_fpn_out_dim = self.trans_out_dim
+            self.out_fpn12_conv3d = nn.Conv3d(d[1], d[2], 1)
+            self.out_fpn23_conv3d = nn.Conv3d(d[2], d[3], 1)
+            self.out_fpn34_conv3d = nn.Conv3d(d[3], d[4], 1)
+            self.out_fpn_bridgeconv3d = nn.Conv3d(d[last_out], self.trans_out_dim, 1)
+            if self.out_fpn_upsampleD_scheme == 'conv':
+                # created here, before the norms, as the reference does: seeded construction draws the same weights
+                self.out_feat_dim = self.out_fpn_out_dim // self.D_pool_K
+                self.out_fpn_upsampleD = nn.Conv3d(self.out_fpn_out_dim, self.out_feat_dim * self.D_pool_K, 1)
+            else:
+                self.out_feat_dim = self.out_fpn_out_dim
+            if self.out_fpn_use_bn:
+                self.out_bn2b, self.out_bn3b, self.out_bn4b = \
+                    nn.BatchNorm3d(d[2]), nn.BatchNorm3d(d[3]), nn.BatchNorm3d(d[4])
+                self.out_fpn_norms = [None, None, self.out_bn2b, self.out_bn3b, self.out_bn4b]
+            else:
+                self.out_gn2b, self.out_gn3b, self.out_gn4b = \
+                    nn.GroupNorm(self.G, d[2]), nn.GroupNorm(self.G, d[3]), nn.GroupNorm(self.G, d[4])
+                self.out_fpn_norms = [None, None, self.out_gn2b, self.out_gn3b, self.out_gn4b]
+            self.out_fpn_convs = [None, self.out_fpn12_conv3d, self.out_fpn23_conv3d, self.out_fpn34_conv3d]
+            self.out_conv3d = nn.Conv3d(self.out_feat_dim, self.num_classes, 1)
+            self.out_fpn_dropout = nn.Dropout(config.hidden_dropout_prob)
         else:
-            self.out_feat_dim = self.out_fpn_out_dim
-        if self.out_fpn_use_bn:
-            self.out_bn2b, self.out_bn3b, self.out_bn4b = nn.BatchNorm3d(d[2]), nn.BatchNorm3d(d[3]), nn.BatchNorm3d(d[4])
-            self.out_fpn_norms = [None, None, self.out_bn2b, self.out_bn3b, self.out_bn4b]
-        else:
-            self.out_gn2b, self.out_gn3b, self.out_gn4b = \
-                nn.GroupNorm(self.G, d[2]), nn.GroupNorm(self.G, d[3]), nn.GroupNorm(self.G, d[4])
-            self.out_fpn_norms = [None, None, self.out_gn2b, self.out_gn3b, self.out_gn4b]
-        self.out_fpn_convs = [None, self.out_fpn12_conv3d, self.out_fpn23_conv3d, self.out_fpn34_conv3d]
-        self.out_conv3d = nn.Conv3d(self.out_feat_dim, self.num_classes, 1)
-        self.out_fpn_dropout = nn.Dropout(config.hidden_dropout_prob)
+            # Class scores straight from the tokens, as the 2-D shell does: ConvTranspose3d (2,2,1) on the (H,W,D)-permuted
+            # tokens (the reference's 1x1x1-conv branch for '234' is never taken, see segtran2d).  --upd conv and --outdrop
+            # have no out-FPN map to act on.
+            self.out_conv3d = nn.ConvTranspose3d(self.trans_out_dim, self.num_classes, (2, 2, 1), (2, 2, 1))
 
         self.apply(self.init_weights)
         self.apply(self.tie_qk)
@@ -248,7 +254,8 @@ class Segtran3d(SegtranInitWeights):
     def hot_path(self, feat_fpn, curr_feat, vmask, out_size):
         """The CUDA segment of the forward: token flatten -> Squeeze-and-Expansion stack -> scatter -> collapsed
         voxel-wise head (reference segtran3d.py:326-332, :442-498 minus the FPN pyramids).
-        feat_fpn [B,C0,D2,H2,W2], curr_feat [B,Cf,D1,H1,W1], vmask [B,N] or None, out_size = (H,W,D) -> logits."""
+        feat_fpn [B,C0,D2,H2,W2], curr_feat [B,Cf,D1,H1,W1] (ignored, may be None, without the out-FPN), vmask [B,N] or
+        None, out_size = (H,W,D) -> logits."""
         B, C0, D2, H2, W2 = feat_fpn.shape
         H, W, D = out_size
         grid = torch.Size((D2, H2, W2))
@@ -268,12 +275,16 @@ class Segtran3d(SegtranInitWeights):
             self._pos_cache_key, self._pos_cache = key, idx
         voxels_pos = self._pos_cache.unsqueeze(0).expand(B, -1, -1)  # one set of positions, shared by the batch
         fused = self.voxel_fusion(vfeat, voxels_pos, None if vmask is None else vmask.unsqueeze(2), grid)
-        head_params = list(self.out_fpn_bridgeconv3d.parameters()) + list(self.out_conv3d.parameters())
-        if self.out_fpn_upsampleD_scheme == 'conv':
+        head_params = list(self.out_conv3d.parameters())
+        if self.do_out_fpn:
+            head_params += list(self.out_fpn_bridgeconv3d.parameters())
+        if self.do_out_fpn and self.out_fpn_upsampleD_scheme == 'conv':
             head_params += list(self.out_fpn_upsampleD.parameters())
         ops.grad_ready(fused, head_params)                            # backward past the head
         self.layers_attn_scores = self.voxel_fusion.layers_attn_scores
         self.orig_feat_shape = grid
+        if not self.do_out_fpn:                 # ConvTranspose3d + trilinear: the direct head (curr_feat unused)
+            return ops.direct_head(fused, tuple(grid), self.out_conv3d.weight, self.out_conv3d.bias, out_size)
         bridge, cls = self.out_fpn_bridgeconv3d, self.out_conv3d
         # the depth upsampling runs only when D_pool_K > 1 (reference segtran3d.py:372)
         unfold = self.D_pool_K > 1 and self.out_fpn_upsampleD_scheme == 'conv'
@@ -307,5 +318,5 @@ class Segtran3d(SegtranInitWeights):
         f = self.backbone.extract_features(x)
         feats = tuple(f[k] for k in _I3D_KEYS)
         feat_fpn, vmask = self.in_fpn_forward(feats, nonzero_mask)
-        curr_feat = self.out_fpn_pyramid(feats)
+        curr_feat = self.out_fpn_pyramid(feats) if self.do_out_fpn else None
         return self.hot_path(feat_fpn, curr_feat, vmask, (H, W, D))

@@ -2043,6 +2043,48 @@ def seg_head(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, d_pool_k=1, perm
     return _head_out(Lo, out_size)
 
 
+class _SubpixelResize(torch.autograd.Function):
+    """Logits of the direct head from its sub-pixel scores S [B,4K,N] (csrc/sx_head.cu): the 2x2(x1) transposed conv's
+    output grid is never written; bi/trilinear interpolation reads S directly and writes [B,K,H,W] / [B,K,H,W,D]."""
+
+    @staticmethod
+    def forward(ctx, S, bias, grid, out_size):
+        S = S.contiguous()
+        B, K4, N = S.shape
+        K = K4 // 4
+        (D2, H2, W2), (H, W, D) = (grid, out_size) if len(grid) == 3 else ((1,) + grid, tuple(out_size) + (1,))
+        out = torch.empty((B, K) + tuple(out_size), device=S.device, dtype=torch.float32)
+        L.call("sx_subpixel_resize_fwd", S.data_ptr(), _ptr(bias), B, K, D2, H2, W2, H, W, D, out.data_ptr(), _stream())
+        ctx.meta = (B, K, N, D2, H2, W2, H, W, D, bias is not None)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        B, K, N, D2, H2, W2, H, W, D, has_bias = ctx.meta
+        dout = dout.contiguous()
+        dS = torch.empty((B, 4 * K, N), device=dout.device, dtype=torch.float32)
+        L.call("sx_subpixel_resize_bwd", dout.data_ptr(), B, K, D2, H2, W2, H, W, D, dS.data_ptr(), _stream())
+        db = None
+        if has_bias and ctx.needs_input_grad[1]:       # sum of the logit gradients of class k = sum of its rows of dS
+            db = _zeros((K,), dout.device)
+            L.call("sx_rowsum", dS.data_ptr(), B * K, 4 * N, 4 * N, K, db.data_ptr(), *_part_args(dout.device), _stream())
+        return dS, db, None, None
+
+
+def direct_head(fused, grid, Wt, bt, out_size):
+    """Class head without the out-FPN (out_fpn_layers == in_fpn_layers; segtran2d.py:198-209, :421-437, segtran3d.py:
+    234-245, :478-498): ConvTranspose2d(C, K, 2, 2) / ConvTranspose3d(C, K, (2,2,1), (2,2,1)) of the fused tokens, then
+    bi/trilinear interpolation (align_corners=False) to out_size.
+    fused [B,N,C] tokens on `grid` ((H2,W2), or (D2,H2,W2) in the reference's token order); Wt [C,K,2,2] / [C,K,2,2,1];
+    bt [K] or None; out_size (H,W) / (H,W,D) -> logits [B,K,H,W] / [B,K,H,W,D].
+    The 4K sub-pixel scores are one exact fp32 contraction of the tokens (sx_token_scores, K <= 8), and the logits come
+    from them in one pass (sx_subpixel_resize_fwd)."""
+    C, K = Wt.shape[0], Wt.shape[1]
+    W2 = transpose(Wt.reshape(1, C, 4 * K)).view(4 * K, C)          # row 4k + 2a + c = tap (a, c) of class k
+    S = _TokenClassScores.apply(fused, W2)
+    return _SubpixelResize.apply(S, bt, tuple(int(g) for g in grid), tuple(int(s) for s in out_size))
+
+
 class _HeadDropout(torch.autograd.Function):
     """Class scores of the dropped out-FPN map (csrc/sx_head_drop.cu), the map itself never written:
         Ls[b,k,d',hw] = bc[k] + sum_f Wc[k,f] keep(b,f,d',hw) X[b,f,d',hw] / (1-p)
