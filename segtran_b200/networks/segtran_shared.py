@@ -300,7 +300,7 @@ class ExpandedFeatTrans(nn.Module):
 
     def supports_fused_attention(self):
         """The expansion block whose P.V / mid / output chain is one autograd node (ops.attn_pv_gelu_group_linear), which
-        ops.squeeze_out_fused feeds with the fused attention probabilities."""
+        CrossAttFeatTrans feeds with the fused attention probabilities (ops.attn_probs)."""
         return self.has_FFN and isinstance(self.output, MMPrivateOutput) and isinstance(self.intermediate, MMSharedMid)
 
     def _value_bank(self, input_feat, tag="big"):
@@ -319,20 +319,6 @@ class ExpandedFeatTrans(nn.Module):
         f2s = self.feat_softaggr.feat2score
         return ops.ln_softaggr(y, ln.weight, ln.bias, f2s.weight, f2s.bias, drop_p=p,
                                seed=ops.new_dropout_seed(y.device) if p > 0 else 0)
-
-    def forward_from_qk(self, input_feat, q, k, clip, att_p, diag, posbias=None):
-        """Fused attention entry: q [Bq,U1,M*d], k [B,U2,M*d] (projected, TF32-rounded) instead of the probabilities —
-        scores, clamp, positional bias, softmax and attention dropout run in one kernel (csrc/sx_attn.cu), whose
-        probabilities ops.squeeze_out_fused hands to the P.V' / mid / output node."""
-        mid = self.intermediate
-        vp = self._value_bank(input_feat, ops.small_tag(input_feat.shape[1], q.shape[1]))
-        p = mid.dropout.p if self.training else 0.0
-        gl = self.output.group_linear
-        dev = vp.device
-        y = ops.squeeze_out_fused(q, k, vp, self.num_modes, clip, att_p, ops.new_dropout_seed(dev) if att_p > 0 else 0,
-                                  mid.shared_linear.bias, p, ops.new_dropout_seed(dev) if p > 0 else 0, gl.weight, gl.bias,
-                                  diag, posbias)
-        return self._norm_aggregate(y)
 
     def _mince_fuse(self, input_feat, probs, grid):
         """(:413-443) U [B,M,N,F]: V = first_linear(x) in full; per scale s its channel window [Lv_s, Rv_s) of every mode
@@ -469,15 +455,6 @@ class MultiHeadFeatTrans(nn.Module):
     def supports_fused_attention(self):
         return True
 
-    def forward_from_qk(self, input_feat, q, k, clip, att_p, diag, posbias=None):
-        """Fused attention entry (the contract of ExpandedFeatTrans.forward_from_qk): the probabilities come from the
-        fused scores / clamp / positional-bias / softmax / dropout kernel (ops.attn_probs)."""
-        M = self.num_modes
-        d = q.shape[-1] // M
-        probs = ops.attn_probs(q, k, M, 1.0 / math.sqrt(d), clip, att_p,
-                               ops.new_dropout_seed(q.device) if att_p > 0 else 0, diag, posbias)
-        return self.forward(input_feat, probs)
-
     def forward(self, input_feat, attention_probs):
         """input_feat [B,U2,C]; attention_probs [B,M,U1,U2] -> [B,U1,F] (:228-253)."""
         v = ops.linear(input_feat, self.first_linear.weight, self.first_linear.bias, tag="proj")       # [B,U2,F]
@@ -495,6 +472,26 @@ class MultiHeadFeatTrans(nn.Module):
                            round_out=False)
         ln = out.resout_norm_layer
         return ops.layer_norm(z, ln.weight, ln.bias, round_out=False)
+
+
+def _new_diag(device):
+    """A layer's attention diagnostics, kept on the device: running max of the scores, clamped calls, rows where the
+    reference's lower clamp could have mattered."""
+    return torch.tensor([-3.0e38, 0.0, 0.0], device=device)
+
+
+def _attention_probs(q, k, M, clip, drop_p, diag, *, fused, posbias=None, alpha=None, row_bias=None, tag="big",
+                     kmajor_dq=False):
+    """P = dropout(softmax(clamp_if(alpha Q K^T [+ row_bias]) [+ posbias])) per mode -> (P, S, amax).
+    fused: one sx_attn_probs_fwd kernel (ops.attn_probs), S = amax = None; with kmajor_dq its backward's dQ = dS K reads
+    a K-major copy of the keys.  Otherwise the raw scores S (ops.attn_scores, their maximum tracked on the device in
+    amax), then ops.softmax."""
+    seed = ops.new_dropout_seed(q.device) if drop_p > 0 else 0
+    if fused:
+        return ops.attn_probs(q, k, M, alpha, clip, drop_p, seed, diag, posbias, kmajor_dq=kmajor_dq), None, None
+    amax = torch.full((1,), -3.0e38, device=q.device)
+    S = ops.attn_scores(q, k, M, amax, row_bias, tag, alpha)
+    return ops.softmax(S, amax, clip, drop_p, seed, diag, posbias), S, amax
 
 
 class CrossAttFeatTrans(nn.Module):
@@ -596,33 +593,25 @@ class CrossAttFeatTrans(nn.Module):
         k = ops.linear(in_key, self.key.weight, self.key.bias, tag=tk)
         dev = q.device
         if self._diag is None or self._diag.device != dev:
-            self._diag = torch.tensor([-3.0e38, 0.0, 0.0], device=dev)
+            self._diag = _new_diag(dev)
         p = self.att_dropout.p if self.training else 0.0
         diag_call = self.training and (self.call_count + 1) % self.attn_diag_cycles == 0     # prints avg-attn: needs S
-        if ops.attn_fusion_enabled() and not self.keep_attn_scores and not diag_call and q.is_cuda and \
-                self.attention_mode_dim % 4 == 0 and self.out_trans.supports_fused_attention():
-            # fused squeeze-out attention: scores / clamp / softmax / dropout inside one wgmma kernel
-            self.attention_scores = None
-            if self.training:
-                self.call_count += 1
-            return self.out_trans.forward_from_qk(in_key, q, k, float(self.attn_clip), p, self._diag, pb)
-        amax = torch.full((1,), -3.0e38, device=dev)
-        s = ops.attn_scores(q, k, M, amax)                                   # [B,M,U1,U2], max tracked on device
-        seed = ops.new_dropout_seed(dev) if p > 0 else 0
-        if pb is not None:
-            probs = ops.softmax_posbias(s, pb, amax, float(self.attn_clip), p, seed, self._diag)
-        else:
-            probs = ops.softmax(s, amax, float(self.attn_clip), p, seed, self._diag)
+        fused = ops.attn_fusion_enabled() and not self.keep_attn_scores and not diag_call and q.is_cuda and \
+            self.attention_mode_dim % 4 == 0 and self.out_trans.supports_fused_attention()
+        # the expansion block's dQ = dS K reads a K-major copy of the keys (the squeeze-out's attractor keys are small
+        # against dS); multi-head reads its keys in place (DESIGN §4.3)
+        probs, s, amax = _attention_probs(q, k, M, float(self.attn_clip), p, self._diag, fused=fused, posbias=pb,
+                                          kmajor_dq=isinstance(self.out_trans, ExpandedFeatTrans))
         # kept after the conditional clamp, as the reference keeps them (:578-598)
         self.attention_scores = ops.clamp_if(s, amax, float(self.attn_clip)) if self.keep_attn_scores else None
         if self.training:
             self.call_count += 1
-            if self.call_count % self.attn_diag_cycles == 0:
+            if self.call_count % self.attn_diag_cycles == 0:        # never on the fused path: diag_call above
                 with torch.no_grad():
                     avg = float(s.sum() / (s > 0).sum().clamp_min(1))
                 mx, cc = self._diag_values()
                 print("max-attn: {:.2f}, avg-attn: {:.2f}, clamp-count: {}".format(mx, avg, cc))
-                self._diag = torch.tensor([-3.0e38, 0.0, 0.0], device=dev)
+                self._diag = _new_diag(dev)
         return self.out_trans(in_key, probs)
 
 
@@ -729,7 +718,7 @@ class CrossMinceAttFeatTrans(nn.Module):
         ks = ops.resize_tokens(k, M, grid, grids, ratios, wins)
         dev = q.device
         if self._diag is None or self._diag[0].device != dev:
-            self._diag = [torch.tensor([-3.0e38, 0.0, 0.0], device=dev) for _ in range(self.num_scales)]
+            self._diag = [_new_diag(dev) for _ in range(self.num_scales)]
         p = self.att_dropout.p if self.training else 0.0
         alpha = 1.0 / math.sqrt(d)                                     # (:736) the full per-mode width
         self.call_count += 1
@@ -737,22 +726,15 @@ class CrossMinceAttFeatTrans(nn.Module):
         fused = ops.attn_fusion_enabled() and not diag_call and q.is_cuda
         probs = []
         for s in range(self.num_scales):
-            seed = ops.new_dropout_seed(dev) if p > 0 else 0
-            if fused:
-                probs.append(ops.attn_probs(qs[s], ks[s], M, alpha, float(self.attn_clip), p, seed, self._diag[s], pbs[s]))
-                continue
-            amax = torch.full((1,), -3.0e38, device=dev)
-            sc = ops.attn_scores(qs[s], ks[s], M, amax, alpha=alpha)   # [B,M,N_s,N_s], max tracked on device
-            if pbs[s] is not None:
-                probs.append(ops.softmax_posbias(sc, pbs[s], amax, float(self.attn_clip), p, seed, self._diag[s]))
-            else:
-                probs.append(ops.softmax(sc, amax, float(self.attn_clip), p, seed, self._diag[s]))
+            P, sc, _ = _attention_probs(qs[s], ks[s], M, float(self.attn_clip), p, self._diag[s], fused=fused,
+                                        posbias=pbs[s], alpha=alpha)  # [B,M,N_s,N_s]
+            probs.append(P)
             if diag_call:
                 with torch.no_grad():
                     avg = float(sc.sum() / (sc > 0).sum().clamp_min(1))
                 mx, cc, _ = self._diag_lists()
                 print("{} attn max: {:.2f}, avg: {:.2f}, clamp-count: {}".format(self.mince_scales[s], mx[s], avg, cc[s]))
-                self._diag[s] = torch.tensor([-3.0e38, 0.0, 0.0], device=dev)
+                self._diag[s] = _new_diag(dev)
         return self.out_trans(in_key, probs, grid)
 
 
@@ -797,11 +779,10 @@ class SqueezedAttFeatTrans(nn.Module):
             rb = ops.scale(ops.matvec(q1[0], t.key.bias), 1.0 / math.sqrt(C))
         dev = in_feat.device
         if t._diag is None or t._diag.device != dev:
-            t._diag = torch.tensor([-3.0e38, 0.0, 0.0], device=dev)
-        amax = torch.full((1,), -3.0e38, device=dev)
-        s = ops.attn_scores(qw, in_feat, 1, amax, rb, tag="insq")                      # [B,1,A,N]
+            t._diag = _new_diag(dev)
         p = t.att_dropout.p if t.training else 0.0
-        probs = ops.softmax(s, amax, float(t.attn_clip), p, ops.new_dropout_seed(dev) if p > 0 else 0, t._diag)
+        probs, s, amax = _attention_probs(qw, in_feat, 1, float(t.attn_clip), p, t._diag, fused=False, row_bias=rb,
+                                          tag="insq")                                  # [B,1,A,N]
         t.attention_scores = ops.clamp_if(s, amax, float(t.attn_clip)) if t.keep_attn_scores else None
         if t.training:
             t.call_count += 1

@@ -1147,17 +1147,6 @@ def _pb_args(posbias):
     return _posbias_table(posbias), (posbias.R, posbias.grid, posbias.w)
 
 
-def squeeze_out_fused(q, k, vp, M, clip, att_p, att_seed, bm, hid_p, hid_seed, Wo, bo, diag, posbias=None):
-    """Y[b,m] = dropout(gelu(P[b,m] V'[b,:,m] + bm)) Wo[m]^T + bo[m]  with  P = dropout(softmax(min(Q K^T/sqrt(d), clip)))
-    — CrossAttFeatTrans.forward (segtran_shared.py:566-605) + ExpandedFeatTrans up to MMPrivateOutput's Linear: the fused
-    probabilities (_AttnProbs: scores, softmax and dropout in sx_attn_probs_fwd) feed attn_pv_gelu_group_linear.  The
-    attractor keys are small against dS, so dQ = dS K reads a K-major copy of them (DESIGN §4.3 on the backward's form).
-    posbias (PosBias): sliding-window positional bias inside the softmax; its table receives a gradient."""
-    P = _AttnProbs.apply(q.contiguous(), k.contiguous(), M, 1.0 / math.sqrt(q.shape[-1] // M), float(clip), att_p,
-                         att_seed, diag, *_pb_args(posbias), True)
-    return attn_pv_gelu_group_linear(P, vp, M, bm, hid_p, hid_seed, Wo, bo)
-
-
 class _LayerNorm(torch.autograd.Function):
     """nn.LayerNorm(C, eps=1e-12, affine) over the last dim (first_norm_layer, segtran_shared.py:456)."""
 
@@ -1404,17 +1393,12 @@ def attn_scores(q, k, M, amax=None, row_bias=None, tag="big", alpha=None):
     return _AttnScores.apply(q, k, M, amax, row_bias, tag, alpha)
 
 
-def softmax(S, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None):
-    """diag: optional device float[2] updated in place: [0] = max(diag[0], *amax), [1] += (*amax > clip)."""
-    return _Softmax.apply(S, amax, clip, drop_p, seed, diag, None, None)
-
-
-def softmax_posbias(S, posbias, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None):
-    """softmax() with the sliding-window positional bias added after the clamp; S [B,M,N,N] with N = posbias.num_tokens."""
-    if S.shape[-1] != posbias.num_tokens or S.shape[-2] != posbias.num_tokens:
-        raise L.SxError("softmax_posbias: scores %s do not match the %s bias grid" % (tuple(S.shape), posbias.grid))
-    table, geom = _pb_args(posbias)
-    return _Softmax.apply(S, amax, clip, drop_p, seed, diag, table, geom)
+def softmax(S, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None):
+    """diag: optional device float[2] updated in place: [0] = max(diag[0], *amax), [1] += (*amax > clip).
+    posbias (PosBias): the sliding-window positional bias, added after the clamp; S [B,M,N,N] with N = posbias.num_tokens."""
+    if posbias is not None and (S.shape[-1] != posbias.num_tokens or S.shape[-2] != posbias.num_tokens):
+        raise L.SxError("softmax: scores %s do not match the %s bias grid" % (tuple(S.shape), posbias.grid))
+    return _Softmax.apply(S, amax, clip, drop_p, seed, diag, *_pb_args(posbias))
 
 
 def attn_pv(P, v, M, tag="big", round_out=True, heads=False):
@@ -1690,10 +1674,14 @@ class _AttnProbs(torch.autograd.Function):
         return dq, dk, None, None, None, None, None, None, dT, None, None
 
 
-def attn_probs(q, k, M, alpha, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None):
-    """Differentiable fused attention probabilities (see _AttnProbs); q, k [B, U, M*d] contiguous, TF32-rounded."""
+def attn_probs(q, k, M, alpha=None, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None, *, kmajor_dq=False):
+    """Differentiable fused attention probabilities (see _AttnProbs); q, k [B, U, M*d] contiguous, TF32-rounded.
+    alpha: score scale (default 1/sqrt(d) of the per-mode width).  posbias (PosBias): sliding-window positional bias
+    inside the softmax; its table receives a gradient."""
+    if alpha is None:
+        alpha = 1.0 / math.sqrt(q.shape[-1] // M)
     return _AttnProbs.apply(q.contiguous(), k.contiguous(), M, float(alpha), float(clip), drop_p, seed, diag,
-                            *_pb_args(posbias), False)
+                            *_pb_args(posbias), bool(kmajor_dq))
 
 
 def _sgemm(A, B, M, N, K, sa, sb, out=None, alpha=1.0, accumulate=False, Z=1, zs=(0, 0, 0)):

@@ -91,6 +91,13 @@ def _sq_inputs(B, M, U1, U2, d, Fd, seed=0, bq=None):
     return q, k, vp, bm, Wo, bo, gY
 
 
+def _fused(q, k, vp, M, att_p, s1, bm, hid_p, s2, Wo, bo, diag):
+    """The fused squeeze-out of CrossAttFeatTrans + ExpandedFeatTrans: dQ reads a K-major copy of the keys."""
+    from segtran_b200 import ops
+    P = ops.attn_probs(q, k, M, None, 500.0, att_p, s1, diag, kmajor_dq=True)
+    return ops.attn_pv_gelu_group_linear(P, vp, M, bm, hid_p, s2, Wo, bo)
+
+
 def _unfused(q, k, vp, M, att_p, s1, bm, hid_p, s2, Wo, bo):
     from segtran_b200 import ops
     amax = torch.full((1,), -3.0e38, device=q.device)
@@ -104,16 +111,15 @@ def _unfused(q, k, vp, M, att_p, s1, bm, hid_p, s2, Wo, bo):
     (2, 1, 4, 520, 1024, 64, 128, 0.0, 0.0),          # two-pass scores, shared queries (dq reduced over the batch)
     (2, 2, 2, 260, 300, 32, 64, 0.2, 0.2),            # both dropouts: masks regenerated in the fused backward
 ])
-def test_squeeze_out_fused_matches_unfused_path(B, bq, M, U1, U2, d, Fd, att_p, hid_p):
+def test_fused_squeeze_out_matches_unfused_path(B, bq, M, U1, U2, d, Fd, att_p, hid_p):
     """Same seeds -> same dropout masks: the fused node (sx_attn + softmax-backward GEMM epilogue) must reproduce the
     separate-kernel path (attn_scores -> sx_softmax -> P.V GEMM -> sx_softmax_bwd) in outputs and all gradients."""
-    from segtran_b200 import ops
     outs = []
     for fused in (True, False):
         q, k, vp, bm, Wo, bo, gY = _sq_inputs(B, M, U1, U2, d, Fd, seed=5, bq=bq)
         diag = torch.tensor([-3.0e38, 0.0, 0.0], device="cuda")
         if fused:
-            Y = ops.squeeze_out_fused(q, k, vp, M, 500.0, att_p, 1111, bm, hid_p, 2222, Wo, bo, diag)
+            Y = _fused(q, k, vp, M, att_p, 1111, bm, hid_p, 2222, Wo, bo, diag)
         else:
             Y = _unfused(q, k, vp, M, att_p, 1111, bm, hid_p, 2222, Wo, bo)
         (Y * gY).sum().backward()
@@ -125,12 +131,11 @@ def test_squeeze_out_fused_matches_unfused_path(B, bq, M, U1, U2, d, Fd, att_p, 
         assert err < (2e-3 if n in ("dq", "dk") else 5e-4), (n, err)
 
 
-def test_squeeze_out_fused_gradients_match_fp64_autograd():
-    from segtran_b200 import ops
+def test_fused_squeeze_out_gradients_match_fp64_autograd():
     B, M, U1, U2, d, Fd = 2, 2, 200, 320, 32, 64
     q, k, vp, bm, Wo, bo, gY = _sq_inputs(B, M, U1, U2, d, Fd, seed=9)
     diag = torch.tensor([-3.0e38, 0.0, 0.0], device="cuda")
-    Y = ops.squeeze_out_fused(q, k, vp, M, 500.0, 0.0, 0, bm, 0.0, 0, Wo, bo, diag)
+    Y = _fused(q, k, vp, M, 0.0, 0, bm, 0.0, 0, Wo, bo, diag)
     (Y * gY).sum().backward()
     got = [Y.detach()] + [t.grad.detach().clone() for t in (q, k, vp, bm, Wo, bo)]
     # fp64 autograd of the same math

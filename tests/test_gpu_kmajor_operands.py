@@ -155,11 +155,11 @@ def test_transposed_copy_has_padded_rows_and_exact_values(Z, R, C):
 
 
 @pytest.mark.parametrize("fused,U2", [(True, 300), (False, 300), (False, 301)])
-def test_squeeze_out_with_and_without_kmajor_copies_is_bit_identical(fused, U2):
+def test_squeeze_out_is_bit_identical_with_and_without_kmajor_copies(fused, U2):
     """Ragged shapes (partial tiles; 301 keys: padded copy rows), both dropouts, the fused and the separate-kernel
     squeeze-out."""
     from segtran_b200 import ops
-    from tests.test_gpu_attn import _sq_inputs, _unfused
+    from tests.test_gpu_attn import _fused, _sq_inputs, _unfused
     B, M, U1, d, Fd = 2, 2, 260, 32, 64
     res = []
     for on in (False, True):
@@ -167,7 +167,7 @@ def test_squeeze_out_with_and_without_kmajor_copies_is_bit_identical(fused, U2):
         q, k, vp, bm, Wo, bo, gY = _sq_inputs(B, M, U1, U2, d, Fd, seed=5)
         if fused:
             diag = torch.tensor([-3.0e38, 0.0, 0.0], device="cuda")
-            Y = ops.squeeze_out_fused(q, k, vp, M, 500.0, 0.2, 1111, bm, 0.2, 2222, Wo, bo, diag)
+            Y = _fused(q, k, vp, M, 0.2, 1111, bm, 0.2, 2222, Wo, bo, diag)
         else:
             Y = _unfused(q, k, vp, M, 0.2, 1111, bm, 0.2, 2222, Wo, bo)
         (Y * gY).sum().backward()

@@ -38,14 +38,14 @@ CASES = [((5, 6, 7), 2, 1.0, 2), ((6, 7), 2, 0.5, 1), ((3, 4, 5), 1, 1.5, 1)]
 
 
 @pytest.mark.parametrize("grid,R,w,B", CASES)
-def test_unfused_softmax_and_table_gradient(grid, R, w, B):
+def test_unfused_softmax_with_posbias_and_table_gradient(grid, R, w, B):
     torch.manual_seed(0)
     N, M = math.prod(grid), 2
     table = (torch.randn([2 * R + 1] * len(grid)) * 0.7).to(DEV).requires_grad_()
     s = (torch.randn(B, M, N, N) * 3).to(DEV).requires_grad_()
     g = torch.randn(B, M, N, N, device=DEV)
     amax = s.detach().max().reshape(1)
-    P = ops.softmax_posbias(s, ops.PosBias(table, R, grid, w), amax, 500.0)
+    P = ops.softmax(s, amax, 500.0, posbias=ops.PosBias(table, R, grid, w))
     (P * g).sum().backward()
     s64 = s.detach().double().cpu().requires_grad_()
     t64 = table.detach().double().cpu().requires_grad_()
@@ -56,7 +56,7 @@ def test_unfused_softmax_and_table_gradient(grid, R, w, B):
     torch.testing.assert_close(table.grad.cpu().double(), t64.grad, rtol=1e-3, atol=1e-4)
 
 
-def test_clamp_then_bias_and_gradient_before_the_clamp_mask():
+def test_softmax_clamp_then_bias_and_gradient_before_the_clamp_mask():
     torch.manual_seed(1)
     grid, R, w, clip = (5, 6, 7), 2, 1.0, 5.0
     N = math.prod(grid)
@@ -65,7 +65,7 @@ def test_clamp_then_bias_and_gradient_before_the_clamp_mask():
     g = torch.randn(1, 1, N, N, device=DEV)
     amax = s.detach().max().reshape(1)
     assert float(amax) > clip
-    P = ops.softmax_posbias(s, ops.PosBias(table, R, grid, w), amax, clip)
+    P = ops.softmax(s, amax, clip, posbias=ops.PosBias(table, R, grid, w))
     (P * g).sum().backward()
     s64 = s.detach().double().cpu().requires_grad_()
     t64 = table.detach().double().cpu().requires_grad_()
@@ -81,7 +81,7 @@ def test_clamp_then_bias_and_gradient_before_the_clamp_mask():
 
 
 @pytest.mark.parametrize("grid,R,w,B", CASES)
-def test_fused_probabilities_match_restatement_and_unfused(grid, R, w, B):
+def test_fused_probabilities_match_restatement_and_unfused_softmax(grid, R, w, B):
     torch.manual_seed(2)
     N, M, d = math.prod(grid), 4, 16
     table = (torch.randn([2 * R + 1] * len(grid)) * 0.7).to(DEV)
@@ -100,7 +100,7 @@ def test_fused_probabilities_match_restatement_and_unfused(grid, R, w, B):
     biased = s64 + w * dense_bias(table, R, grid)
     torch.testing.assert_close(lse.cpu().double(), torch.logsumexp(biased, -1), rtol=1e-4, atol=1e-4)
     # the unfused kernel on the same raw scores
-    Pu = ops.softmax_posbias(Sraw, pb, stat[2:], 500.0)
+    Pu = ops.softmax(Sraw, stat[2:], 500.0, posbias=pb)
     torch.testing.assert_close(P, Pu.detach(), rtol=1e-3, atol=1e-6)
 
 
