@@ -410,6 +410,15 @@ int sx_groupnorm_fwd(const float* x, int32_t B, int32_t C, int64_t V, int32_t G,
                      float eps, double* csum, float* stats, float* y, int32_t round_tf32, void* stream);
 int sx_groupnorm_bwd(const float* dy, const float* x, int32_t B, int32_t C, int64_t V, int32_t G, const float* gamma,
                      const float* stats, double* csum, float* coef, float* dx, float* dgamma, float* dbeta, void* stream);
+/* Cross-slice GroupNorm (the 2.5-D out-FPN's GroupNorm on a [B,C,H,W,D] volume, segtran25d.py:342, kept slice-major):
+ * x, y, dy, dx: [B, D, C, V] fp32; the statistics of group g of sample b span all D slices, D (C/G) V elements.
+ * csum: [B*D*C*2] double workspace; stats, coef, dgamma, dbeta as above.  D = 1 is sx_groupnorm_fwd / _bwd. */
+int sx_groupnorm_slices_fwd(const float* x, int32_t B, int32_t D, int32_t C, int64_t V, int32_t G, const float* gamma,
+                            const float* beta, float eps, double* csum, float* stats, float* y, int32_t round_tf32,
+                            void* stream);
+int sx_groupnorm_slices_bwd(const float* dy, const float* x, int32_t B, int32_t D, int32_t C, int64_t V, int32_t G,
+                            const float* gamma, const float* stats, double* csum, float* coef, float* dx, float* dgamma,
+                            float* dbeta, void* stream);
 
 /* -------------------------------------------------------------------------------------------
  * Training-step tail (SURVEY.md section 8 row f.2): segmentation loss and BertAdam on flat buckets.

@@ -137,6 +137,8 @@ _PROTOS = {
     "sx_resize_tokens_bwd": [_P, _L, _L, _L, _P, _L, _L, _L, _I, _I, _I, _I, C.POINTER(sx_resample_grid), _I, _P],
     "sx_groupnorm_fwd": [_P, _I, _I, _L, _I, _P, _P, _F, _P, _P, _P, _I, _P],
     "sx_groupnorm_bwd": [_P, _P, _I, _I, _L, _I, _P, _P, _P, _P, _P, _P, _P, _P],
+    "sx_groupnorm_slices_fwd": [_P, _I, _I, _I, _L, _I, _P, _P, _F, _P, _P, _P, _I, _P],
+    "sx_groupnorm_slices_bwd": [_P, _P, _I, _I, _I, _L, _I, _P, _P, _P, _P, _P, _P, _P, _P],
     "sx_seg_loss_fwd": [_P, _P, _I, _I, _L, _P, _P, _F, _P, _P, _P, _P],
     "sx_seg_loss_bwd": [_P, _P, _I, _I, _L, _P, _P, _F, _P, _P, _P],
     "sx_adam_step": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _D, _D, _D, _F, _F, _F, _L, _I, _P, _P, _P, _P, _P, _P],

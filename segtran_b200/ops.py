@@ -1845,38 +1845,51 @@ class _Conv1x1Add(torch.autograd.Function):
 
 
 class _GroupNorm(torch.autograd.Function):
-    """nn.GroupNorm(G, C) on channels-first [B,C,V] (segtran3d.py:150, :174; eps 1e-5): one reduction pass + one apply pass."""
+    """nn.GroupNorm(G, C) on channels-first [B,C,V] (segtran3d.py:150, :174; eps 1e-5): one reduction pass + one apply pass.
+    D > 1: x is D consecutive slices per sample, [B*D, C, V] read as [B, D, C, V], and the statistics of group g of sample
+    b span all D slices (nn.GroupNorm on the [B,C,*,D] volume the slices came from, segtran25d.py:342)."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, G, eps, round_out):
+    def forward(ctx, x, gamma, beta, G, eps, round_out, D):
         x = x.contiguous()
-        B, Cd, V = x.shape
+        BD, Cd, V = x.shape
+        B = BD // D
         y = torch.empty_like(x)
-        csum = torch.empty(B * Cd * 2, device=x.device, dtype=torch.float64)
+        csum = torch.empty(BD * Cd * 2, device=x.device, dtype=torch.float64)
         stats = torch.empty(B * G * 2, device=x.device, dtype=torch.float32)
-        L.call("sx_groupnorm_fwd", x.data_ptr(), B, Cd, V, G, _ptr(gamma), _ptr(beta), float(eps), csum.data_ptr(),
-               stats.data_ptr(), y.data_ptr(), _rt() if round_out else 0, _stream())
+        rt = _rt() if round_out else 0
+        if D == 1:
+            L.call("sx_groupnorm_fwd", x.data_ptr(), B, Cd, V, G, _ptr(gamma), _ptr(beta), float(eps), csum.data_ptr(),
+                   stats.data_ptr(), y.data_ptr(), rt, _stream())
+        else:
+            L.call("sx_groupnorm_slices_fwd", x.data_ptr(), B, D, Cd, V, G, _ptr(gamma), _ptr(beta), float(eps),
+                   csum.data_ptr(), stats.data_ptr(), y.data_ptr(), rt, _stream())
         ctx.save_for_backward(x, gamma, stats)
-        ctx.meta = (G,)
+        ctx.meta = (G, D)
         ctx.leaves = (gamma, beta)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, gamma, stats = ctx.saved_tensors
-        (G,) = ctx.meta
-        B, Cd, V = x.shape
+        G, D = ctx.meta
+        BD, Cd, V = x.shape
+        B = BD // D
         dy = dy.contiguous()
         dx = torch.empty_like(x)
-        csum = torch.empty(B * Cd * 2, device=x.device, dtype=torch.float64)
+        csum = torch.empty(BD * Cd * 2, device=x.device, dtype=torch.float64)
         coef = torch.empty(B * G * 2, device=x.device, dtype=torch.float32)
         dg = db = dgb = dbb = None
         if gamma is not None:
             dgb, dg = _sink_or_zeros(ctx.leaves[0])
             dbb, db = _sink_or_zeros(ctx.leaves[1])
-        L.call("sx_groupnorm_bwd", dy.data_ptr(), x.data_ptr(), B, Cd, V, G, _ptr(gamma), stats.data_ptr(), csum.data_ptr(),
-               coef.data_ptr(), dx.data_ptr(), _ptr(dgb), _ptr(dbb), _stream())
-        return dx, dg, db, None, None, None
+        if D == 1:
+            L.call("sx_groupnorm_bwd", dy.data_ptr(), x.data_ptr(), B, Cd, V, G, _ptr(gamma), stats.data_ptr(),
+                   csum.data_ptr(), coef.data_ptr(), dx.data_ptr(), _ptr(dgb), _ptr(dbb), _stream())
+        else:
+            L.call("sx_groupnorm_slices_bwd", dy.data_ptr(), x.data_ptr(), B, D, Cd, V, G, _ptr(gamma), stats.data_ptr(),
+                   csum.data_ptr(), coef.data_ptr(), dx.data_ptr(), _ptr(dgb), _ptr(dbb), _stream())
+        return dx, dg, db, None, None, None, None
 
 
 def conv1x1_add(x, W, b=None, addend=None):
@@ -1887,9 +1900,14 @@ def conv1x1_add(x, W, b=None, addend=None):
     return y.view(B, W.shape[0], *sp)
 
 
-def group_norm(x, gamma, beta, num_groups, eps=1e-5, round_out=False):
+def group_norm(x, gamma, beta, num_groups, eps=1e-5, round_out=False, slices=1):
+    """nn.GroupNorm on channels-first x [B,C,*sp].  slices=D: x is [B*D, C, *sp], D slices per sample (slice b*D + d),
+    normalised with per-sample statistics over all D slices, as nn.GroupNorm on the stacked [B,C,*sp,D] volume."""
     sp = x.shape
-    return _GroupNorm.apply(x.reshape(sp[0], sp[1], -1), gamma, beta, int(num_groups), float(eps), round_out).view(sp)
+    D = int(slices)
+    if sp[0] % D:
+        raise ValueError("group_norm: batch %d is not a multiple of slices=%d" % (sp[0], D))
+    return _GroupNorm.apply(x.reshape(sp[0], sp[1], -1), gamma, beta, int(num_groups), float(eps), round_out, D).view(sp)
 
 
 _FPN_FUSION = True
@@ -1916,17 +1934,20 @@ def conv1x1_ok(x, conv) -> bool:
         V % 4 == 0 and conv.in_channels % 4 == 0
 
 
-def fpn_stage(cur, higher, conv, norm, scheme="AN"):
+def fpn_stage(cur, higher, conv, norm, scheme="AN", slices=1):
     """One bottom-up FPN stage (segtran3d.py:299-313 / :347-359, segtran2d.py:244-257 / :286-300):
         'AN': norm(conv(cur) + upsample(higher))        otherwise: norm(conv(cur)) + upsample(higher)
-    conv: nn.Conv2d/3d with a 1x1(x1) kernel, norm: nn.GroupNorm.  The upsampled level is the GEMM epilogue's addend."""
+    conv: nn.Conv2d/3d with a 1x1(x1) kernel, norm: nn.GroupNorm.  The upsampled level is the GEMM epilogue's addend.
+    slices=D: cur and higher are slice-major 2-D maps [B*D, C, h, w] of a [B,C,h,w,D] volume (segtran25d.py:332-347); a
+    Conv3d 1x1x1 is the same per-slice GEMM, the depth-preserving trilinear upsampling is bilinear per slice, and the
+    GroupNorm takes its statistics over all D slices of a sample (group_norm(slices=D))."""
     up_size = tuple(cur.shape[2:])
     hi = higher if tuple(higher.shape[2:]) == up_size else resize_linear(higher, up_size)
     if scheme == 'AN':
         y = conv1x1_add(cur, conv.weight, conv.bias, addend=hi)
-        return group_norm(y, norm.weight, norm.bias, norm.num_groups, norm.eps)
+        return group_norm(y, norm.weight, norm.bias, norm.num_groups, norm.eps, slices=slices)
     y = conv1x1_add(cur, conv.weight, conv.bias)
-    return _Add.apply(group_norm(y, norm.weight, norm.bias, norm.num_groups, norm.eps), hi)
+    return _Add.apply(group_norm(y, norm.weight, norm.bias, norm.num_groups, norm.eps, slices=slices), hi)
 
 
 HEAD_MAXK = 8        # classes per pass of the head-contraction entry points (csrc/sx_head.cu MAXK)
@@ -2031,6 +2052,39 @@ def seg_head(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, d_pool_k=1, perm
     return _head_out(Lo, out_size)
 
 
+def seg_head_slices(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, d_pool_k=1, d_unfold=1):
+    """Collapsed voxel-wise head of the 2.5-D model on slice-major maps (segtran25d.py:351-377, :464-477).
+    curr [B*D2, Cf, H1, W1] (slice b*D2 + d); vfeat_fused [B, N, F] tokens on grid = (H2, W2, D3); Wb/bb the bridge conv,
+    Wc/bc the class conv (or the folded one from fold_unfold for --upd conv); out_size = (H, W, D) -> [B, K, H, W, D].
+    The token class scores are upsampled to (H1, W1, D2) and turned slice-major, so the head contraction runs with batch
+    B*D2 and the [B, F, H1, W1, D2] map is never built.  Depth map before the final trilinear interpolation:
+    d_unfold = Dk > 1: class row k*Dk + j at slice i lands at depth i*Dk + j; d_pool_k = Dk > 1: linear D2 -> D2*Dk."""
+    BD, Cf, H1, W1 = curr.shape
+    B = vfeat_fused.shape[0]
+    D2 = BD // B
+    K = Wc.shape[0]
+    Wc2 = Wc.reshape(K, -1)
+    HW = H1 * W1
+    parts = []
+    for k0 in range(0, K, HEAD_MAXK):
+        Wk = Wc2[k0:k0 + HEAD_MAXK]
+        kc = Wk.shape[0]
+        tv = _TokenClassScores.apply(vfeat_fused, Wk).view(B, kc, *grid)
+        tvup = resize_linear(tv, (H1, W1, D2))                                        # [B, kc, H1, W1, D2]
+        tvs = transpose(tvup.reshape(B, kc * HW, D2)).view(BD, kc, HW)               # slice-major addend
+        parts.append(_HeadContract.apply(curr, Wb, bb, Wk, None if bc is None else bc[k0:k0 + HEAD_MAXK], tvs))
+    Lo = parts[0] if len(parts) == 1 else torch.cat(parts, 1)                          # [B*D2, K, H1, W1]
+    Lo = transpose(Lo.reshape(B, D2, K * HW))                                          # [B, K*H1*W1, D2]
+    if d_unfold > 1:
+        Kc = K // d_unfold                                  # [B*Kc, Dk, H1*W1*D2] -> [B*Kc, H1*W1*D2, Dk]
+        Lo = transpose(Lo.reshape(B * Kc, d_unfold, HW * D2)).view(B, Kc, H1, W1, D2 * d_unfold)
+    else:
+        Lo = Lo.view(B, K, H1, W1, D2)
+        if d_pool_k > 1:
+            Lo = resize_linear(Lo, (H1, W1, D2 * d_pool_k))
+    return resize_linear(Lo, tuple(out_size))
+
+
 class _SubpixelResize(torch.autograd.Function):
     """Logits of the direct head from its sub-pixel scores S [B,4K,N] (csrc/sx_head.cu): the 2x2(x1) transposed conv's
     output grid is never written; bi/trilinear interpolation reads S directly and writes [B,K,H,W] / [B,K,H,W,D]."""
@@ -2059,18 +2113,28 @@ class _SubpixelResize(torch.autograd.Function):
         return dS, db, None, None
 
 
-def direct_head(fused, grid, Wt, bt, out_size):
+def direct_head(fused, grid, Wt, bt, out_size, token_order="dhw"):
     """Class head without the out-FPN (out_fpn_layers == in_fpn_layers; segtran2d.py:198-209, :421-437, segtran3d.py:
-    234-245, :478-498): ConvTranspose2d(C, K, 2, 2) / ConvTranspose3d(C, K, (2,2,1), (2,2,1)) of the fused tokens, then
-    bi/trilinear interpolation (align_corners=False) to out_size.
-    fused [B,N,C] tokens on `grid` ((H2,W2), or (D2,H2,W2) in the reference's token order); Wt [C,K,2,2] / [C,K,2,2,1];
+    234-245, :478-498, segtran25d.py:229-237): ConvTranspose2d(C, K, 2, 2) / ConvTranspose3d(C, K, (2,2,1), (2,2,1)) of
+    the fused tokens, then bi/trilinear interpolation (align_corners=False) to out_size.
+    fused [B,N,C] tokens on `grid` ((H2,W2), or (D2,H2,W2) in the 3-D model's token order); Wt [C,K,2,2] / [C,K,2,2,1];
     bt [K] or None; out_size (H,W) / (H,W,D) -> logits [B,K,H,W] / [B,K,H,W,D].
+    token_order='hwd': 3-D tokens in (h, w, d) order on grid (H2,W2,D3) (the 2.5-D model); the small sub-pixel score
+    tensor is transposed to (d, h, w) order before the resize.
     The 4K sub-pixel scores are one exact fp32 contraction of the tokens (sx_token_scores, K <= 8), and the logits come
     from them in one pass (sx_subpixel_resize_fwd)."""
     C, K = Wt.shape[0], Wt.shape[1]
     W2 = transpose(Wt.reshape(1, C, 4 * K)).view(4 * K, C)          # row 4k + 2a + c = tap (a, c) of class k
     S = _TokenClassScores.apply(fused, W2)
-    return _SubpixelResize.apply(S, bt, tuple(int(g) for g in grid), tuple(int(s) for s in out_size))
+    grid = tuple(int(g) for g in grid)
+    if token_order == "hwd":
+        H2, W2_, D3 = grid
+        B = fused.shape[0]
+        S = transpose(S.reshape(B * 4 * K, H2 * W2_, D3)).view(B, 4 * K, D3 * H2 * W2_)
+        grid = (D3, H2, W2_)
+    elif token_order != "dhw":
+        raise ValueError("direct_head: token_order must be 'dhw' or 'hwd', not %r" % (token_order,))
+    return _SubpixelResize.apply(S, bt, grid, tuple(int(s) for s in out_size))
 
 
 class _HeadDropout(torch.autograd.Function):
