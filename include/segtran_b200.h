@@ -17,7 +17,8 @@
  *  - every call is asynchronous on the cudaStream_t given (passed as void*);
  *  - return 0 on success, negative on error; sx_last_error() returns a thread-local message;
  *  - no global mutable state apart from one-time function-attribute setup (thread safe: the
- *    autograd engine calls backward entry points from its own worker thread);
+ *    autograd engine calls backward entry points from its own worker thread) and two thread-local
+ *    slots: sx_last_error's message and the transposed output sx_gemm_set_tout arms;
  *  - the device is the current CUDA context's device (torch sets it); never assumed to be 0.
  *  - there is NO CPU fallback: a missing GPU / non-sm_90 device is an error.
  */
@@ -97,6 +98,19 @@ typedef struct {
 } sx_gemm_args;
 
 int sx_gemm(const sx_gemm_args* args, void* stream);
+
+/* Transposed second output of the next sx_gemm call made on the same host thread (sx_gemm_set_tout arms it, that call
+ * consumes it whether it succeeds or not; NULL disarms): a copy of the final fp32 C values (after alpha, bias,
+ * activation, dropout and TF32 rounding) at ct[z1*ct_stride_z1 + z0*ct_stride_z0 + n*ldct + m] = C[z1][z0][m][n], so
+ * that a later product contracting over m reads it K-major.  Requirements: tf32 operands, both K-major; split_k = 1,
+ * accumulate = 0, fp32 C; ct 16-byte aligned, ldct >= M, ldct and the z strides multiples of 4.  It is a separate
+ * block so that sx_gemm_args keeps its layout. */
+typedef struct {
+  float* ct;
+  int64_t ldct, ct_stride_z0, ct_stride_z1;
+} sx_gemm_tout;
+
+int sx_gemm_set_tout(const sx_gemm_tout* tout);
 
 /* ---------------------------------------------------------------------------------------------
  * Sliding-window positional biases (SlidingPosBiases2D/3D, segtran_shared.py:1002-1175), never expanded to [N,N]:

@@ -41,6 +41,10 @@ class sx_gemm_args(C.Structure):
                 ("part", C.c_void_p), ("part_floats", C.c_int64)]
 
 
+class sx_gemm_tout(C.Structure):
+    _fields_ = [("ct", C.c_void_p), ("ldct", C.c_int64), ("ct_stride_z0", C.c_int64), ("ct_stride_z1", C.c_int64)]
+
+
 class sx_posbias(C.Structure):
     _fields_ = [("table", C.c_void_p), ("pd", C.c_int32), ("R", C.c_int32), ("grid", C.c_int32 * 3), ("w", C.c_float)]
 
@@ -79,6 +83,7 @@ _P, _I, _L, _F, _U64, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint
 # name -> argtypes (every function returns int; 0 = success)
 _PROTOS = {
     "sx_gemm": [C.POINTER(sx_gemm_args), _P],
+    "sx_gemm_set_tout": [C.POINTER(sx_gemm_tout)],
     "sx_gemm_debug_set": [C.c_char_p, _L],
     "sx_attn_probs_fwd": [C.POINTER(sx_attn_probs_args), _P],
     "sx_attn_consist_fwd": [C.POINTER(sx_consist_args), _P],
@@ -176,7 +181,7 @@ def check(rc, what):
 
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
-_LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
+_LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0, "sx_gemm_set_tout": 0,
              "sx_attn_probs_fwd": 2, "sx_colsum_batched": 2, "sx_dot": 2, "sx_head_contract_bwd_weight": 2,
              "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2, "sx_head_dropout_bwd": 2, "sx_edt_sq": 3}
 launch_count = 0

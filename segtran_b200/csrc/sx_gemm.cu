@@ -16,6 +16,8 @@
 // A 128 x 256 tile (each consumer issues m64n256k8 into 128 accumulators) moves 25 % fewer operand bytes from L2 into
 // shared memory per FLOP than a 128 x 128 tile.  Every output element still sees the same k-blocks in the same order and
 // the same k8 steps, so both tile widths give bit-identical results.
+// K-major tf32 launches may also write the final values transposed (`ct`), staged through shared memory so the stores
+// stay coalesced: a product that later contracts over C's rows then reads that copy K-major.
 //
 // Replaces in the reference: nn.Linear / torch.matmul / grouped Conv1d call sites on the hot path,
 // code/networks/segtran_shared.py:243, :267, :414, :447, :559-560, :566 (and their autograd backward).
@@ -32,10 +34,15 @@ constexpr int NUM_THREADS = 384;          // warpgroup 0: TMA + transposers; war
 constexpr int STAGES = 4;                 // K-major operand ring (what wgmma reads)
 constexpr int XPOSE_WARPS = 3;            // warps 1-3 of warpgroup 0
 constexpr int BN_WIDE = 256;              // tile cols of the wide instantiation (tf32, both operands K-major)
+// transposed second output (ct): each consumer warpgroup stages one 64-row x 32-column chunk column-major, 68 floats per
+// column: a warp's fragment stores (8 rows x 4 column pairs) then hit 32 distinct banks, and a column is 16-byte aligned
+constexpr int CT_LD = 68;
+constexpr int CT_WG_FLOATS = 32 * CT_LD;  // 8.5 KB per warpgroup
 
 // Shared-memory plan of one instantiation.  A tf32 MN-major operand goes through a raw ring (as TMA lands it) before
 // the transposers write its K-major copy into the stage; everything else lands in the stage directly.  BN_T = 256 (the
-// wide tile) has K-major tf32 operands only: 16 KB of A + 32 KB of B per stage, no raw ring.
+// wide tile) has K-major tf32 operands only: 16 KB of A + 32 KB of B per stage, no raw ring.  The K-major tf32
+// instantiations also hold the two warpgroups' ct staging chunks.
 template <int ES, bool A_MN, bool B_MN, int BN_T>
 struct Plan {
   static_assert(BN_T == BN || (BN_T == BN_WIDE && ES == 4 && !A_MN && !B_MN),
@@ -47,8 +54,10 @@ struct Plan {
   static constexpr int RAW_BYTES = (XA ? A_STAGE_BYTES : 0) + (XB ? B_STAGE_BYTES : 0);      // per raw slot
   static constexpr int RAW_SLOTS = !XPOSE ? 0 : (XA && XB ? 3 : 4);
   static constexpr int DIRECT_BYTES = STAGE_BYTES - RAW_BYTES;   // per stage, loaded by TMA straight into the stage
-  static constexpr int SMEM = STAGES * STAGE_BYTES + RAW_SLOTS * RAW_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  static_assert(SMEM <= 227 * 1024, "sx_gemm: shared memory plan exceeds 227 KB");   // wide: 4 x 48 KB + 1.25 KB
+  static constexpr bool CT = ES == 4 && !A_MN && !B_MN;
+  static constexpr int CT_BYTES = CT ? 2 * CT_WG_FLOATS * 4 : 0;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + RAW_SLOTS * RAW_BYTES + 1024 /*align*/ + 256 /*barriers*/ + CT_BYTES;
+  static_assert(SMEM <= 227 * 1024, "sx_gemm: shared memory plan exceeds 227 KB");   // wide: 4 x 48 KB + 18.25 KB
   // the transposers address B at A's offset + A_STAGE_BYTES in both the raw slot and the stage, and move 256 4 x 4
   // blocks (4 boxes of 32 x 32) per operand: both hold only for 128 x 128 tf32 operand tiles
   static_assert(!XPOSE || (A_STAGE_BYTES == 16384 && B_STAGE_BYTES == 16384 && BM == 128 && BN == 128),
@@ -79,6 +88,8 @@ struct GemmParams {
   const unsigned long long* drop_seed_dev;
   const float* addend;   // optional fp32 tensor in C's layout added to alpha*acc before bias/activation (tf32x3 passes)
   int stream_out;        // output larger than half the L2: store with evict-first (st.global.cs), keep operands (evict-last)
+  float* ct;             // optional transposed copy of the final C values: ct[z][n][m] (K-major tf32 instantiations)
+  long long ldct, ct_sz0, ct_sz1;
 };
 
 // MN-major tf32 operand tile as TMA left it (4 boxes of 32 k rows x 128 B of MN, SWIZZLE_128B: 16-byte chunk c of k row
@@ -110,6 +121,9 @@ __device__ __forceinline__ void xpose_store(uint32_t dst, int b, const float4 (&
   st(3, v[0].w, v[1].w, v[2].w, v[3].w);
 }
 
+// barrier of one consumer warpgroup (ids 1, 2; id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
 template <int ES, bool A_MN, bool B_MN, int BN_T>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
@@ -131,6 +145,7 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* empty_bar = bars + STAGES;         // [STAGES]  consumers -> TMA / transposers (one arrival per warpgroup)
   uint64_t* raw_full = bars + 2 * STAGES;      // [RAW_SLOTS]  TMA -> transposers
   uint64_t* raw_empty = raw_full + PL::RAW_SLOTS;   // [RAW_SLOTS]  transposers -> TMA
+  float* ct_stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);   // [2][32][CT_LD] (PL::CT)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -498,6 +513,38 @@ sx_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       } else {
         store_frag(p.C, f, zoff, row0, col0, p.accumulate != 0);
       }
+      if constexpr (PL::CT) {
+        if (p.ct) {                             // the same values, transposed: staged so each ct row segment is 256 B
+          float* cs = ct_stage + cw * CT_WG_FLOATS;
+          named_bar_sync(1 + cw);               // the previous chunk's reads of cs are done
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) cs[(8 * j + tc + e) * CT_LD + wq * 16 + 8 * h + tr] = f[4 * j + 2 * h + e];
+          named_bar_sync(1 + cw);
+          const int m0 = mb * BM + cw * 64;
+          const long long ctz = (long long)z1 * p.ct_sz1 + (long long)z0 * p.ct_sz0;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {         // 32 columns x 16 float4 over the 128 threads
+            const int v = wtid + 128 * i, n = v >> 4, r = (v & 15) * 4;
+            const int gn = col0 + n, gm = m0 + r;
+            if (gn < p.N && gm < p.M) {
+              const float4 x = *reinterpret_cast<const float4*>(cs + n * CT_LD + r);
+              float* o = p.ct + ctz + (long long)gn * p.ldct + gm;
+              if (gm + 3 < p.M) {
+                if (p.stream_out) __stcs(reinterpret_cast<float4*>(o), x);
+                else *reinterpret_cast<float4*>(o) = x;
+              } else {
+                o[0] = x.x;
+                if (gm + 1 < p.M) o[1] = x.y;
+                if (gm + 2 < p.M) o[2] = x.z;
+              }
+            }
+          }
+        }
+      }
       if constexpr (WIDE) {
 #pragma unroll
         for (int i = 0; i < BN_T / 2 - 16; ++i) acc[i] = acc[i + 16];
@@ -564,7 +611,8 @@ extern "C" int sx_gemm_debug_set(const char* key, int64_t value) {
   return 0;
 }
 
-extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
+// t: the transposed second output, or null
+static int gemm_run(const sx_gemm_args* a, const sx_gemm_tout* t, void* stream) {
   SX_REQUIRE(a != nullptr, "sx_gemm: null args");
   SX_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0 && a->Z0 > 0 && a->Z1 > 0, "sx_gemm: bad shape M=%d N=%d K=%d Z=%dx%d",
              a->M, a->N, a->K, a->Z0, a->Z1);
@@ -633,9 +681,20 @@ extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
   SX_REQUIRE(!a->addend || (p.split_k == 1 && !a->accumulate && a->c_dtype == SX_F32), "sx_gemm: addend needs split_k=1, accumulate=0, fp32 C");
   p.drop_p = a->drop_p; p.drop_seed = a->drop_seed;
   p.drop_seed_dev = reinterpret_cast<const unsigned long long*>(a->drop_seed_dev);
+  if (t) {
+    SX_REQUIRE(t->ct != nullptr, "sx_gemm: null ct");
+    SX_REQUIRE(es == 4 && !amn && !bmn, "sx_gemm: ct needs tf32 operands, both K-major");
+    SX_REQUIRE(p.split_k == 1 && !a->accumulate && a->c_dtype == SX_F32,
+               "sx_gemm: ct needs split_k=1, accumulate=0, fp32 C");
+    SX_REQUIRE((reinterpret_cast<uintptr_t>(t->ct) & 15) == 0 && t->ldct % 4 == 0 && t->ct_stride_z0 % 4 == 0 &&
+                   t->ct_stride_z1 % 4 == 0 && t->ldct >= a->M,
+               "sx_gemm: ct must be 16-byte aligned with ldct >= M and ldct, z strides multiples of 4");
+    p.ct = t->ct; p.ldct = t->ldct; p.ct_sz0 = t->ct_stride_z0; p.ct_sz1 = t->ct_stride_z1;
+  }
   {
     // H100: 50 MB of L2
-    const double out_bytes = (double)a->M * a->N * a->Z0 * a->Z1 * (p.c_bf16 ? 2 : 4) * (a->preact ? 2 : 1);
+    const double out_bytes =
+        (double)a->M * a->N * a->Z0 * a->Z1 * (p.c_bf16 ? 2 : 4) * (1 + (a->preact ? 1 : 0) + (t ? 1 : 0));
     p.stream_out = out_bytes > 25.0 * 1024 * 1024;
   }
 
@@ -660,4 +719,19 @@ extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
   if (!amn && bmn) return launch<2, false, true>(ta, tb, p, grid, st);
   if (amn && !bmn) return launch<2, true, false>(ta, tb, p, grid, st);
   return launch<2, true, true>(ta, tb, p, grid, st);
+}
+
+// the transposed output armed for the next sx_gemm call of this host thread
+static thread_local sx_gemm_tout g_tout{};
+
+extern "C" int sx_gemm_set_tout(const sx_gemm_tout* t) {
+  g_tout = t ? *t : sx_gemm_tout{};
+  SX_REQUIRE(t == nullptr || t->ct != nullptr, "sx_gemm_set_tout: null ct");
+  return 0;
+}
+
+extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
+  const sx_gemm_tout t = g_tout;          // consumed by this call, whether it succeeds or not
+  g_tout = sx_gemm_tout{};
+  return gemm_run(a, t.ct ? &t : nullptr, stream);
 }

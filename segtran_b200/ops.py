@@ -376,9 +376,10 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
                preact: Optional[torch.Tensor] = None, accumulate: bool = False, split_k: Optional[int] = None,
                amax: Optional[torch.Tensor] = None, drop_p: float = 0.0, seed: int = 0, round_out: bool = True,
                reduce_z1: bool = False, addend: Optional[torch.Tensor] = None,
-               gelu_bwd: Optional[torch.Tensor] = None) -> torch.Tensor:
+               gelu_bwd: Optional[torch.Tensor] = None, ct: Optional[torch.Tensor] = None) -> torch.Tensor:
     """a [..., M, K], b [..., N, K] (strided fp32 views; either dim may be the contiguous one) ->
-    out [z1, z0, M, N] fp32.  With reduce_z1 the z1 batch dim is summed into one output (atomic accumulate)."""
+    out [z1, z0, M, N] fp32.  With reduce_z1 the z1 batch dim is summed into one output (atomic accumulate).
+    ct [..., N, M] (m contiguous): the epilogue also writes the final values transposed there (both operands K-major)."""
     _req_cuda(a, b, out, bias, preact, amax)
     if a.dtype != torch.float32 or b.dtype != torch.float32:
         raise L.SxError("gemm_nt: fp32 operands expected (precision policy %s)" % _PRECISION)
@@ -394,7 +395,7 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
             raise L.SxError("gemm_nt: batch dims do not broadcast")
     oz1 = 1 if reduce_z1 else Z1
     fresh = out is None
-    linear_epi = (not gelu) and preact is None and drop_p == 0.0 and amax is None and gelu_bwd is None
+    linear_epi = (not gelu) and preact is None and drop_p == 0.0 and amax is None and gelu_bwd is None and ct is None
     if split_k is None:
         split_k = _pick_split_k(M, N, K, Z0 * Z1) if (linear_epi and (fresh or accumulate or reduce_z1)) else 1
     if fresh:
@@ -451,6 +452,16 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
         if addend.dtype != torch.float32 or tuple(addend.shape[-2:]) != (M, N) or _as4(addend).stride() != o4.stride():
             raise L.SxError("gemm_nt: addend must be an fp32 tensor in the output's layout")
         g.addend = addend.data_ptr()
+    if ct is not None:
+        t4 = _as4(ct)
+        if ct.dtype != torch.float32 or tuple(t4.shape[-2:]) != (N, M) or t4.stride(-1) != 1 or round_after:
+            raise L.SxError("gemm_nt: ct must be an fp32 [..., N, M] view with m contiguous, on a single-pass product")
+        t = L.sx_gemm_tout()
+        t.ct = t4.data_ptr()
+        t.ldct = t4.stride(-2)
+        t.ct_stride_z0 = t4.stride(1) if t4.shape[1] > 1 else 0
+        t.ct_stride_z1 = t4.stride(0) if t4.shape[0] > 1 else 0
+        L.call("sx_gemm_set_tout", C.byref(t))             # consumed by the next sx_gemm call of this thread
     L.call("sx_gemm", C.byref(g), _stream())
     if round_after and fresh:                # (caller-provided accumulators are gradient buffers: never rounded)
         L.call("sx_convert", out.data_ptr(), L.SX_F32, out.numel(), out.data_ptr(), L.SX_F32, 1, _stream())
@@ -462,14 +473,16 @@ def gemm_nt(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] = N
             preact: Optional[torch.Tensor] = None, accumulate: bool = False, split_k: Optional[int] = None,
             amax: Optional[torch.Tensor] = None, drop_p: float = 0.0, seed: int = 0, round_out: bool = True,
             reduce_z1: bool = False, gelu_bwd: Optional[torch.Tensor] = None,
-            addend: Optional[torch.Tensor] = None, tag: str = "big") -> torch.Tensor:
+            addend: Optional[torch.Tensor] = None, tag: str = "big", ct: Optional[torch.Tensor] = None) -> torch.Tensor:
     """C[..., m, n] = epilogue(alpha * sum_k a[..., m, k] b[..., n, k]) on the wgmma GEMM.  One launch on TF32-rounded
     operands, or — in 'tf32x3' mode / for call-site classes the precision policy maps to it — three passes on the hi/lo
-    operand splits (fp32-grade products)."""
+    operand splits (fp32-grade products).  ct: see _gemm_nt_1 (single-pass products only)."""
     if not _three_pass(tag):
         return _gemm_nt_1(a, b, out=out, alpha=alpha, bias=bias, bias_mode=bias_mode, gelu=gelu, preact=preact,
                           accumulate=accumulate, split_k=split_k, amax=amax, drop_p=drop_p, seed=seed,
-                          round_out=round_out, reduce_z1=reduce_z1, gelu_bwd=gelu_bwd, addend=addend)
+                          round_out=round_out, reduce_z1=reduce_z1, gelu_bwd=gelu_bwd, addend=addend, ct=ct)
+    if ct is not None:
+        raise L.SxError("gemm_nt: ct needs a single-pass product")
     _req_cuda(a, b)
     # ONE launch over K-concatenated operand splits: [A_hi | A_lo | A_hi] . [B_hi | B_hi | B_lo]^T (fp32 accumulation in registers
     # over the three partial products), so every epilogue / accumulate / split-K option works unchanged
@@ -544,8 +557,8 @@ def round_tf32(x: torch.Tensor) -> torch.Tensor:
 # feeds (the grouped output Linear's Wo, the token-row Linear weights, the attractor-side keys and the value bank V'),
 # it is transposed once into a K-major copy (rows padded to 16 bytes for TMA); the product reads the same values, so the
 # result keeps its bits.  bf16 products use wgmma's transpose bits and tf32x3 products read contiguous split copies:
-# neither needs this.  SEGTRAN_KMAJOR_COPIES=0 (or set_kmajor_copies(False)) keeps the MN-major operands, to time the
-# two paths against each other.
+# neither needs this.  The same switch covers the large token contractions (_token_kmajor).  SEGTRAN_KMAJOR_COPIES=0
+# (or set_kmajor_copies(False)) keeps the MN-major operands, to time the two paths against each other.
 _KMAJOR_COPIES = os.environ.get("SEGTRAN_KMAJOR_COPIES", "1") != "0"
 
 
@@ -564,6 +577,18 @@ def _transposed(x: torch.Tensor, Z: int, R: int, Cd: int) -> torch.Tensor:
     y = _rowpad_empty((Z, Cd, R), x.device)
     L.call("sx_transpose", x.data_ptr(), Z, R, Cd, y.stride(1), y.data_ptr(), _stream())
     return y
+
+
+def _token_kmajor(M: int, N: int, K: int, Z: int, tag: str = "big") -> bool:
+    """K-major operands for a product that contracts over K tokens (both operands token-major in the forward): a
+    transposed copy, or a transposed second output of the GEMM that made the operand (sx_gemm's `ct`), lets the product
+    skip the in-kernel transposes and take the 128 x 256 tile.  Taken when the copies are on and the K-major product
+    would run on wide tiles (the sx_gemm() rule: N > 128 and more than one wave of 128 x 256 tiles over 132 SMs) over a
+    contraction of at least 1024 tokens, with M and N of at least 512: an element of a copied operand then feeds 2 x 512
+    FLOPs or more.  On an H100 the K-major product saves about 0.0045 ps per FLOP (~120 -> ~260 TFLOP/s) against about
+    3 ps per copied element (8 bytes at ~2.6 TB/s), which breaks even near 350 outputs per element."""
+    return _kmajor_copies(tag) and min(M, N) >= 512 and K >= 1024 and \
+        2 * ((M + 127) // 128) * ((N + 255) // 256) * Z > 132
 
 
 def _weight_t(Wr: torch.Tensor, Z: int, O: int, I: int) -> torch.Tensor:
@@ -959,7 +984,8 @@ class _AttnPV(torch.autograd.Function):
             gemm_nt(P, _head_cols(v, B, U2, M, Fd, _kmajor_copies(tag)), out=U.view(B, U1, M, Fd).permute(0, 2, 1, 3),
                     tag=tag, round_out=round_out)
         else:
-            vv = v.view(B, U2, M, Fd).permute(0, 2, 3, 1)          # [B,M,F,U2]: the "N x K" operand, F contiguous
+            # [B,M,F,U2]: the "N x K" operand, F contiguous (or a K-major copy, when the token contraction pays for it)
+            vv = _head_cols(v, B, U2, M, Fd, _token_kmajor(U1, Fd, U2, B * M, tag))
             U = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
             gemm_nt(P, vv, out=U, tag=tag, round_out=round_out)
         ctx.save_for_backward(P, v)
@@ -989,9 +1015,11 @@ class _AttnPV(torch.autograd.Function):
         return dP, dv, None, None, None, None
 
 
-def _pv_grads(dU, P, v, M, Fd, need_p, need_v, tag):
+def _pv_grads(dU, P, v, M, Fd, need_p, need_v, tag, dUt=None):
     """Gradients of U[b,m] = P[b,m] V[b,:,m] (v [B,U2,M*F], dU [B,M,U1,F] contiguous):
-    dP[b,m] = dU[b,m] V[b,:,m]^T (row-padded like P) and dV[b,:,m] = P[b,m]^T dU[b,m]."""
+    dP[b,m] = dU[b,m] V[b,:,m]^T (row-padded like P) and dV[b,:,m] = P[b,m]^T dU[b,m].  dUt [B,M,F,U1] (U1
+    contiguous): dU transposed; dV then reads K-major operands (P through a transposed copy).  Without dUt, both are
+    transposed copies where _token_kmajor takes them."""
     B, _, U1, U2 = P.shape
     dP = dv = None
     if need_p:
@@ -999,8 +1027,15 @@ def _pv_grads(dU, P, v, M, Fd, need_p, need_v, tag):
         gemm_nt(dU, v.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False, tag=tag)
     if need_v:
         dv = torch.empty_like(v)
-        gemm_nt(P.transpose(-1, -2), dU.transpose(-1, -2), out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3),
-                round_out=False, tag=tag)
+        if dUt is None and _token_kmajor(U2, Fd, U1, B * M, tag):
+            dUt = _transposed(dU, B * M, U1, Fd).unflatten(0, (B, M))
+        if dUt is not None:
+            Pt = _transposed(P, B * M, U1, U2).unflatten(0, (B, M))
+            gemm_nt(Pt, dUt, out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3), round_out=False, tag=tag)
+            del Pt
+        else:
+            gemm_nt(P.transpose(-1, -2), dU.transpose(-1, -2), out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3),
+                    round_out=False, tag=tag)
     return dP, dv
 
 
@@ -1062,16 +1097,22 @@ def _group_linear_fwd(G, Wo, bo):
     return Y, Wr
 
 
-def _group_linear_param_grads(dY, G, Wo, bo, need_w, need_b):
+def _group_linear_param_grads(dY, G, Wo, bo, need_w, need_b, Gt=None):
     """(dWo, dbo) of _group_linear_fwd: dWo[m] = sum_b dY[b,m]^T G[b,m] and the column sums of dY (dY contiguous); a
-    gradient that goes straight into the parameter's .grad is returned as None."""
-    B, M, N, Fd = G.shape
+    gradient that goes straight into the parameter's .grad is returned as None.  Gt [B,M,F,N] (tokens contiguous): G
+    transposed; the product then reads K-major operands (dY through a transposed copy), G is not read."""
+    B, M, N, Fd = dY.shape
     dW = db = None
     if need_w:
-        dW = _param_grad(Wo, dY.transpose(-1, -2), G.transpose(-1, -2), (1, M, Fd, Fd), reduce_z1=True)
+        if Gt is not None:
+            dYt = _transposed(dY, B * M, N, Fd).unflatten(0, (B, M))
+            dW = _param_grad(Wo, dYt, Gt, (1, M, Fd, Fd), reduce_z1=True)
+            del dYt
+        else:
+            dW = _param_grad(Wo, dY.transpose(-1, -2), G.transpose(-1, -2), (1, M, Fd, Fd), reduce_z1=True)
     if need_b:
         tgt = _grad_target(bo)
-        buf = tgt if tgt is not None else _zeros((M * Fd,), G.device)
+        buf = tgt if tgt is not None else _zeros((M * Fd,), dY.device)
         L.call("sx_colsum_batched", dY.data_ptr(), B, M * N * Fd, M, N * Fd, N, Fd, Fd, buf.data_ptr(),
                *_part_args(dY.device), _stream())
         db = None if tgt is not None else buf
@@ -1093,18 +1134,22 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
         P = _rowpad(P)
         G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
         H = torch.empty_like(G)
+        # the token contractions of backward (dWo = dY^T G, dV' = P^T dH) read K-major operands when that pays: G and dH
+        # come transposed out of the epilogues of the GEMMs that make them, P and dY through transposed copies
+        kt = _token_kmajor(Fd, Fd, U1, M) and _token_kmajor(U2, Fd, U1, B * M)
+        Gt = _rowpad_empty((B, M, Fd, U1), P.device) if kt else None
         gemm_nt(P, _head_cols(v, B, U2, M, Fd, _kmajor_copies()), out=G, bias=bm, gelu=True, preact=H, drop_p=drop_p,
-                seed=seed)
+                seed=seed, ct=Gt)
         Y, Wr = _group_linear_fwd(G, Wo, bo)
-        ctx.save_for_backward(P, v, H, G, Wr)
-        ctx.meta = (M, Fd, drop_p, seed)
+        ctx.save_for_backward(P, v, H, Gt if kt else G, Wr)      # backward reads G only through one of the two
+        ctx.meta = (M, Fd, drop_p, seed, kt)
         ctx.leaves = (bm, Wo, bo)
         return Y
 
     @staticmethod
     def backward(ctx, dY):
         P, v, H, G, Wr = ctx.saved_tensors
-        M, Fd, drop_p, seed = ctx.meta
+        M, Fd, drop_p, seed, kt = ctx.meta
         bm, Wo, bo = ctx.leaves
         dY = dY.contiguous()
         dbm_buf = dbm = None
@@ -1114,11 +1159,14 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
             dbm = None if tgt is not None else dbm_buf
         # dH = mask * (dY Wo) * gelu'(H), TF32-rounded for the two GEMMs that consume it
         dH = torch.empty_like(H)
-        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=seed)
+        B, _, U1, _ = P.shape
+        dHt = _rowpad_empty((B, M, Fd, U1), dY.device) if kt and ctx.needs_input_grad[1] else None
+        gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=seed, ct=dHt)
         if dbm_buf is not None:             # column sums of dH = the gradient of MMSharedMid's bias
             colsum(dH.view(-1, Fd), out=dbm_buf)
-        dW, dbo = _group_linear_param_grads(dY, G, Wo, bo, ctx.needs_input_grad[6], ctx.needs_input_grad[7])
-        dP, dv = _pv_grads(dH, P, v, M, Fd, ctx.needs_input_grad[0], ctx.needs_input_grad[1], "big")
+        dW, dbo = _group_linear_param_grads(dY, None if kt else G, Wo, bo, ctx.needs_input_grad[6],
+                                            ctx.needs_input_grad[7], Gt=G if kt else None)
+        dP, dv = _pv_grads(dH, P, v, M, Fd, ctx.needs_input_grad[0], ctx.needs_input_grad[1], "big", dUt=dHt)
         return dP, dv, None, dbm, None, None, dW, dbo
 
 
