@@ -547,6 +547,35 @@ int sx_surface_hist(const uint8_t* src_border, const int32_t* dist, int32_t K, i
                     int64_t ldh, void* stream);
 int sx_surface_stats(const uint32_t* hist, int32_t K, int32_t nbins, int64_t ldh, double* out, int64_t ldo, void* stream);
 
+/* -------------------------------------------------------------------------------------------
+ * Batch preparation of the 3-D training loop (csrc/sx_prep3d.cu; code/train3d.py:711-715, brats_map_label and
+ * RandomResizedCrop of dataloaders/datasets3d.py:16-40, :611-657).
+ * sx_brats_map_label: out [B][K][V] fp32 (written; K = 2 if binarize else 4) = the BraTS n-hot map of the [B][V] labels
+ *   of type `dtype` (SX_LABEL_*), compared in that type: class 0 is label == 0; binarized, class 1 is label > 0;
+ *   otherwise classes 1, 2, 3 are label == 3 (ET), label in {1, 2, 3} (WT), label in {1, 3} (TC).
+ * sx_draw_resized_crop: rec[0..5] (fp32, written by one thread) = (s_h, s_w, s_d, h_start, w_start, d_start): s uniform
+ *   on [min_scale, max_scale) with 2^-24 resolution (one draw for all axes if isotropic, else three in H, W, D order),
+ *   then per axis a start uniform on [0, max(int(L s), out) - out], int(L s) in float32.  The draws are a function of the
+ *   64-bit seed (*seed_dev when seed_dev is not NULL, else seed) only.
+ * sx_resized_crop: for each operand, y [B][C][oh][ow][od] (contiguous, written) = the crop at the starts of rec of
+ *   F.pad(F.interpolate(x, (int(H s_h), int(W s_w), int(D s_d)), trilinear, align_corners=False)), padded by
+ *   max(out - L', 0) split pad/2 before and the rest after; every cell outside the padded intermediate is 0, so any
+ *   record is safe.  x has any element strides.  The taps of a voxel are shared by both operands; b may be NULL.
+ * ------------------------------------------------------------------------------------------- */
+enum { SX_LABEL_U8 = 0, SX_LABEL_I16 = 1, SX_LABEL_I32 = 2, SX_LABEL_I64 = 3, SX_LABEL_F32 = 4 };
+typedef struct {
+  const float* x;       /* [B][C][H][W][D] at the element strides below */
+  int64_t stride[5];
+  float* y;             /* [B][C][oh][ow][od], contiguous */
+  int32_t C;
+  int32_t _pad;
+} sx_crop_operand;
+int sx_brats_map_label(const void* label, int32_t dtype, int32_t B, int64_t V, int32_t binarize, float* out, void* stream);
+int sx_draw_resized_crop(const uint64_t* seed_dev, uint64_t seed, int32_t H, int32_t W, int32_t D, int32_t oh, int32_t ow,
+                         int32_t od, float min_scale, float max_scale, int32_t isotropic, float* rec, void* stream);
+int sx_resized_crop(const sx_crop_operand* a, const sx_crop_operand* b, int32_t B, int32_t H, int32_t W, int32_t D,
+                    int32_t oh, int32_t ow, int32_t od, const float* rec, void* stream);
+
 /* debug knobs for bring-up (descriptor field overrides); not part of the stable ABI */
 int sx_gemm_debug_set(const char* key, int64_t value);
 

@@ -19,6 +19,7 @@ SX_ACT_NONE, SX_ACT_GELU, SX_ACT_GELU_BWD = 0, 1, 2
 SX_SCHED_WARMUP_LINEAR, SX_SCHED_WARMUP_CONSTANT = 0, 1
 SX_CONSIST_BCE, SX_CONSIST_MARGIN = 0, 1
 SX_HEAD_DMAP_NONE, SX_HEAD_DMAP_INTERP, SX_HEAD_DMAP_UNFOLD = 0, 1, 2
+SX_LABEL_U8, SX_LABEL_I16, SX_LABEL_I32, SX_LABEL_I64, SX_LABEL_F32 = 0, 1, 2, 3, 4
 
 
 class SxError(RuntimeError):
@@ -78,6 +79,10 @@ class sx_resample_grid(C.Structure):
     _fields_ = [("lin", C.c_int32 * 3), ("lout", C.c_int32 * 3), ("ratio", C.c_float * 3)]
 
 
+class sx_crop_operand(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("stride", C.c_int64 * 5), ("y", C.c_void_p), ("C", C.c_int32), ("_pad", C.c_int32)]
+
+
 _P, _I, _L, _F, _U64, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64, C.c_double
 
 # name -> argtypes (every function returns int; 0 = success)
@@ -119,6 +124,9 @@ _PROTOS = {
     "sx_edt_sq": [_P, _I, _I, _I, _I, _P, _P],
     "sx_surface_hist": [_P, _P, _I, _L, _I, _P, _L, _P],
     "sx_surface_stats": [_P, _I, _I, _L, _P, _L, _P],
+    "sx_brats_map_label": [_P, _I, _I, _L, _I, _P, _P],
+    "sx_draw_resized_crop": [_P, _U64, _I, _I, _I, _I, _I, _I, _F, _F, _I, _P, _P],
+    "sx_resized_crop": [C.POINTER(sx_crop_operand), C.POINTER(sx_crop_operand), _I, _I, _I, _I, _I, _I, _I, _P, _P],
     "sx_split_tf32": [_P, _L, _P, _P, _P],
     "sx_split_tf32_cat": [_P, _I, _I, _I, _I, _L, _L, _L, _L, _I, _I, _P, _P],
     "sx_transpose": [_P, _L, _I, _I, _I, _P, _P],
