@@ -380,17 +380,23 @@ int sx_subpixel_resize_bwd(const float* dout, int32_t B, int32_t K, int32_t D2, 
 /* Out-FPN dropout head (--outdrop; segtran3d.py:372-396, :488-490; segtran2d.py:304-311, :427), which cannot be
  * collapsed: the dropout mask is per channel.  The dropped map X [B,F',D',HW] is never written:
  *   Ls[b,k,d',hw] = bc[k] + sum_f Wc[k,f] keep(b,f,d',hw) X[b,f,d',hw] / (1-p)
- * with X formed on the fly from src [B,Fs,Ds,HW] by the depth map `dmap`:
+ * with X formed on the fly from src (element src[b,fs,i,hw]) by the depth map `dmap`:
  *   SX_HEAD_DMAP_NONE   X = src                                    (F' = Fs, D' = Ds; 2-D heads pass Ds = 1)
  *   SX_HEAD_DMAP_INTERP X = linear resize of src along depth to D' = Dk*Ds (F.interpolate, align_corners=False)
  *   SX_HEAD_DMAP_UNFOLD X[b,f,j*Ds+i,hw] = src[b,f*Dk+j,i,hw]      (out_fpn_upsampleD's reshape; F' = Fs/Dk, D' = Dk*Ds)
+ *   SX_HEAD_DMAP_UNFOLD_INTERLEAVED X[b,f,i*Dk+j,hw] = src[b,f*Dk+j,i,hw]   (the 2.5-D model's reshape,
+ *                       segtran25d.py:357-362; F' = Fs/Dk, D' = Dk*Ds)
+ * src_layout says where src[b,fs,i,hw] sits (dsrc uses the same layout); every depth map works on either:
+ *   SX_HEAD_SRC_DEPTH_MAJOR (0)  ((b*Fs + fs)*Ds + i)*HW + hw   [B,Fs,Ds,HW] (3-D and 2-D heads; zero-initialised args)
+ *   SX_HEAD_SRC_SLICE_MAJOR (1)  ((b*Ds + i)*Fs + fs)*HW + hw   [B,Ds,Fs,HW] (the 2.5-D head's [B*Ds,Fs,H1,W1] maps)
  * keep(e) = the counter-based dropout hash of the flat index e of the element in [B,F',D',HW] layout with the effective
  * seed seed + *seed_dev (CUDA-graph safe), p in [0, 1).  Wc [K][F'], bc [K] (optional); any K (classes are processed
  * in chunks of 4).  Ls / dLs: [B][K][D'][HW].
- * fwd writes Ls.  bwd writes dsrc [B,Fs,Ds,HW] (or adds to it when accumulate) in gather form and ADDS
+ * fwd writes Ls.  bwd writes dsrc (src's shape and layout; or adds to it when accumulate) in gather form and ADDS
  * dWc[k,f] = sum keep dLs X / (1-p) into dWc through ordered per-CTA slots of `part`; the class-bias gradient is the
  * row sum of dLs (sx_rowsum).  No float atomics: two runs give the same bits. */
-enum { SX_HEAD_DMAP_NONE = 0, SX_HEAD_DMAP_INTERP = 1, SX_HEAD_DMAP_UNFOLD = 2 };
+enum { SX_HEAD_DMAP_NONE = 0, SX_HEAD_DMAP_INTERP = 1, SX_HEAD_DMAP_UNFOLD = 2, SX_HEAD_DMAP_UNFOLD_INTERLEAVED = 3 };
+enum { SX_HEAD_SRC_DEPTH_MAJOR = 0, SX_HEAD_SRC_SLICE_MAJOR = 1 };
 typedef struct {
   const float* src;
   int32_t B, Fs, Ds;
@@ -399,7 +405,7 @@ typedef struct {
   int32_t Dk;                    /* D_pool_K */
   int32_t dmap;                  /* SX_HEAD_DMAP_* */
   int32_t K;
-  int32_t _pad;
+  int32_t src_layout;            /* SX_HEAD_SRC_* */
   const float* Wc;
   const float* bc;
   float p;

@@ -18,7 +18,8 @@ SX_BIAS_NONE, SX_BIAS_N, SX_BIAS_M = 0, 1, 2
 SX_ACT_NONE, SX_ACT_GELU, SX_ACT_GELU_BWD = 0, 1, 2
 SX_SCHED_WARMUP_LINEAR, SX_SCHED_WARMUP_CONSTANT = 0, 1
 SX_CONSIST_BCE, SX_CONSIST_MARGIN = 0, 1
-SX_HEAD_DMAP_NONE, SX_HEAD_DMAP_INTERP, SX_HEAD_DMAP_UNFOLD = 0, 1, 2
+SX_HEAD_DMAP_NONE, SX_HEAD_DMAP_INTERP, SX_HEAD_DMAP_UNFOLD, SX_HEAD_DMAP_UNFOLD_INTERLEAVED = 0, 1, 2, 3
+SX_HEAD_SRC_DEPTH_MAJOR, SX_HEAD_SRC_SLICE_MAJOR = 0, 1
 SX_LABEL_U8, SX_LABEL_I16, SX_LABEL_I32, SX_LABEL_I64, SX_LABEL_F32 = 0, 1, 2, 3, 4
 
 
@@ -70,7 +71,7 @@ class sx_consist_args(C.Structure):
 
 class sx_head_dropout_args(C.Structure):
     _fields_ = [("src", C.c_void_p), ("B", C.c_int32), ("Fs", C.c_int32), ("Ds", C.c_int32), ("Fo", C.c_int32),
-                ("HW", C.c_int64), ("Dk", C.c_int32), ("dmap", C.c_int32), ("K", C.c_int32), ("_pad", C.c_int32),
+                ("HW", C.c_int64), ("Dk", C.c_int32), ("dmap", C.c_int32), ("K", C.c_int32), ("src_layout", C.c_int32),
                 ("Wc", C.c_void_p), ("bc", C.c_void_p), ("p", C.c_float), ("_pad2", C.c_uint32), ("seed", C.c_uint64),
                 ("seed_dev", C.c_void_p), ("part", C.c_void_p), ("part_floats", C.c_int64)]
 

@@ -3,10 +3,14 @@
 //
 //   Ls[b,k,v'] = bc[k] + sum_f Wc[k,f] keep(b,f,v') X[b,f,v'] / (1-p)          v' = (d', hw) on [D', H1*W1]
 //
-// X [B,F',D',HW] is formed on the fly from the source map Y [B,Fs,Ds,HW] by the depth map:
+// X [B,F',D',HW] is formed on the fly from the source map Y (element (b, fs, i, hw)) by the depth map:
 //   SX_HEAD_DMAP_NONE   X = Y                                   (F' = Fs, D' = Ds; the 2-D head passes Ds = 1)
 //   SX_HEAD_DMAP_INTERP X = linear(Y) along depth, D' = Dk Ds  (F.interpolate, align_corners=False: sx::src_index)
 //   SX_HEAD_DMAP_UNFOLD X[f, j Ds + i] = Y[f Dk + j, i]        (the reshape after out_fpn_upsampleD, F' = Fs / Dk)
+//   SX_HEAD_DMAP_UNFOLD_INTERLEAVED X[f, i Dk + j] = Y[f Dk + j, i]   (the 2.5-D model's reshape, segtran25d.py:357-362)
+// Y is depth-major [B,Fs,Ds,HW] (3-D and 2-D heads) or slice-major [B,Ds,Fs,HW] (the 2.5-D head, whose maps are
+// [B*Ds, Fs, H1, W1]); the layout is the template parameter SLICE, so the depth-major instantiations keep their
+// addressing: a source channel's base is src_chan() and its depth slices are `sD` floats apart.
 // keep() is sx::drop_keep1 at the flat index of the element in [B,F',D',HW], so the mask is the one a dropout over the
 // materialised map with the same counter-based hash would draw.
 //
@@ -36,8 +40,24 @@ struct DropGeom {
   const unsigned long long* seed_dev;
 };
 
+// offset of element (b, fs, 0, 0) of the source, and the distance between its depth slices
+template <int SLICE>
+__device__ __forceinline__ long long src_chan(const DropGeom& g, int b, int fs) {
+  if constexpr (SLICE) return ((long long)b * g.Ds * g.Fs + fs) * g.HW;
+  return ((long long)b * g.Fs + fs) * g.Ds * g.HW;
+}
+template <int SLICE>
+__device__ __forceinline__ long long src_dstride(const DropGeom& g) {
+  if constexpr (SLICE) return (long long)g.Fs * g.HW;
+  return g.HW;
+}
+
+__device__ __forceinline__ bool is_unfold(int dmap) {
+  return dmap == SX_HEAD_DMAP_UNFOLD || dmap == SX_HEAD_DMAP_UNFOLD_INTERLEAVED;
+}
+
 // one thread: VEC consecutive hw of one output depth plane; all classes of the chunk
-template <int VEC>
+template <int VEC, int SLICE>
 __global__ void __launch_bounds__(THREADS)
 head_dropout_fwd_kernel(DropGeom g, const float* __restrict__ Wc, const float* __restrict__ bc, int kc,
                         float* __restrict__ Ls, long long ls_bstride) {
@@ -61,21 +81,24 @@ head_dropout_fwd_kernel(DropGeom g, const float* __restrict__ Wc, const float* _
   float w1 = 0.f;
   if (g.dmap == SX_HEAD_DMAP_INTERP) sx::src_index(d, (float)g.Ds / (float)g.Do, g.Ds, i0, i1, w1);
   if (g.dmap == SX_HEAD_DMAP_UNFOLD) { jj = d / g.Ds; i0 = i1 = d - jj * g.Ds; }
+  if (g.dmap == SX_HEAD_DMAP_UNFOLD_INTERLEAVED) { i0 = i1 = d / g.Dk; jj = d - i0 * g.Dk; }
+  const bool unfold = is_unfold(g.dmap);
+  const long long sD = src_dstride<SLICE>(g);
   const float w0 = 1.f - w1;
   for (int f = 0; f < g.Fo; ++f) {
-    const int fs = g.dmap == SX_HEAD_DMAP_UNFOLD ? f * g.Dk + jj : f;
-    const float* s = g.src + ((long long)b * g.Fs + fs) * g.Ds * g.HW + hw;
+    const int fs = unfold ? f * g.Dk + jj : f;
+    const float* s = g.src + src_chan<SLICE>(g, b, fs) + hw;
     float x[VEC];
     if constexpr (VEC == 4) {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(s + (long long)i0 * g.HW));
+      const float4 a = __ldg(reinterpret_cast<const float4*>(s + (long long)i0 * sD));
       x[0] = a.x; x[1] = a.y; x[2] = a.z; x[3] = a.w;
       if (g.dmap == SX_HEAD_DMAP_INTERP) {
-        const float4 c = __ldg(reinterpret_cast<const float4*>(s + (long long)i1 * g.HW));
+        const float4 c = __ldg(reinterpret_cast<const float4*>(s + (long long)i1 * sD));
         x[0] = w0 * a.x + w1 * c.x; x[1] = w0 * a.y + w1 * c.y; x[2] = w0 * a.z + w1 * c.z; x[3] = w0 * a.w + w1 * c.w;
       }
     } else {
-      x[0] = __ldg(s + (long long)i0 * g.HW);
-      if (g.dmap == SX_HEAD_DMAP_INTERP) x[0] = w0 * x[0] + w1 * __ldg(s + (long long)i1 * g.HW);
+      x[0] = __ldg(s + (long long)i0 * sD);
+      if (g.dmap == SX_HEAD_DMAP_INTERP) x[0] = w0 * x[0] + w1 * __ldg(s + (long long)i1 * sD);
     }
     const unsigned long long base = (((unsigned long long)b * g.Fo + f) * g.Do + d) * (unsigned long long)g.HW + hw;
 #pragma unroll
@@ -99,9 +122,9 @@ head_dropout_fwd_kernel(DropGeom g, const float* __restrict__ Wc, const float* _
 }
 
 // one thread: VEC consecutive hw of one source depth slice i of batch b; walks every source channel.
-// Candidates t: the output planes d'_t that read slice i (interp: nonzero tap weight; unfold: d' = t Ds + i, only the
-// candidate t = fs % Dk is live for source channel fs; none: d' = i).
-template <int VEC, int TMAX>
+// Candidates t: the output planes d'_t that read slice i (interp: nonzero tap weight; unfold: d' = t Ds + i, interleaved
+// unfold: d' = i Dk + t, only the candidate t = fs % Dk is live for source channel fs; none: d' = i).
+template <int VEC, int TMAX, int SLICE>
 __global__ void __launch_bounds__(THREADS)
 head_dropout_bwd_kernel(DropGeom g, const float* __restrict__ Wc, int kc, const float* __restrict__ dLs,
                         long long dl_bstride, float* __restrict__ dsrc, int accumulate, float* __restrict__ part,
@@ -147,10 +170,10 @@ head_dropout_bwd_kernel(DropGeom g, const float* __restrict__ Wc, int kc, const 
         }
       }
     } else {
-      nt = g.dmap == SX_HEAD_DMAP_UNFOLD ? g.Dk : 1;
+      nt = is_unfold(g.dmap) ? g.Dk : 1;
 #pragma unroll
       for (int t = 0; t < TMAX; ++t) {
-        dc[t] = g.dmap == SX_HEAD_DMAP_UNFOLD ? t * g.Ds + i : i;
+        dc[t] = g.dmap == SX_HEAD_DMAP_UNFOLD ? t * g.Ds + i : (g.dmap == SX_HEAD_DMAP_UNFOLD_INTERLEAVED ? i * g.Dk + t : i);
         wt[t] = 1.f; own[t] = 1; oth[t] = i; wo0[t] = 1.f; wo1[t] = 0.f;
       }
     }
@@ -165,14 +188,17 @@ head_dropout_bwd_kernel(DropGeom g, const float* __restrict__ Wc, int kc, const 
                             ? __ldg(dLs + (long long)b * dl_bstride + (long long)k * Vo + (long long)dc[t] * g.HW + hw + v)
                             : 0.f;
 
+    const bool unfold = is_unfold(g.dmap);
+    const long long sD = src_dstride<SLICE>(g);
     for (int fs = 0; fs < g.Fs; ++fs) {
-      const int f = g.dmap == SX_HEAD_DMAP_UNFOLD ? fs / g.Dk : fs;
-      const int tsel = g.dmap == SX_HEAD_DMAP_UNFOLD ? fs - f * g.Dk : -1;
-      const float* s = g.src + ((long long)b * g.Fs + fs) * g.Ds * g.HW + hw;
+      const int f = unfold ? fs / g.Dk : fs;
+      const int tsel = unfold ? fs - f * g.Dk : -1;
+      const long long chan = src_chan<SLICE>(g, b, fs);
+      const float* s = g.src + chan + hw;
       float y[VEC], dy[VEC], cw[KC];
 #pragma unroll
       for (int v = 0; v < VEC; ++v) {
-        y[v] = live ? __ldg(s + (long long)i * g.HW + v) : 0.f;
+        y[v] = live ? __ldg(s + (long long)i * sD + v) : 0.f;
         dy[v] = 0.f;
       }
 #pragma unroll
@@ -187,7 +213,7 @@ head_dropout_bwd_kernel(DropGeom g, const float* __restrict__ Wc, int kc, const 
         if (own[t] && g.dmap == SX_HEAD_DMAP_INTERP) {
 #pragma unroll
           for (int v = 0; v < VEC; ++v)
-            xo[v] = wo0[t] * y[v] + wo1[t] * (live ? __ldg(s + (long long)oth[t] * g.HW + v) : 0.f);
+            xo[v] = wo0[t] * y[v] + wo1[t] * (live ? __ldg(s + (long long)oth[t] * sD + v) : 0.f);
         }
 #pragma unroll
         for (int v = 0; v < VEC; ++v) {
@@ -205,7 +231,7 @@ head_dropout_bwd_kernel(DropGeom g, const float* __restrict__ Wc, int kc, const 
         }
       }
       if (live) {
-        float* d = dsrc + ((long long)b * g.Fs + fs) * g.Ds * g.HW + (long long)i * g.HW + hw;
+        float* d = dsrc + chan + (long long)i * sD + hw;
 #pragma unroll
         for (int v = 0; v < VEC; ++v) d[v] = accumulate ? d[v] + dy[v] : dy[v];
       }
@@ -231,12 +257,15 @@ int check_args(const sx_head_dropout_args* a, const char* who) {
   SX_REQUIRE(a != nullptr && a->src && a->Wc, "%s: null pointer", who);
   SX_REQUIRE(a->B >= 1 && a->B <= 65535 && a->Fs >= 1 && a->Ds >= 1 && a->HW >= 1 && a->K >= 1 && a->Dk >= 1,
              "%s: bad shape", who);
-  SX_REQUIRE(a->dmap == SX_HEAD_DMAP_NONE || a->dmap == SX_HEAD_DMAP_INTERP || a->dmap == SX_HEAD_DMAP_UNFOLD,
+  SX_REQUIRE(a->dmap == SX_HEAD_DMAP_NONE || a->dmap == SX_HEAD_DMAP_INTERP || a->dmap == SX_HEAD_DMAP_UNFOLD ||
+                 a->dmap == SX_HEAD_DMAP_UNFOLD_INTERLEAVED,
              "%s: unknown depth map %d", who, a->dmap);
-  SX_REQUIRE(a->dmap != SX_HEAD_DMAP_UNFOLD || (a->Fs % a->Dk == 0 && a->Fo == a->Fs / a->Dk),
-             "%s: unfold needs Fs = F' * D_pool_K", who);
-  SX_REQUIRE(a->dmap == SX_HEAD_DMAP_UNFOLD || a->Fo == a->Fs, "%s: F' must equal the source channels", who);
-  SX_REQUIRE(a->dmap != SX_HEAD_DMAP_UNFOLD || a->Dk <= 8, "%s: unfold supports D_pool_K <= 8", who);
+  SX_REQUIRE(a->src_layout == SX_HEAD_SRC_DEPTH_MAJOR || a->src_layout == SX_HEAD_SRC_SLICE_MAJOR,
+             "%s: unknown source layout %d", who, a->src_layout);
+  const bool unfold = a->dmap == SX_HEAD_DMAP_UNFOLD || a->dmap == SX_HEAD_DMAP_UNFOLD_INTERLEAVED;
+  SX_REQUIRE(!unfold || (a->Fs % a->Dk == 0 && a->Fo == a->Fs / a->Dk), "%s: unfold needs Fs = F' * D_pool_K", who);
+  SX_REQUIRE(unfold || a->Fo == a->Fs, "%s: F' must equal the source channels", who);
+  SX_REQUIRE(!unfold || a->Dk <= 8, "%s: unfold supports D_pool_K <= 8", who);
   SX_REQUIRE(a->dmap != SX_HEAD_DMAP_INTERP || a->Dk <= 4, "%s: interp supports D_pool_K <= 4", who);
   SX_REQUIRE(a->p >= 0.f && a->p < 1.f, "%s: dropout probability %g not in [0, 1)", who, (double)a->p);
   SX_REQUIRE((size_t)5 * KC * a->Fo * 4 <= 200 * 1024, "%s: F'=%d too large", who, a->Fo);
@@ -266,6 +295,17 @@ cudaError_t allow_smem(Kern k, size_t bytes) {
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
+template <int VEC, int SLICE>
+static int launch_fwd(const DropGeom& g, const float* W, const float* bc, int kc, float* out, int K, int B, size_t smem,
+                      cudaStream_t st) {
+  const long long Vo = (long long)g.Do * g.HW;
+  SX_CHECK_CUDA(allow_smem(head_dropout_fwd_kernel<VEC, SLICE>, smem));
+  dim3 grid(sx_ceil_div(Vo, THREADS * VEC), B);
+  head_dropout_fwd_kernel<VEC, SLICE><<<grid, THREADS, smem, st>>>(g, W, bc, kc, out, (long long)K * Vo);
+  SX_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
 extern "C" int sx_head_dropout_fwd(const sx_head_dropout_args* a, float* Ls, void* stream) {
   if (int rc = check_args(a, "sx_head_dropout_fwd")) return rc;
   SX_REQUIRE(Ls, "sx_head_dropout_fwd: null output");
@@ -278,21 +318,17 @@ extern "C" int sx_head_dropout_fwd(const sx_head_dropout_args* a, float* Ls, voi
     const float* W = a->Wc + (long long)c0 * g.Fo;
     const float* bc = a->bc ? a->bc + c0 : nullptr;
     float* out = Ls + (long long)c0 * Vo;
-    if (vec4) {
-      SX_CHECK_CUDA(allow_smem(head_dropout_fwd_kernel<4>, smem));
-      dim3 grid(sx_ceil_div(Vo, THREADS * 4), a->B);
-      head_dropout_fwd_kernel<4><<<grid, THREADS, smem, ST(stream)>>>(g, W, bc, kc, out, (long long)a->K * Vo);
-    } else {
-      SX_CHECK_CUDA(allow_smem(head_dropout_fwd_kernel<1>, smem));
-      dim3 grid(sx_ceil_div(Vo, THREADS), a->B);
-      head_dropout_fwd_kernel<1><<<grid, THREADS, smem, ST(stream)>>>(g, W, bc, kc, out, (long long)a->K * Vo);
-    }
-    SX_CHECK_CUDA(cudaGetLastError());
+    const bool slice = a->src_layout == SX_HEAD_SRC_SLICE_MAJOR;
+    if (int rc = vec4 ? (slice ? launch_fwd<4, 1>(g, W, bc, kc, out, a->K, a->B, smem, ST(stream))
+                               : launch_fwd<4, 0>(g, W, bc, kc, out, a->K, a->B, smem, ST(stream)))
+                      : (slice ? launch_fwd<1, 1>(g, W, bc, kc, out, a->K, a->B, smem, ST(stream))
+                               : launch_fwd<1, 0>(g, W, bc, kc, out, a->K, a->B, smem, ST(stream))))
+      return rc;
   }
   return 0;
 }
 
-template <int VEC, int TMAX>
+template <int VEC, int TMAX, int SLICE>
 static int launch_bwd(const DropGeom& g, const sx_head_dropout_args* a, const float* dLs, float* dsrc, int accumulate,
                       float* dWc, cudaStream_t st) {
   const long long Vo = (long long)g.Do * g.HW;
@@ -306,8 +342,8 @@ static int launch_bwd(const DropGeom& g, const sx_head_dropout_args* a, const fl
     const long long slots = a->part_floats / ((long long)kc * g.Fo);
     const int grid = (int)std::min<long long>({tiles, (long long)sms * 4, slots});
     SX_REQUIRE(grid >= 1, "sx_head_dropout_bwd: needs at least %d floats of scratch", kc * g.Fo);
-    SX_CHECK_CUDA(allow_smem(head_dropout_bwd_kernel<VEC, TMAX>, smem));
-    head_dropout_bwd_kernel<VEC, TMAX><<<grid, THREADS, smem, st>>>(
+    SX_CHECK_CUDA(allow_smem(head_dropout_bwd_kernel<VEC, TMAX, SLICE>, smem));
+    head_dropout_bwd_kernel<VEC, TMAX, SLICE><<<grid, THREADS, smem, st>>>(
         g, a->Wc + (long long)c0 * g.Fo, kc, dLs + (long long)c0 * Vo, (long long)a->K * Vo, dsrc,
         (accumulate || c0 > 0) ? 1 : 0, a->part, tps, tiles);
     SX_CHECK_CUDA(cudaGetLastError());
@@ -318,6 +354,17 @@ static int launch_bwd(const DropGeom& g, const sx_head_dropout_args* a, const fl
   return 0;
 }
 
+template <int SLICE>
+static int dispatch_bwd(const DropGeom& g, const sx_head_dropout_args* a, const float* dLs, float* dsrc, int accumulate,
+                        float* dWc, int need, bool vec2, cudaStream_t st) {
+  if (need <= 1) return vec2 ? launch_bwd<2, 1, SLICE>(g, a, dLs, dsrc, accumulate, dWc, st)
+                             : launch_bwd<1, 1, SLICE>(g, a, dLs, dsrc, accumulate, dWc, st);
+  if (need <= 6) return vec2 ? launch_bwd<2, 6, SLICE>(g, a, dLs, dsrc, accumulate, dWc, st)
+                             : launch_bwd<1, 6, SLICE>(g, a, dLs, dsrc, accumulate, dWc, st);
+  return vec2 ? launch_bwd<2, 10, SLICE>(g, a, dLs, dsrc, accumulate, dWc, st)
+              : launch_bwd<1, 10, SLICE>(g, a, dLs, dsrc, accumulate, dWc, st);
+}
+
 extern "C" int sx_head_dropout_bwd(const sx_head_dropout_args* a, const float* dLs, float* dsrc, int32_t accumulate,
                                    float* dWc, void* stream) {
   if (int rc = check_args(a, "sx_head_dropout_bwd")) return rc;
@@ -326,12 +373,11 @@ extern "C" int sx_head_dropout_bwd(const sx_head_dropout_args* a, const float* d
   const bool vec2 = g.HW % 2 == 0 && ((reinterpret_cast<uintptr_t>(a->src) | reinterpret_cast<uintptr_t>(dLs) |
                                        reinterpret_cast<uintptr_t>(dsrc)) & 7) == 0;
   // live candidate planes per source slice: 1 (none), D_pool_K (unfold), up to 2 D_pool_K + 1 (interp, first taps too)
-  const int need = a->dmap == SX_HEAD_DMAP_NONE ? 1 : (a->dmap == SX_HEAD_DMAP_UNFOLD ? a->Dk : 2 * a->Dk + 2);
+  const int need = a->dmap == SX_HEAD_DMAP_NONE
+                       ? 1
+                       : ((a->dmap == SX_HEAD_DMAP_UNFOLD || a->dmap == SX_HEAD_DMAP_UNFOLD_INTERLEAVED) ? a->Dk
+                                                                                                       : 2 * a->Dk + 2);
   cudaStream_t st = ST(stream);
-  if (need <= 1) return vec2 ? launch_bwd<2, 1>(g, a, dLs, dsrc, accumulate, dWc, st)
-                             : launch_bwd<1, 1>(g, a, dLs, dsrc, accumulate, dWc, st);
-  if (need <= 6) return vec2 ? launch_bwd<2, 6>(g, a, dLs, dsrc, accumulate, dWc, st)
-                             : launch_bwd<1, 6>(g, a, dLs, dsrc, accumulate, dWc, st);
-  return vec2 ? launch_bwd<2, 10>(g, a, dLs, dsrc, accumulate, dWc, st)
-              : launch_bwd<1, 10>(g, a, dLs, dsrc, accumulate, dWc, st);
+  if (a->src_layout == SX_HEAD_SRC_SLICE_MAJOR) return dispatch_bwd<1>(g, a, dLs, dsrc, accumulate, dWc, need, vec2, st);
+  return dispatch_bwd<0>(g, a, dLs, dsrc, accumulate, dWc, need, vec2, st);
 }

@@ -12,14 +12,19 @@ for Conv3d + GroupNorm and builds the full out-FPN map before its class conv; he
     (sx_groupnorm_slices_fwd/bwd).  Without the fused path (BatchNorm, unaligned pitches, fusion off) the stock modules
     run on a permuted [B,C,h,w,D2] view.
   * head: the collapsed form (ops.seg_head_slices) — the bridged out-FPN map is never built; with out_fpn_layers ==
-    in_fpn_layers the ConvTranspose3d (2,2,1) direct head (ops.direct_head(token_order='hwd')).
+    in_fpn_layers the ConvTranspose3d (2,2,1) direct head (ops.direct_head(token_order='hwd')).  Training with
+    ``--outdrop`` runs the dropout head on the slice-major map (ops.seg_head_slices_dropout, csrc/sx_head_drop.cu): the
+    dropped, depth-upsampled map is never written.  With out_fpn_layers == in_fpn_layers ``--outdrop`` does nothing, as
+    in the reference.
 
 Deliberate deviations from the reference:
   * the fusion encoder is called with orig_feat_shape = (H2, W2, D3); the reference passes three arguments to a
     four-argument forward (segtran25d.py:457) and cannot run;
   * positions and scales are built on the input's device, not a 'cuda' literal (:448);
   * an input size that is not an integer multiple of the token grid raises ValueError instead of breakpoint() (:436-437);
-  * ``--outdrop`` in training raises NotImplementedError (in evaluation the dropout is the identity, as in the reference).
+  * the ``--outdrop`` mask comes from the library's counter-based generator (seeded per call on the device), so
+    ``torch.manual_seed`` does not select it; training with ``--outdrop`` on host tensors raises NotImplementedError
+    before any work (the dropout head is CUDA only).
 ``out_fpn_upsampleD_scheme`` follows the reference's branches (:355-371): 'conv' unfolds depth, 'interpolate' is linear
 x D_pool_K, and any other value, including the drivers' default 'interp', leaves the depth at D2.
 """
@@ -252,9 +257,6 @@ class Segtran25d(SegtranInitWeights):
         voxel-wise head (reference segtran25d.py:290-315, :351-377, :425-477 minus the FPN pyramids).
         feat_fpn [B, D2, C0, H2, W2] (the slice-major in-FPN output viewed per sample); curr_feat [B*D2, Cf, H1, W1]
         (ignored, may be None, without the out-FPN); vmask [B, D2, H2, W2] per-slice mask or None; out_size = (H,W,D)."""
-        if self.do_out_fpn and self.out_fpn_do_dropout and self.training:
-            raise NotImplementedError("segtran_b200: --outdrop (out_fpn_do_dropout) in training is not supported by "
-                                      "Segtran25d; the dropout head reads depth-major maps")
         B, D2, C0, H2, W2 = feat_fpn.shape
         H, W, D = out_size
         D3 = D2 // self.D_pool_K
@@ -262,6 +264,10 @@ class Segtran25d(SegtranInitWeights):
         sH, sW, sD = H // H2, W // W2, D // max(D3, 1)
         if D3 < 1 or sH * H2 != H or sW * W2 != W or sD * D3 != D:
             raise ValueError("input size %s is not an integer multiple of the token grid %s" % ((H, W, D), tuple(grid)))
+        drop = self.do_out_fpn and self.out_fpn_do_dropout and self.training
+        if drop and not feat_fpn.is_cuda:                     # checked before any work: the head has no host version
+            raise NotImplementedError("segtran_b200: --outdrop (out_fpn_do_dropout) in training runs on the CUDA "
+                                      "dropout head (csrc/sx_head_drop.cu) only; got %s tensors" % feat_fpn.device)
         HW, X = H2 * W2, C0 * H2 * W2
         # depth pooling on the [B, D2, C0*H2*W2] view, then [B, D3*C0, H2*W2] -> [B, H2*W2, D3*C0] = tokens in (h,w,d)
         pooled = ops.resize_linear(feat_fpn.reshape(B, D2, X), (D3, X))
@@ -294,6 +300,12 @@ class Segtran25d(SegtranInitWeights):
             return ops.direct_head(fused, tuple(grid), self.out_conv3d.weight, self.out_conv3d.bias, out_size,
                                    token_order='hwd')
         bridge, cls = self.out_fpn_bridgeconv3d, self.out_conv3d
+        if drop:                                              # per-channel mask: the dropout head (sx_head_drop.cu)
+            ud = self.out_fpn_upsampleD if unfold else None
+            return ops.seg_head_slices_dropout(curr_feat, fused, tuple(grid), bridge.weight, bridge.bias, cls.weight,
+                                               cls.bias, out_size, self.out_fpn_dropout.p, self.D_pool_K,
+                                               self.out_fpn_upsampleD_scheme, Wu=None if ud is None else ud.weight,
+                                               bu=None if ud is None else ud.bias)
         if unfold:
             ud = self.out_fpn_upsampleD
             Wc, bc = ops.fold_unfold(cls.weight, cls.bias, ud.weight, ud.bias, self.D_pool_K)

@@ -2185,41 +2185,54 @@ def direct_head(fused, grid, Wt, bt, out_size, token_order="dhw"):
     return _SubpixelResize.apply(S, bt, grid, tuple(int(s) for s in out_size))
 
 
+def _src_dims(src, layout):
+    """(B, Fs, Ds, HW) of a dropout-head source: [B,Fs,Ds,HW] depth-major or [B,Ds,Fs,HW] slice-major."""
+    if layout == L.SX_HEAD_SRC_SLICE_MAJOR:
+        B, Ds, Fs, HW = src.shape
+    else:
+        B, Fs, Ds, HW = src.shape
+    return B, Fs, Ds, HW
+
+
 class _HeadDropout(torch.autograd.Function):
     """Class scores of the dropped out-FPN map (csrc/sx_head_drop.cu), the map itself never written:
         Ls[b,k,d',hw] = bc[k] + sum_f Wc[k,f] keep(b,f,d',hw) X[b,f,d',hw] / (1-p)
-    src [B,Fs,Ds,HW] is the map before the depth upsampling (Y, or Y2 = out_fpn_upsampleD(Y) for --upd conv); X is src
-    through the depth map (none / interp x Dk / unfold).  The mask is regenerated in backward from the saved seed."""
+    src is the map before the depth upsampling (Y, or Y2 = out_fpn_upsampleD(Y) for --upd conv), [B,Fs,Ds,HW] with
+    layout SX_HEAD_SRC_DEPTH_MAJOR or [B,Ds,Fs,HW] with SX_HEAD_SRC_SLICE_MAJOR (the 2.5-D model); X is src through the
+    depth map (none / interp x Dk / unfold / interleaved unfold).  The mask is regenerated in backward from the saved
+    seed."""
 
     @staticmethod
-    def forward(ctx, src, Wc, bc, p, seed, dmap, Dk):
+    def forward(ctx, src, Wc, bc, p, seed, dmap, Dk, layout=L.SX_HEAD_SRC_DEPTH_MAJOR):
         src = src.contiguous()
         Wc = Wc.contiguous()
-        B, Fs, Ds, HW = src.shape
+        B, Fs, Ds, HW = _src_dims(src, layout)
         K, Fo = Wc.shape
         Do = Ds if dmap == L.SX_HEAD_DMAP_NONE else Ds * Dk
         sv, sp = _seed_args(seed)
         a = L.sx_head_dropout_args()
         a.src, a.B, a.Fs, a.Ds, a.Fo, a.HW, a.Dk, a.dmap, a.K = src.data_ptr(), B, Fs, Ds, Fo, HW, Dk, dmap, K
+        a.src_layout = layout
         a.Wc, a.bc, a.p, a.seed, a.seed_dev = Wc.data_ptr(), _ptr(bc), float(p), sv, sp
         a.part, a.part_floats = _part_args(src.device)
         Ls = torch.empty((B, K, Do, HW), device=src.device, dtype=torch.float32)
         L.call("sx_head_dropout_fwd", C.byref(a), Ls.data_ptr(), _stream())
         ctx.save_for_backward(src, Wc)
-        ctx.meta = (float(p), seed, dmap, Dk, bc is not None)
+        ctx.meta = (float(p), seed, dmap, Dk, bc is not None, layout)
         return Ls
 
     @staticmethod
     def backward(ctx, dLs):
         src, Wc = ctx.saved_tensors
-        p, seed, dmap, Dk, has_bc = ctx.meta
-        B, Fs, Ds, HW = src.shape
+        p, seed, dmap, Dk, has_bc, layout = ctx.meta
+        B, Fs, Ds, HW = _src_dims(src, layout)
         K, Fo = Wc.shape
         dLs = dLs.contiguous()
         dev = src.device
         sv, sp = _seed_args(seed)
         a = L.sx_head_dropout_args()
         a.src, a.B, a.Fs, a.Ds, a.Fo, a.HW, a.Dk, a.dmap, a.K = src.data_ptr(), B, Fs, Ds, Fo, HW, Dk, dmap, K
+        a.src_layout = layout
         a.Wc, a.bc, a.p, a.seed, a.seed_dev = Wc.data_ptr(), None, p, sv, sp
         a.part, a.part_floats = _part_args(dev)
         dsrc = torch.empty_like(src)
@@ -2230,7 +2243,7 @@ class _HeadDropout(torch.autograd.Function):
             dbc = _zeros((K,), dev)
             V = dLs.shape[2] * HW
             L.call("sx_rowsum", dLs.data_ptr(), B * K, V, V, K, dbc.data_ptr(), *_part_args(dev), _stream())
-        return dsrc, dWc, dbc, None, None, None, None
+        return dsrc, dWc, dbc, None, None, None, None, None
 
 
 def seg_head_dropout(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, p, d_pool_k=1, upsample_d="interp", Wu=None,
@@ -2261,6 +2274,67 @@ def seg_head_dropout(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, p, d_poo
     src = Y.reshape(B, Y.shape[1], Ds, HW)
     Ls = _HeadDropout.apply(src, Wc.reshape(K, -1), bc, float(p), seed, dmap, Dk)
     return _head_out(Ls.view(B, K, Ls.shape[2], *sp1[-2:]) if len(sp1) == 3 else Ls.view(B, K, *sp1), out_size)
+
+
+def seg_head_slices_dropout(curr, vfeat_fused, grid, Wb, bb, Wc, bc, out_size, p, d_pool_k, upsample_d, Wu=None,
+                            bu=None, seed=None):
+    """Voxel-wise head of the 2.5-D model with dropout on the out-FPN map (training with --outdrop; segtran25d.py:
+    351-377, :464-477), on slice-major maps.  curr [B*D2, Cf, H1, W1] (slice b*D2 + d); vfeat_fused [B, N, F] tokens in
+    (h, w, d) order on grid = (H2, W2, D3); Wb/bb the bridge conv; Wc/bc the class conv; Wu/bu out_fpn_upsampleD (used
+    with upsample_d='conv' and d_pool_k > 1); out_size = (H, W, D) -> logits [B, K, H, W, D].
+    The tokens' addend is built slice-major from the small tensor (depth D3 -> D2, one transpose to [B, D2, F, H2*W2],
+    bilinear per slice: trilinear interpolation is separable), so Y = Wb curr + bb + up(vfeat) (and Y2 = Wu Y + bu) come
+    out as [B*D2, F, H1, W1] and no full-size map is permuted.  Depth map: 'conv' unfolds channel f*Dk + j of slice i to
+    depth i*Dk + j, 'interpolate' is linear x Dk, any other scheme (the drivers' default 'interp', 'none') or
+    d_pool_k = 1 keeps D2.  The dropped, depth-upsampled map only exists inside _HeadDropout.  seed: None draws a
+    per-call device seed (a new mask on every call and every CUDA-graph replay); an int or an int64 device tensor fixes
+    it."""
+    if curr.dim() != 4 or vfeat_fused.dim() != 3:
+        raise ValueError("seg_head_slices_dropout: curr [B*D2, Cf, H1, W1] and vfeat_fused [B, N, F] expected, got %s "
+                         "and %s" % (tuple(curr.shape), tuple(vfeat_fused.shape)))
+    BD, Cf, H1, W1 = (int(s) for s in curr.shape)
+    B, N, Fd = (int(s) for s in vfeat_fused.shape)
+    H2, W2, D3 = (int(g) for g in grid)
+    if B < 1 or BD % B:
+        raise ValueError("seg_head_slices_dropout: %d slices are not a multiple of the batch %d" % (BD, B))
+    if H2 * W2 * D3 != N:
+        raise ValueError("seg_head_slices_dropout: grid %s does not hold %d tokens" % ((H2, W2, D3), N))
+    if not 0.0 <= float(p) < 1.0:
+        raise ValueError("seg_head_slices_dropout: dropout probability %g not in [0, 1)" % float(p))
+    if len(tuple(out_size)) != 3:
+        raise ValueError("seg_head_slices_dropout: out_size must be (H, W, D), got %s" % (tuple(out_size),))
+    D2, HW, K, Dk = BD // B, H1 * W1, int(Wc.shape[0]), int(d_pool_k)
+    if Dk < 1:
+        raise ValueError("seg_head_slices_dropout: d_pool_k must be >= 1, got %d" % Dk)
+    conv = upsample_d == "conv" and Dk > 1
+    if conv:
+        if Wu is None:
+            raise ValueError("seg_head_slices_dropout: upsample_d='conv' needs out_fpn_upsampleD's weight Wu")
+        if Wu.shape[0] % Dk or Wc.reshape(K, -1).shape[1] * Dk != Wu.shape[0]:
+            raise ValueError("seg_head_slices_dropout: Wu has %d output channels; the class conv reads %d x D_pool_K %d"
+                             % (Wu.shape[0], Wc.reshape(K, -1).shape[1], Dk))
+    elif Wc.reshape(K, -1).shape[1] != Fd:
+        raise ValueError("seg_head_slices_dropout: the class conv reads %d channels, the map has %d"
+                         % (Wc.reshape(K, -1).shape[1], Fd))
+    _req_cuda(curr, vfeat_fused)
+    t = resize_linear(vfeat_fused.reshape(B, H2 * W2, D3, Fd), (D2, Fd))                  # [B, H2*W2, D2, F]
+    t = transpose(t.view(B, H2 * W2, D2 * Fd)).view(BD, Fd, H2, W2)                      # [B*D2, F, H2, W2]
+    up = resize_linear(t, (H1, W1))
+    Y = conv1x1_add(curr, Wb, bb, addend=up)                                             # [B*D2, F, H1, W1]
+    del up, t
+    if conv:
+        Y = conv1x1_add(Y, Wu, bu)
+        dmap = L.SX_HEAD_DMAP_UNFOLD_INTERLEAVED
+    elif Dk > 1 and upsample_d == "interpolate":
+        dmap = L.SX_HEAD_DMAP_INTERP
+    else:
+        dmap, Dk = L.SX_HEAD_DMAP_NONE, 1
+    if seed is None:
+        seed = new_dropout_seed(curr.device)
+    src = Y.view(B, D2, Y.shape[1], HW)
+    del Y
+    Ls = _HeadDropout.apply(src, Wc.reshape(K, -1), bc, float(p), seed, dmap, Dk, L.SX_HEAD_SRC_SLICE_MAJOR)
+    return _head_out(Ls.view(B, K, Ls.shape[2], H1, W1), out_size)
 
 
 # ------------------------------------------------------------------------------------------------
