@@ -500,20 +500,28 @@ int sx_sgemm_small(const float* A, const float* B, float* C, int32_t M, int32_t 
 
 /* -------------------------------------------------------------------------------------------
  * Sliding-window inference post-process (SURVEY.md section 8 row f.4; code/test_util3d.py:93-184):
- * sx_sw_accumulate: preds[k][window] += sigmoid(scores[k]), cnt[window] += 1 for one patch ([K][dx][dy][dz] scores, window
- *   origin (x0,y0,z0) in the [K][H][W][D] accumulators)                                              (test_util3d.py:155-159)
+ * Mirror masks (test-time augmentation): bit 0 reverses the window's H axis (dx), bit 1 W (dy), bit 2 D (dz).
+ * sx_sw_accumulate: preds[k][window] += sigmoid(flip_mirror(scores)[k]), cnt[window] += 1 for one patch ([K][dx][dy][dz]
+ *   scores, window origin (x0,y0,z0) in the [K][H][W][D] accumulators; the scores are read through reversed indices, and
+ *   mirror 0 is the plain update)                                                                     (test_util3d.py:155-159)
  * sx_sw_finalize: preds /= cnt; brats: make_brats_pred_consistent(is_conservative=False) (datasets3d.py:53-59), hard[1:] =
  *   preds >= 0.5, hard[0] = no class fired (hard is [K][V]); otherwise hard[0..V) = argmax_k as a float class index.
+ * sx_sw_gather: out[w][b] = flip_mirror(img[b][:, x0_w:x0_w+dx, y0_w:y0_w+dy, z0_w:z0_w+dz]) for the n windows whose
+ *   origins are the HOST array origins[3n] (x0, y0, z0 each), from the contiguous fp32 [B][C][H][W][D] image into the
+ *   contiguous [n][B][C][dx][dy][dz] out.  A 2-D batch [B][C][H][W] is D = dz = 1.
  * ------------------------------------------------------------------------------------------- */
 int sx_sw_accumulate(const float* scores, int32_t K, int32_t dx, int32_t dy, int32_t dz, float* preds, float* cnt,
-                     int32_t H, int32_t W, int32_t D, int32_t x0, int32_t y0, int32_t z0, void* stream);
+                     int32_t H, int32_t W, int32_t D, int32_t x0, int32_t y0, int32_t z0, int32_t mirror, void* stream);
 int sx_sw_finalize(float* preds, const float* cnt, int32_t K, int64_t V, int32_t brats, float* hard, void* stream);
+int sx_sw_gather(const float* img, int32_t B, int32_t C, int32_t H, int32_t W, int32_t D, const int32_t* origins, int32_t n,
+                 int32_t dx, int32_t dy, int32_t dz, int32_t mirror, float* out, void* stream);
 
 /* -------------------------------------------------------------------------------------------
  * 2-D sliding-window inference and per-image evaluation (csrc/sx_eval2d.cu; code/test_util2d.py:169-265, harden_segmap2d
  * of dataloaders/datasets2d.py:178-196, calc_vcdr of utils/losses.py:76-127).  Bilinear resizes use align_corners=False.
  * sx_sw2d_accumulate: for one window at (xs, ys) of the [B][K][H2][W2] accumulator, preds += sigmoid(scores bilinearly
- *   resized from [B][K][h][w] to dx x dy) and the shared [H2][W2] cnt += 1; the resized scores are never written.
+ *   resized from [B][K][h][w] to dx x dy) and the shared [H2][W2] cnt += 1; the resized scores are never written.  With
+ *   mirror bit 0 (1) set the scores' h (w) axis is reversed before the resize, by reversing the source taps.
  * sx_sw2d_finalize: soft = preds / cnt cropped to [B][K][H][W] at (hl, wl); hard (int32, same shape): class k >= 1 is
  *   soft >= 0.5, class 0 is "no class >= 1 fired".
  * sx_eval2d_counts: per image b, the [K][h][w] soft prediction bilinearly resized to the [K][Hg][Wg] ground truth and
@@ -524,7 +532,7 @@ int sx_sw_finalize(float* preds, const float* cnt, int32_t K, int64_t V, int32_t
  *   2 <= K <= 8.  Integer atomics only: the counts do not depend on scheduling.
  * ------------------------------------------------------------------------------------------- */
 int sx_sw2d_accumulate(const float* scores, int32_t B, int32_t K, int32_t h, int32_t w, int32_t dx, int32_t dy, float* preds,
-                       float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, void* stream);
+                       float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, int32_t mirror, void* stream);
 int sx_sw2d_finalize(const float* preds, const float* cnt, int32_t B, int32_t K, int32_t H2, int32_t W2, int32_t hl,
                      int32_t wl, int32_t H, int32_t W, float* soft, int32_t* hard, void* stream);
 int sx_eval2d_counts(const float* pred, int32_t B, int32_t K, int32_t h, int32_t w, const float* gt, int32_t Hg, int32_t Wg,

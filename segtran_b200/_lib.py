@@ -115,9 +115,10 @@ _PROTOS = {
     "sx_seed_derive": [_P, _U64, _P, _P],
     "sx_seed_advance": [_P, _U64, _P],
     "sx_convert": [_P, _I, _L, _P, _I, _I, _P],
-    "sx_sw_accumulate": [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P],
+    "sx_sw_accumulate": [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
     "sx_sw_finalize": [_P, _P, _I, _L, _I, _P, _P],
-    "sx_sw2d_accumulate": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P],
+    "sx_sw_gather": [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P],
+    "sx_sw2d_accumulate": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _P],
     "sx_sw2d_finalize": [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P],
     "sx_eval2d_counts": [_P, _I, _I, _I, _I, _P, _I, _I, _P, _P],
     "sx_mask_counts": [_P, _P, _I, _L, _P, _L, _P],

@@ -27,9 +27,11 @@ __device__ __forceinline__ float bilerp(const float* __restrict__ p, int w, int 
          wy * (hx * __ldg(p + (long long)y1 * w + x0) + wx * __ldg(p + (long long)y1 * w + x1));
 }
 
-// preds[b][k][xs+i][ys+j] += sigmoid(upsample(scores[b][k])[i][j]);  cnt[xs+i][ys+j] += 1     (test_util2d.py:209-214)
+// preds[b][k][xs+i][ys+j] += sigmoid(upsample(flip_m(scores[b][k]))[i][j]);  cnt[xs+i][ys+j] += 1   (test_util2d.py:209-214)
+// mirror bit 0 reverses the h axis, bit 1 the w axis: the flip is applied to the source taps, before the upsample.
 __global__ void sw2d_accumulate_kernel(const float* __restrict__ scores, int B, int K, int h, int w, int dx, int dy,
-                                       float* __restrict__ preds, float* __restrict__ cnt, int H2, int W2, int xs, int ys) {
+                                       float* __restrict__ preds, float* __restrict__ cnt, int H2, int W2, int xs, int ys,
+                                       int mirror) {
   const long long pw = (long long)dx * dy;
   const long long total = (long long)B * pw;
   const float ry = (float)h / (float)dx, rx = (float)w / (float)dy;
@@ -42,6 +44,8 @@ __global__ void sw2d_accumulate_kernel(const float* __restrict__ scores, int B, 
     float wy, wx;
     sx::src_index(i, ry, h, y0, y1, wy);
     sx::src_index(j, rx, w, x0, x1, wx);
+    if (mirror & 1) { y0 = h - 1 - y0; y1 = h - 1 - y1; }
+    if (mirror & 2) { x0 = w - 1 - x0; x1 = w - 1 - x1; }
     const long long o = (long long)(xs + i) * W2 + (ys + j);
     for (int k = 0; k < K; ++k) {
       const long long bk = (long long)b * K + k;
@@ -179,13 +183,15 @@ int grid_for(long long work, int per_launch_cap) {
 }  // namespace
 
 extern "C" int sx_sw2d_accumulate(const float* scores, int32_t B, int32_t K, int32_t h, int32_t w, int32_t dx, int32_t dy,
-                                  float* preds, float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, void* stream) {
+                                  float* preds, float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, int32_t mirror,
+                                  void* stream) {
   SX_REQUIRE(B > 0 && K > 0 && h > 0 && w > 0 && dx > 0 && dy > 0 && xs >= 0 && ys >= 0 && xs + dx <= H2 && ys + dy <= W2,
              "sx_sw2d_accumulate: window [%d+%d, %d+%d] outside the %dx%d image, or empty scores (%dx%d)", xs, dx, ys, dy, H2, W2,
              h, w);
+  SX_REQUIRE(mirror >= 0 && mirror <= 3, "sx_sw2d_accumulate: mirror mask %d is not a subset of {H, W} (0..3)", mirror);
   const int blocks = grid_for((long long)B * dx * dy, sm_count_cached() * 8);
   sw2d_accumulate_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(scores, B, K, h, w, dx, dy, preds, cnt,
-                                                                                     H2, W2, xs, ys);
+                                                                                     H2, W2, xs, ys, mirror);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
