@@ -118,6 +118,7 @@ _PROTOS = {
     "sx_sw_accumulate": [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
     "sx_sw_finalize": [_P, _P, _I, _L, _I, _P, _P],
     "sx_sw_gather": [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P],
+    "sx_sw_set_weights": [_P, _I, _P, _I, _P, _I],
     "sx_sw2d_accumulate": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _P],
     "sx_sw2d_finalize": [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P],
     "sx_eval2d_counts": [_P, _I, _I, _I, _I, _P, _I, _I, _P, _P],
@@ -192,7 +193,7 @@ def check(rc, what):
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
 _LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0, "sx_gemm_set_tout": 0,
-             "sx_attn_probs_fwd": 2, "sx_colsum_batched": 2, "sx_dot": 2, "sx_head_contract_bwd_weight": 2,
+             "sx_sw_set_weights": 0, "sx_attn_probs_fwd": 2, "sx_colsum_batched": 2, "sx_dot": 2, "sx_head_contract_bwd_weight": 2,
              "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2, "sx_head_dropout_bwd": 2, "sx_edt_sq": 3}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing

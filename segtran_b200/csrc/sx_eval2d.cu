@@ -29,9 +29,12 @@ __device__ __forceinline__ float bilerp(const float* __restrict__ p, int w, int 
 
 // preds[b][k][xs+i][ys+j] += sigmoid(upsample(flip_m(scores[b][k]))[i][j]);  cnt[xs+i][ys+j] += 1   (test_util2d.py:209-214)
 // mirror bit 0 reverses the h axis, bit 1 the w axis: the flip is applied to the source taps, before the upsample.
+// kWeighted: both terms are scaled by g = max(tx[i] * ty[j], 1e-3), the window weight at the upsampled position (i, j);
+// the weight tables are the trailing arguments, which the unweighted instantiation never reads.
+template <bool kWeighted>
 __global__ void sw2d_accumulate_kernel(const float* __restrict__ scores, int B, int K, int h, int w, int dx, int dy,
                                        float* __restrict__ preds, float* __restrict__ cnt, int H2, int W2, int xs, int ys,
-                                       int mirror) {
+                                       int mirror, const float* __restrict__ tx, const float* __restrict__ ty) {
   const long long pw = (long long)dx * dy;
   const long long total = (long long)B * pw;
   const float ry = (float)h / (float)dx, rx = (float)w / (float)dy;
@@ -47,12 +50,22 @@ __global__ void sw2d_accumulate_kernel(const float* __restrict__ scores, int B, 
     if (mirror & 1) { y0 = h - 1 - y0; y1 = h - 1 - y1; }
     if (mirror & 2) { x0 = w - 1 - x0; x1 = w - 1 - x1; }
     const long long o = (long long)(xs + i) * W2 + (ys + j);
-    for (int k = 0; k < K; ++k) {
-      const long long bk = (long long)b * K + k;
-      const float s = bilerp(scores + bk * plane_in, w, y0, y1, wy, x0, x1, wx);
-      preds[bk * plane_out + o] += 1.f / (1.f + expf(-s));     // torch.sigmoid
+    if constexpr (kWeighted) {
+      const float g = fmaxf(__ldg(tx + i) * __ldg(ty + j), kSwMinWeight);
+      for (int k = 0; k < K; ++k) {
+        const long long bk = (long long)b * K + k;
+        const float s = bilerp(scores + bk * plane_in, w, y0, y1, wy, x0, x1, wx);
+        preds[bk * plane_out + o] += __fmul_rn(g, 1.f / (1.f + expf(-s)));   // rounded product, then the add
+      }
+      if (b == 0) cnt[o] += g;
+    } else {
+      for (int k = 0; k < K; ++k) {
+        const long long bk = (long long)b * K + k;
+        const float s = bilerp(scores + bk * plane_in, w, y0, y1, wy, x0, x1, wx);
+        preds[bk * plane_out + o] += 1.f / (1.f + expf(-s));     // torch.sigmoid
+      }
+      if (b == 0) cnt[o] += 1.f;                                   // one count map: every image sees the same windows
     }
-    if (b == 0) cnt[o] += 1.f;                                   // one count map: every image sees the same windows
   }
 }
 
@@ -185,13 +198,21 @@ int grid_for(long long work, int per_launch_cap) {
 extern "C" int sx_sw2d_accumulate(const float* scores, int32_t B, int32_t K, int32_t h, int32_t w, int32_t dx, int32_t dy,
                                   float* preds, float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, int32_t mirror,
                                   void* stream) {
+  const SxSwWeights wt = sx_sw_take_weights();              // consumed by this call, whether it succeeds or not
   SX_REQUIRE(B > 0 && K > 0 && h > 0 && w > 0 && dx > 0 && dy > 0 && xs >= 0 && ys >= 0 && xs + dx <= H2 && ys + dy <= W2,
              "sx_sw2d_accumulate: window [%d+%d, %d+%d] outside the %dx%d image, or empty scores (%dx%d)", xs, dx, ys, dy, H2, W2,
              h, w);
   SX_REQUIRE(mirror >= 0 && mirror <= 3, "sx_sw2d_accumulate: mirror mask %d is not a subset of {H, W} (0..3)", mirror);
+  SX_REQUIRE(!wt.wx || (wt.nx == dx && wt.ny == dy && wt.nz == 1),
+             "sx_sw2d_accumulate: window weight tables of %dx%dx%d for a %dx%d window", wt.nx, wt.ny, wt.nz, dx, dy);
   const int blocks = grid_for((long long)B * dx * dy, sm_count_cached() * 8);
-  sw2d_accumulate_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(scores, B, K, h, w, dx, dy, preds, cnt,
-                                                                                     H2, W2, xs, ys, mirror);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (wt.wx)
+    sw2d_accumulate_kernel<true><<<blocks, 256, 0, st>>>(scores, B, K, h, w, dx, dy, preds, cnt, H2, W2, xs, ys, mirror, wt.wx,
+                                                         wt.wy);
+  else
+    sw2d_accumulate_kernel<false><<<blocks, 256, 0, st>>>(scores, B, K, h, w, dx, dy, preds, cnt, H2, W2, xs, ys, mirror,
+                                                          nullptr, nullptr);
   SX_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

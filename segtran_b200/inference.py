@@ -8,7 +8,12 @@ upsample folded into the accumulating kernel.  No CPU fallback: the images must 
 Both take an opt-in ``mirror_axes`` (mirror test-time augmentation, beyond the reference): every window batch is also
 predicted mirrored along each non-empty subset of those axes, and the scores, flipped back, are averaged with the
 plain ones.  The mirrored windows are gathered straight from the padded image by one kernel (``sx_sw_gather``), and the
-accumulating kernels read the scores through reversed indices, so no flipped score map is written."""
+accumulating kernels read the scores through reversed indices, so no flipped score map is written.
+
+Both also take an opt-in ``gaussian_sigma_scale`` (Gaussian importance weighting of the overlapping windows, as in
+nnU-Net and MONAI's ``mode="gaussian"``): each window adds w * sigmoid(score) and w to the count, with w a separable
+Gaussian of the position inside the window, so voxels near a window's centre count more than those at its edges.  The
+accumulating kernels apply the weight from per-axis tables armed by ``sx_sw_set_weights``."""
 from __future__ import annotations
 
 import ctypes
@@ -16,6 +21,7 @@ import math
 import numbers
 from collections.abc import Sequence
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -45,6 +51,43 @@ def _mirror_masks(mirror_axes, ndim, who):
     return [sum(1 << a for i, a in enumerate(axes) if m >> i & 1) for m in range(1 << len(axes))]
 
 
+def _sigma_scale(gaussian_sigma_scale, who):
+    """None, or the finite sigma scale s > 0 as a float."""
+    s = gaussian_sigma_scale
+    if s is None:
+        return None
+    if isinstance(s, bool) or not isinstance(s, numbers.Real) or not math.isfinite(s) or not s > 0:
+        raise ValueError("%s: gaussian_sigma_scale must be None or a finite real number > 0, got %r" % (who, s))
+    return float(s)
+
+
+def gaussian_window_tables(size, sigma_scale):
+    """The per-axis weight tables of a window of extent ``size`` = (d_0, d_1, ...), concatenated in axis order as one fp32
+    tensor: g(i) = exp(-(i - (d-1)/2)^2 / (2 (s d)^2)) for i = 0..d-1, computed in float64 and divided by its maximum
+    over i, then rounded to fp32.  An element's weight is max(g_0(i) * g_1(j) [* g_2(l)], 1e-3), taken in fp32 by the
+    accumulating kernels.  The division by the maximum is taken in the exponent (the maximum is at the centre cell(s),
+    (i - (d-1)/2)^2 = m with m = 0 or 1/4), so a tiny s cannot make it 0 / 0."""
+    out = []
+    for d in size:
+        sd = sigma_scale * d
+        q = (np.arange(d, dtype=np.float64) - (d - 1) / 2.0) ** 2
+        out.append(np.exp(-(q - q.min()) / (2.0 * sd * sd)))
+    return torch.from_numpy(np.concatenate(out)).float()
+
+
+def _window_weights(size, sigma_scale, device):
+    """(tables, args): the per-axis tables of the ``size`` window on ``device`` (built once per call) and the
+    sx_sw_set_weights arguments that arm them for the next accumulate launch; (None, None) without weighting.  A 2-D
+    window passes no z table."""
+    if sigma_scale is None:
+        return None, None
+    tab = gaussian_window_tables(size, sigma_scale).to(device)
+    p, n = tab.data_ptr(), [int(d) for d in size]
+    if len(n) == 2:
+        return tab, (p, n[0], p + 4 * n[0], n[1], None, 1)
+    return tab, (p, n[0], p + 4 * n[0], n[1], p + 4 * (n[0] + n[1]), n[2])
+
+
 def _tta_image(img, who):
     if img.dtype != torch.float32:
         raise ValueError("%s: mirror_axes needs a float32 image, got %s" % (who, img.dtype))
@@ -64,7 +107,7 @@ def _gather(img, origins, win, mirror):
 
 
 def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, stride_xy, stride_z, task_name, net_type,
-                     num_classes, *, mirror_axes=()):
+                     num_classes, *, mirror_axes=(), gaussian_sigma_scale=None):
     """image [C,H,W,D] (CUDA) -> (preds_hard, preds_soft), exactly as the reference's function of the same name.
 
     mirror_axes: distinct axes among 0, 1, 2 (H, W, D).  With k of them, each window batch is predicted 2^k times, on
@@ -72,8 +115,14 @@ def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, 
     scores are flipped back, resized, passed through the sigmoid and accumulated, each variant adding one to the window
     count.  The soft output is the mean over the variants of this function run with the net x -> flip_m(net(flip_m(x))).
     The flip back is read by the accumulating kernel after the resize to the window size; it commutes with the resize up
-    to rounding.  The image must be float32 then.  () is the reference's computation."""
+    to rounding.  The image must be float32 then.  () is the reference's computation.
+
+    gaussian_sigma_scale: None (the reference's flat average) or s > 0: every window, and every mirror variant of it,
+    adds w * sigmoid(score) to the soft map and w to the count, with w the Gaussian weight of the position inside the
+    orig_patch_size window (gaussian_window_tables; sigma = s times the window's extent along each axis, floored at 1e-3).
+    The soft output is then the weighted average.  nnU-Net uses s = 1/8."""
     masks = _mirror_masks(mirror_axes, 3, "test_single_case")
+    sigma = _sigma_scale(gaussian_sigma_scale, "test_single_case")
     ops._req_cuda(image)
     C, H, W, D = image.shape
     dx, dy, dz = orig_patch_size
@@ -94,6 +143,7 @@ def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, 
     cnt = torch.zeros((H2, W2, D2), device=dev, dtype=torch.float32)
     st = ops._stream
     img = _tta_image(image, "test_single_case").unsqueeze(0) if len(masks) > 1 else None
+    wtab, warm = _window_weights((dx, dy, dz), sigma, dev)     # wtab owns the tables the armed pointers address
 
     for x in range(sx):
         xs = min(stride_xy * x, H2 - dx)
@@ -117,6 +167,8 @@ def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, 
                             scores_raw = scores_raw[1]
                         scores_raw = _resize(scores_raw, orig_patch_size).float().contiguous()
                         for i, (ys_i, zs_i) in enumerate(yzs_batch):   # sequential launches: overlapping windows never race
+                            if warm:
+                                L.call("sx_sw_set_weights", *warm)
                             L.call("sx_sw_accumulate", scores_raw[i].data_ptr(), K, dx, dy, dz, preds_soft.data_ptr(),
                                    cnt.data_ptr(), H2, W2, D2, xs, ys_i, zs_i, m, st())
                         del test_batch, scores_raw                     # one variant's batch alive at a time
@@ -134,7 +186,7 @@ def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, 
 
 
 def test_single_batch(net, image_batch, orig_input_size, patch_size, stride, task_name, num_classes, model_type, *,
-                      mirror_axes=()):
+                      mirror_axes=(), gaussian_sigma_scale=None):
     """image_batch [B,C,H,W] (CUDA) -> (preds_hard int32 [B,K,H,W], preds_soft fp32 [B,K,H,W]), exactly as the reference's
     test_util2d.test_single_batch (code/test_util2d.py:151-225): zero-pad to orig_input_size, one window per launch in the
     reference's order, each window's scores upsampled, passed through the sigmoid and accumulated by one kernel
@@ -143,8 +195,12 @@ def test_single_batch(net, image_batch, orig_input_size, patch_size, stride, tas
     mirror_axes: distinct axes among 0, 1 (H, W); as in test_single_case, each window is predicted on flip_m(window) for
     every subset m, and the scores are flipped back (by reversing the upsample's source taps), upsampled and accumulated,
     so the soft output is the mean over the variants of the net x -> flip_m(net(flip_m(x))).  The image must be float32
-    then.  () is the reference's computation."""
+    then.  () is the reference's computation.
+
+    gaussian_sigma_scale: as in test_single_case, on the orig_input_size window: the weight is applied after the
+    upsample, at the window position the upsampled score lands on."""
     masks = _mirror_masks(mirror_axes, 2, "test_single_batch")
+    sigma = _sigma_scale(gaussian_sigma_scale, "test_single_batch")
     ops._req_cuda(image_batch)
     B, C, H, W = image_batch.shape
     dx, dy = orig_input_size
@@ -163,6 +219,7 @@ def test_single_batch(net, image_batch, orig_input_size, patch_size, stride, tas
     cnt = torch.zeros((H2, W2), device=dev, dtype=torch.float32)
     st = ops._stream
     img = _tta_image(image_batch, "test_single_batch") if len(masks) > 1 else None
+    wtab, warm = _window_weights((dx, dy), sigma, dev)         # wtab owns the tables the armed pointers address
 
     for x in range(sx):
         xs = min(stride[0] * x, H2 - dx)
@@ -185,6 +242,8 @@ def test_single_batch(net, image_batch, orig_input_size, patch_size, stride, tas
                     raise ValueError("test_single_batch: the net returned scores of shape %s, expected [%d, %d, h, w]"
                                      % (tuple(scores_raw.shape), B, K))
                 h, w = scores_raw.shape[2:]
+                if warm:
+                    L.call("sx_sw_set_weights", *warm)
                 L.call("sx_sw2d_accumulate", scores_raw.data_ptr(), B, K, h, w, dx, dy, preds.data_ptr(), cnt.data_ptr(),
                        H2, W2, xs, ys, m, st())
                 del test_patch, scores_raw                  # one variant's window alive at a time
