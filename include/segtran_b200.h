@@ -17,9 +17,8 @@
  *  - every call is asynchronous on the cudaStream_t given (passed as void*);
  *  - return 0 on success, negative on error; sx_last_error() returns a thread-local message;
  *  - no global mutable state apart from one-time function-attribute setup (thread safe: the
- *    autograd engine calls backward entry points from its own worker thread) and three thread-local
- *    slots: sx_last_error's message, the transposed output sx_gemm_set_tout arms and the window
- *    weight tables sx_sw_set_weights arms;
+ *    autograd engine calls backward entry points from its own worker thread) and one thread-local
+ *    slot, sx_last_error's message;
  *  - the device is the current CUDA context's device (torch sets it); never assumed to be 0.
  *  - there is NO CPU fallback: a missing GPU / non-sm_90 device is an error.
  */
@@ -98,20 +97,17 @@ typedef struct {
   int64_t part_floats;
 } sx_gemm_args;
 
-int sx_gemm(const sx_gemm_args* args, void* stream);
-
-/* Transposed second output of the next sx_gemm call made on the same host thread (sx_gemm_set_tout arms it, that call
- * consumes it whether it succeeds or not; NULL disarms): a copy of the final fp32 C values (after alpha, bias,
- * activation, dropout and TF32 rounding) at ct[z1*ct_stride_z1 + z0*ct_stride_z0 + n*ldct + m] = C[z1][z0][m][n], so
- * that a later product contracting over m reads it K-major.  Requirements: tf32 operands, both K-major; split_k = 1,
- * accumulate = 0, fp32 C; ct 16-byte aligned, ldct >= M, ldct and the z strides multiples of 4.  It is a separate
- * block so that sx_gemm_args keeps its layout. */
+/* Optional transposed second output of sx_gemm (tout == NULL: none): a copy of the final fp32 C values (after alpha,
+ * bias, activation, dropout and TF32 rounding) at ct[z1*ct_stride_z1 + z0*ct_stride_z0 + n*ldct + m] = C[z1][z0][m][n],
+ * so that a later product contracting over m reads it K-major.  Requirements: tf32 operands, both K-major; split_k = 1,
+ * accumulate = 0, fp32 C; ct non-NULL and 16-byte aligned, ldct >= M, ldct and the z strides multiples of 4.  It is a
+ * separate block so that sx_gemm_args keeps its layout. */
 typedef struct {
   float* ct;
   int64_t ldct, ct_stride_z0, ct_stride_z1;
 } sx_gemm_tout;
 
-int sx_gemm_set_tout(const sx_gemm_tout* tout);
+int sx_gemm(const sx_gemm_args* args, const sx_gemm_tout* tout, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Sliding-window positional biases (SlidingPosBiases2D/3D, segtran_shared.py:1002-1175), never expanded to [N,N]:
@@ -510,20 +506,26 @@ int sx_sgemm_small(const float* A, const float* B, float* C, int32_t M, int32_t 
  * sx_sw_gather: out[w][b] = flip_mirror(img[b][:, x0_w:x0_w+dx, y0_w:y0_w+dy, z0_w:z0_w+dz]) for the n windows whose
  *   origins are the HOST array origins[3n] (x0, y0, z0 each), from the contiguous fp32 [B][C][H][W][D] image into the
  *   contiguous [n][B][C][dx][dy][dz] out.  A 2-D batch [B][C][H][W] is D = dz = 1.
- * sx_sw_set_weights: window weights (Gaussian blending) for the next sx_sw_accumulate or sx_sw2d_accumulate call made on
- *   the same host thread, which consumes them whether it succeeds or not (wx == NULL disarms).  wx, wy, wz are fp32
- *   DEVICE tables of the window's axes, read while that call's kernel runs; the call then adds w * sigmoid(...) to preds
- *   and w to cnt, with w = max(wx[i] * wy[j] * wz[l], 1e-3) (fp32, in that order) at window position (i, j, l), the
- *   accumulator's coordinates (after the 2-D upsample; mirror does not move it).  nx, ny, nz must equal that call's
- *   (dx, dy, dz): otherwise the call fails before any launch.  A 2-D call takes wz == NULL or nz == 1, and does not read
- *   wz.  Without armed tables the accumulates add sigmoid(...) and 1, as above.
+ * sx_sw_weights: the window weights (Gaussian blending) of one sx_sw_accumulate or sx_sw2d_accumulate call, whose
+ *   `weights` argument is NULL for the unweighted update above.  wx, wy, wz are fp32 DEVICE tables of the window's axes,
+ *   read while that call's kernel runs; the call then adds w * sigmoid(...) to preds and w to cnt, with
+ *   w = max(wx[i] * wy[j] * wz[l], 1e-3) (fp32, in that order) at window position (i, j, l), the accumulator's
+ *   coordinates (after the 2-D upsample; mirror does not move it).  wx and wy must be given with nx, ny, nz > 0, and
+ *   (nx, ny, nz) must equal the call's (dx, dy, dz): otherwise the call fails before any launch.  A 3-D call needs wz; a
+ *   2-D call takes nz == 1 and does not read wz.
  * ------------------------------------------------------------------------------------------- */
+typedef struct {
+  const float* wx;
+  const float* wy;
+  const float* wz;
+  int32_t nx, ny, nz, _pad;
+} sx_sw_weights;
 int sx_sw_accumulate(const float* scores, int32_t K, int32_t dx, int32_t dy, int32_t dz, float* preds, float* cnt,
-                     int32_t H, int32_t W, int32_t D, int32_t x0, int32_t y0, int32_t z0, int32_t mirror, void* stream);
+                     int32_t H, int32_t W, int32_t D, int32_t x0, int32_t y0, int32_t z0, int32_t mirror,
+                     const sx_sw_weights* weights, void* stream);
 int sx_sw_finalize(float* preds, const float* cnt, int32_t K, int64_t V, int32_t brats, float* hard, void* stream);
 int sx_sw_gather(const float* img, int32_t B, int32_t C, int32_t H, int32_t W, int32_t D, const int32_t* origins, int32_t n,
                  int32_t dx, int32_t dy, int32_t dz, int32_t mirror, float* out, void* stream);
-int sx_sw_set_weights(const float* wx, int32_t nx, const float* wy, int32_t ny, const float* wz, int32_t nz);
 
 /* -------------------------------------------------------------------------------------------
  * 2-D sliding-window inference and per-image evaluation (csrc/sx_eval2d.cu; code/test_util2d.py:169-265, harden_segmap2d
@@ -541,7 +543,8 @@ int sx_sw_set_weights(const float* wx, int32_t nx, const float* wy, int32_t ny, 
  *   2 <= K <= 8.  Integer atomics only: the counts do not depend on scheduling.
  * ------------------------------------------------------------------------------------------- */
 int sx_sw2d_accumulate(const float* scores, int32_t B, int32_t K, int32_t h, int32_t w, int32_t dx, int32_t dy, float* preds,
-                       float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, int32_t mirror, void* stream);
+                       float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, int32_t mirror,
+                       const sx_sw_weights* weights, void* stream);
 int sx_sw2d_finalize(const float* preds, const float* cnt, int32_t B, int32_t K, int32_t H2, int32_t W2, int32_t hl,
                      int32_t wl, int32_t H, int32_t W, float* soft, int32_t* hard, void* stream);
 int sx_eval2d_counts(const float* pred, int32_t B, int32_t K, int32_t h, int32_t w, const float* gt, int32_t Hg, int32_t Wg,

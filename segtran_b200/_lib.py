@@ -47,6 +47,11 @@ class sx_gemm_tout(C.Structure):
     _fields_ = [("ct", C.c_void_p), ("ldct", C.c_int64), ("ct_stride_z0", C.c_int64), ("ct_stride_z1", C.c_int64)]
 
 
+class sx_sw_weights(C.Structure):
+    _fields_ = [("wx", C.c_void_p), ("wy", C.c_void_p), ("wz", C.c_void_p), ("nx", C.c_int32), ("ny", C.c_int32),
+                ("nz", C.c_int32), ("_pad", C.c_int32)]
+
+
 class sx_posbias(C.Structure):
     _fields_ = [("table", C.c_void_p), ("pd", C.c_int32), ("R", C.c_int32), ("grid", C.c_int32 * 3), ("w", C.c_float)]
 
@@ -88,8 +93,7 @@ _P, _I, _L, _F, _U64, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint
 
 # name -> argtypes (every function returns int; 0 = success)
 _PROTOS = {
-    "sx_gemm": [C.POINTER(sx_gemm_args), _P],
-    "sx_gemm_set_tout": [C.POINTER(sx_gemm_tout)],
+    "sx_gemm": [C.POINTER(sx_gemm_args), C.POINTER(sx_gemm_tout), _P],
     "sx_gemm_debug_set": [C.c_char_p, _L],
     "sx_attn_probs_fwd": [C.POINTER(sx_attn_probs_args), _P],
     "sx_attn_consist_fwd": [C.POINTER(sx_consist_args), _P],
@@ -115,11 +119,10 @@ _PROTOS = {
     "sx_seed_derive": [_P, _U64, _P, _P],
     "sx_seed_advance": [_P, _U64, _P],
     "sx_convert": [_P, _I, _L, _P, _I, _I, _P],
-    "sx_sw_accumulate": [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P],
+    "sx_sw_accumulate": [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _I, C.POINTER(sx_sw_weights), _P],
     "sx_sw_finalize": [_P, _P, _I, _L, _I, _P, _P],
     "sx_sw_gather": [_P, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P],
-    "sx_sw_set_weights": [_P, _I, _P, _I, _P, _I],
-    "sx_sw2d_accumulate": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, _P],
+    "sx_sw2d_accumulate": [_P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _I, C.POINTER(sx_sw_weights), _P],
     "sx_sw2d_finalize": [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P],
     "sx_eval2d_counts": [_P, _I, _I, _I, _I, _P, _I, _I, _P, _P],
     "sx_mask_counts": [_P, _P, _I, _L, _P, _L, _P],
@@ -192,8 +195,8 @@ def check(rc, what):
 
 
 # kernels launched per C-ABI call (for bench.py's gpu_launches claim); default 1
-_LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0, "sx_gemm_set_tout": 0,
-             "sx_sw_set_weights": 0, "sx_attn_probs_fwd": 2, "sx_colsum_batched": 2, "sx_dot": 2, "sx_head_contract_bwd_weight": 2,
+_LAUNCHES = {"sx_pos_lsinu_bwd": 3, "sx_ln_softaggr_bwd": 2, "sx_prologue_bwd": 3, "sx_layernorm_bwd": 3, "sx_gemm_debug_set": 0,
+             "sx_attn_probs_fwd": 2, "sx_colsum_batched": 2, "sx_dot": 2, "sx_head_contract_bwd_weight": 2,
              "sx_softmax_posbias_bwd": 2, "sx_attn_consist_fwd": 2, "sx_head_dropout_bwd": 2, "sx_edt_sq": 3}
 launch_count = 0
 _hook = None          # optional callable(name, args) -> context manager, installed by bench.py for per-kernel timing

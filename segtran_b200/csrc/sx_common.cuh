@@ -31,22 +31,13 @@ void sx_set_error(const char* fmt, ...);
     }                                                                                           \
   } while (0)
 
-// Window weight tables of the sliding-window accumulates, armed by sx_sw_set_weights (sx_infer.cu) on this host thread.
-struct SxSwWeights {
-  const float* wx;
-  const float* wy;
-  const float* wz;
-  int nx, ny, nz;
-};
-// the armed tables (wx == nullptr: none); disarms them
-SxSwWeights sx_sw_take_weights();
 // floor of a window weight (MONAI's): keeps cnt > 0 at window corners that only one window covers
 constexpr float kSwMinWeight = 1e-3f;
 
 static inline int sx_ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
 // SM count of the CURRENT device (cached per device ordinal: a process may drive several GPUs)
-static int sm_count_cached() {
+static inline int sm_count_cached() {
   static int n[64] = {0};
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 0;

@@ -197,19 +197,21 @@ int grid_for(long long work, int per_launch_cap) {
 
 extern "C" int sx_sw2d_accumulate(const float* scores, int32_t B, int32_t K, int32_t h, int32_t w, int32_t dx, int32_t dy,
                                   float* preds, float* cnt, int32_t H2, int32_t W2, int32_t xs, int32_t ys, int32_t mirror,
-                                  void* stream) {
-  const SxSwWeights wt = sx_sw_take_weights();              // consumed by this call, whether it succeeds or not
+                                  const sx_sw_weights* wt, void* stream) {
   SX_REQUIRE(B > 0 && K > 0 && h > 0 && w > 0 && dx > 0 && dy > 0 && xs >= 0 && ys >= 0 && xs + dx <= H2 && ys + dy <= W2,
              "sx_sw2d_accumulate: window [%d+%d, %d+%d] outside the %dx%d image, or empty scores (%dx%d)", xs, dx, ys, dy, H2, W2,
              h, w);
   SX_REQUIRE(mirror >= 0 && mirror <= 3, "sx_sw2d_accumulate: mirror mask %d is not a subset of {H, W} (0..3)", mirror);
-  SX_REQUIRE(!wt.wx || (wt.nx == dx && wt.ny == dy && wt.nz == 1),
-             "sx_sw2d_accumulate: window weight tables of %dx%dx%d for a %dx%d window", wt.nx, wt.ny, wt.nz, dx, dy);
+  SX_REQUIRE(!wt || (wt->wx && wt->wy && wt->nx > 0 && wt->ny > 0 && wt->nz > 0),
+             "sx_sw2d_accumulate: empty or missing table (wx=%p nx=%d, wy=%p ny=%d, nz=%d)", (const void*)wt->wx, wt->nx,
+             (const void*)wt->wy, wt->ny, wt->nz);
+  SX_REQUIRE(!wt || (wt->nx == dx && wt->ny == dy && wt->nz == 1),
+             "sx_sw2d_accumulate: window weight tables of %dx%dx%d for a %dx%d window", wt->nx, wt->ny, wt->nz, dx, dy);
   const int blocks = grid_for((long long)B * dx * dy, sm_count_cached() * 8);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (wt.wx)
-    sw2d_accumulate_kernel<true><<<blocks, 256, 0, st>>>(scores, B, K, h, w, dx, dy, preds, cnt, H2, W2, xs, ys, mirror, wt.wx,
-                                                         wt.wy);
+  if (wt)
+    sw2d_accumulate_kernel<true><<<blocks, 256, 0, st>>>(scores, B, K, h, w, dx, dy, preds, cnt, H2, W2, xs, ys, mirror, wt->wx,
+                                                         wt->wy);
   else
     sw2d_accumulate_kernel<false><<<blocks, 256, 0, st>>>(scores, B, K, h, w, dx, dy, preds, cnt, H2, W2, xs, ys, mirror,
                                                           nullptr, nullptr);

@@ -612,7 +612,7 @@ extern "C" int sx_gemm_debug_set(const char* key, int64_t value) {
 }
 
 // t: the transposed second output, or null
-static int gemm_run(const sx_gemm_args* a, const sx_gemm_tout* t, void* stream) {
+extern "C" int sx_gemm(const sx_gemm_args* a, const sx_gemm_tout* t, void* stream) {
   SX_REQUIRE(a != nullptr, "sx_gemm: null args");
   SX_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0 && a->Z0 > 0 && a->Z1 > 0, "sx_gemm: bad shape M=%d N=%d K=%d Z=%dx%d",
              a->M, a->N, a->K, a->Z0, a->Z1);
@@ -719,19 +719,4 @@ static int gemm_run(const sx_gemm_args* a, const sx_gemm_tout* t, void* stream) 
   if (!amn && bmn) return launch<2, false, true>(ta, tb, p, grid, st);
   if (amn && !bmn) return launch<2, true, false>(ta, tb, p, grid, st);
   return launch<2, true, true>(ta, tb, p, grid, st);
-}
-
-// the transposed output armed for the next sx_gemm call of this host thread
-static thread_local sx_gemm_tout g_tout{};
-
-extern "C" int sx_gemm_set_tout(const sx_gemm_tout* t) {
-  g_tout = t ? *t : sx_gemm_tout{};
-  SX_REQUIRE(t == nullptr || t->ct != nullptr, "sx_gemm_set_tout: null ct");
-  return 0;
-}
-
-extern "C" int sx_gemm(const sx_gemm_args* a, void* stream) {
-  const sx_gemm_tout t = g_tout;          // consumed by this call, whether it succeeds or not
-  g_tout = sx_gemm_tout{};
-  return gemm_run(a, t.ct ? &t : nullptr, stream);
 }

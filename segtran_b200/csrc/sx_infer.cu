@@ -4,8 +4,8 @@
 // Mirror test-time augmentation: a window-gather kernel writes a batch of mirrored windows straight from the padded image,
 // and the accumulate kernel reads a variant's scores through reversed indices, so no flipped map is ever written.
 // Mirror masks: bit 0 reverses H (dx), bit 1 W (dy), bit 2 D (dz).
-// Window weighting (Gaussian blending): sx_sw_set_weights arms per-axis tables for the next accumulate of the host thread,
-// which then adds w * sigmoid and w instead of sigmoid and 1; the tables live here for both the 3-D and 2-D accumulates.
+// Window weighting (Gaussian blending): an accumulate given per-axis weight tables (sx_sw_weights) adds w * sigmoid and w
+// instead of sigmoid and 1; the 2-D accumulate of sx_eval2d.cu takes the same tables.
 #include "sx_common.cuh"
 
 namespace {
@@ -111,41 +111,25 @@ __global__ void sw_gather_kernel(const float* __restrict__ img, int B, int C, in
 
 }  // namespace
 
-// the window weight tables armed for the next sliding-window accumulate of this host thread
-static thread_local SxSwWeights g_sw_weights{};
-
-SxSwWeights sx_sw_take_weights() {
-  const SxSwWeights w = g_sw_weights;
-  g_sw_weights = SxSwWeights{};
-  return w;
-}
-
-extern "C" int sx_sw_set_weights(const float* wx, int32_t nx, const float* wy, int32_t ny, const float* wz, int32_t nz) {
-  g_sw_weights = SxSwWeights{};
-  if (wx == nullptr) return 0;                                // disarm
-  SX_REQUIRE(nx > 0 && wy != nullptr && ny > 0 && (wz == nullptr || nz > 0),
-             "sx_sw_set_weights: empty or missing table (nx=%d, wy=%p ny=%d, wz=%p nz=%d)", nx, (const void*)wy, ny,
-             (const void*)wz, nz);
-  g_sw_weights = SxSwWeights{wx, wy, wz, nx, ny, wz ? nz : 1};
-  return 0;
-}
-
 extern "C" int sx_sw_accumulate(const float* scores, int32_t K, int32_t dx, int32_t dy, int32_t dz, float* preds, float* cnt,
-                                int32_t H, int32_t W, int32_t D, int32_t x0, int32_t y0, int32_t z0, int32_t mirror, void* stream) {
-  const SxSwWeights wt = sx_sw_take_weights();              // consumed by this call, whether it succeeds or not
+                                int32_t H, int32_t W, int32_t D, int32_t x0, int32_t y0, int32_t z0, int32_t mirror,
+                                const sx_sw_weights* wt, void* stream) {
   SX_REQUIRE(K > 0 && dx > 0 && dy > 0 && dz > 0 && x0 >= 0 && y0 >= 0 && z0 >= 0 && x0 + dx <= H && y0 + dy <= W && z0 + dz <= D,
              "sx_sw_accumulate: window [%d+%d, %d+%d, %d+%d] outside the %dx%dx%d volume", x0, dx, y0, dy, z0, dz, H, W, D);
   SX_REQUIRE(mirror >= 0 && mirror <= 7, "sx_sw_accumulate: mirror mask %d is not a subset of {H, W, D} (0..7)", mirror);
-  SX_REQUIRE(!wt.wx || (wt.wz && wt.nx == dx && wt.ny == dy && wt.nz == dz),
-             "sx_sw_accumulate: window weight tables of %dx%dx%d (z table %s) for a %dx%dx%d window", wt.nx, wt.ny, wt.nz,
-             wt.wz ? "given" : "missing", dx, dy, dz);
+  SX_REQUIRE(!wt || (wt->wx && wt->wy && wt->nx > 0 && wt->ny > 0 && wt->nz > 0),
+             "sx_sw_accumulate: empty or missing table (wx=%p nx=%d, wy=%p ny=%d, wz=%p nz=%d)", (const void*)wt->wx,
+             wt->nx, (const void*)wt->wy, wt->ny, (const void*)wt->wz, wt->nz);
+  SX_REQUIRE(!wt || (wt->wz && wt->nx == dx && wt->ny == dy && wt->nz == dz),
+             "sx_sw_accumulate: window weight tables of %dx%dx%d (z table %s) for a %dx%dx%d window", wt->nx, wt->ny,
+             wt->nz, wt->wz ? "given" : "missing", dx, dy, dz);
   const long long pv = (long long)dx * dy * dz;
   long long blocks = (pv + 255) / 256;
   if (blocks > sm_count_cached() * 8) blocks = sm_count_cached() * 8;
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (wt.wx)
+  if (wt)
     sw_accumulate_kernel<true><<<(int)blocks, 256, 0, st>>>(scores, K, dx, dy, dz, preds, cnt, H, W, D, x0, y0, z0, mirror,
-                                                            wt.wx, wt.wy, wt.wz);
+                                                            wt->wx, wt->wy, wt->wz);
   else
     sw_accumulate_kernel<false><<<(int)blocks, 256, 0, st>>>(scores, K, dx, dy, dz, preds, cnt, H, W, D, x0, y0, z0, mirror,
                                                              nullptr, nullptr, nullptr);

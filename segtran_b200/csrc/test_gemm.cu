@@ -95,7 +95,7 @@ static int run_case(const Case& c, bool verbose) {
   g.bias_stride_z0 = c.bias_mode == SX_BIAS_M ? c.M : c.N;
   g.bias_stride_z1 = g.bias_stride_z0 * c.Z0;
   g.act = c.act; g.accumulate = c.split_k > 1; g.preact = dP; g.split_k = c.split_k; g.amax = damax;
-  int rc = sx_gemm(&g, nullptr);
+  int rc = sx_gemm(&g, nullptr, nullptr);
   cudaError_t e = cudaDeviceSynchronize();
   if (rc != 0 || e != cudaSuccess) {
     printf("CASE %-28s LAUNCH-FAIL rc=%d err=%s cuda=%s\n", c.name, rc, sx_last_error(), cudaGetErrorString(e));
@@ -198,11 +198,11 @@ static void perf(int op, int amaj, int bmaj, int M, int N, int K, int Z) {
   g.C = dC; g.c_dtype = SX_F32; g.ldc = N; g.c_stride_z0 = (long long)M * N; g.alpha = 1.f; g.split_k = 1;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  for (int i = 0; i < 3; ++i) sx_gemm(&g, nullptr);
+  for (int i = 0; i < 3; ++i) sx_gemm(&g, nullptr, nullptr);
   cudaDeviceSynchronize();
   const int iters = 10;
   cudaEventRecord(e0);
-  for (int i = 0; i < iters; ++i) sx_gemm(&g, nullptr);
+  for (int i = 0; i < iters; ++i) sx_gemm(&g, nullptr, nullptr);
   cudaEventRecord(e1);
   cudaEventSynchronize(e1);
   float ms = 0;
@@ -234,11 +234,11 @@ static void perf_epi(const char* name, int bias, int pre, int gelu, float drop, 
   g.preact = dP; g.act = gelu ? SX_ACT_GELU : SX_ACT_NONE; g.drop_p = drop; g.drop_seed = 77; g.round_tf32 = rnd;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  for (int i = 0; i < 3; ++i) sx_gemm(&g, nullptr);
+  for (int i = 0; i < 3; ++i) sx_gemm(&g, nullptr, nullptr);
   cudaDeviceSynchronize();
   const int iters = 20;
   cudaEventRecord(e0);
-  for (int i = 0; i < iters; ++i) sx_gemm(&g, nullptr);
+  for (int i = 0; i < iters; ++i) sx_gemm(&g, nullptr, nullptr);
   cudaEventRecord(e1);
   cudaEventSynchronize(e1);
   float ms = 0;
@@ -279,14 +279,14 @@ static void perf_wide(int M, int N, int K, int Z, int epi, int rounds) {
   std::vector<float> t[2];
   for (int w = 0; w < 2; ++w) {
     sx_gemm_debug_set("wide_tiles", w);
-    for (int i = 0; i < 3; ++i) sx_gemm(&g, nullptr);
+    for (int i = 0; i < 3; ++i) sx_gemm(&g, nullptr, nullptr);
   }
   for (int r = 0; r < rounds; ++r)
     for (int w = 0; w < 2; ++w) {
       sx_gemm_debug_set("wide_tiles", w);
       cudaDeviceSynchronize();
       cudaEventRecord(e0);
-      for (int i = 0; i < iters; ++i) sx_gemm(&g, nullptr);
+      for (int i = 0; i < iters; ++i) sx_gemm(&g, nullptr, nullptr);
       cudaEventRecord(e1);
       cudaEventSynchronize(e1);
       float ms = 0;

@@ -13,7 +13,7 @@ accumulating kernels read the scores through reversed indices, so no flipped sco
 Both also take an opt-in ``gaussian_sigma_scale`` (Gaussian importance weighting of the overlapping windows, as in
 nnU-Net and MONAI's ``mode="gaussian"``): each window adds w * sigmoid(score) and w to the count, with w a separable
 Gaussian of the position inside the window, so voxels near a window's centre count more than those at its edges.  The
-accumulating kernels apply the weight from per-axis tables armed by ``sx_sw_set_weights``."""
+accumulating kernels apply the weight from per-axis tables that each accumulate call is given (``sx_sw_weights``)."""
 from __future__ import annotations
 
 import ctypes
@@ -76,16 +76,18 @@ def gaussian_window_tables(size, sigma_scale):
 
 
 def _window_weights(size, sigma_scale, device):
-    """(tables, args): the per-axis tables of the ``size`` window on ``device`` (built once per call) and the
-    sx_sw_set_weights arguments that arm them for the next accumulate launch; (None, None) without weighting.  A 2-D
-    window passes no z table."""
+    """(tables, weights): the per-axis tables of the ``size`` window on ``device`` (built once per call) and the
+    ``weights`` argument of every accumulate launch, a reference to the sx_sw_weights descriptor that addresses them;
+    (None, None) without weighting.  A 2-D window passes no z table."""
     if sigma_scale is None:
         return None, None
     tab = gaussian_window_tables(size, sigma_scale).to(device)
     p, n = tab.data_ptr(), [int(d) for d in size]
     if len(n) == 2:
-        return tab, (p, n[0], p + 4 * n[0], n[1], None, 1)
-    return tab, (p, n[0], p + 4 * n[0], n[1], p + 4 * (n[0] + n[1]), n[2])
+        desc = L.sx_sw_weights(p, p + 4 * n[0], None, n[0], n[1], 1)
+    else:
+        desc = L.sx_sw_weights(p, p + 4 * n[0], p + 4 * (n[0] + n[1]), *n)
+    return tab, ctypes.byref(desc)
 
 
 def _tta_image(img, who):
@@ -143,7 +145,7 @@ def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, 
     cnt = torch.zeros((H2, W2, D2), device=dev, dtype=torch.float32)
     st = ops._stream
     img = _tta_image(image, "test_single_case").unsqueeze(0) if len(masks) > 1 else None
-    wtab, warm = _window_weights((dx, dy, dz), sigma, dev)     # wtab owns the tables the armed pointers address
+    wtab, wts = _window_weights((dx, dy, dz), sigma, dev)      # wtab owns the tables the descriptor points to
 
     for x in range(sx):
         xs = min(stride_xy * x, H2 - dx)
@@ -167,10 +169,8 @@ def test_single_case(net, image, orig_patch_size, input_patch_size, batch_size, 
                             scores_raw = scores_raw[1]
                         scores_raw = _resize(scores_raw, orig_patch_size).float().contiguous()
                         for i, (ys_i, zs_i) in enumerate(yzs_batch):   # sequential launches: overlapping windows never race
-                            if warm:
-                                L.call("sx_sw_set_weights", *warm)
                             L.call("sx_sw_accumulate", scores_raw[i].data_ptr(), K, dx, dy, dz, preds_soft.data_ptr(),
-                                   cnt.data_ptr(), H2, W2, D2, xs, ys_i, zs_i, m, st())
+                                   cnt.data_ptr(), H2, W2, D2, xs, ys_i, zs_i, m, wts, st())
                         del test_batch, scores_raw                     # one variant's batch alive at a time
                     test_patches, yzs_batch = [], []
 
@@ -219,7 +219,7 @@ def test_single_batch(net, image_batch, orig_input_size, patch_size, stride, tas
     cnt = torch.zeros((H2, W2), device=dev, dtype=torch.float32)
     st = ops._stream
     img = _tta_image(image_batch, "test_single_batch") if len(masks) > 1 else None
-    wtab, warm = _window_weights((dx, dy), sigma, dev)         # wtab owns the tables the armed pointers address
+    wtab, wts = _window_weights((dx, dy), sigma, dev)          # wtab owns the tables the descriptor points to
 
     for x in range(sx):
         xs = min(stride[0] * x, H2 - dx)
@@ -242,10 +242,8 @@ def test_single_batch(net, image_batch, orig_input_size, patch_size, stride, tas
                     raise ValueError("test_single_batch: the net returned scores of shape %s, expected [%d, %d, h, w]"
                                      % (tuple(scores_raw.shape), B, K))
                 h, w = scores_raw.shape[2:]
-                if warm:
-                    L.call("sx_sw_set_weights", *warm)
                 L.call("sx_sw2d_accumulate", scores_raw.data_ptr(), B, K, h, w, dx, dy, preds.data_ptr(), cnt.data_ptr(),
-                       H2, W2, xs, ys, m, st())
+                       H2, W2, xs, ys, m, wts, st())
                 del test_patch, scores_raw                  # one variant's window alive at a time
 
     preds_soft = torch.empty((B, K, H, W), device=dev, dtype=torch.float32)

@@ -452,6 +452,7 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
         if addend.dtype != torch.float32 or tuple(addend.shape[-2:]) != (M, N) or _as4(addend).stride() != o4.stride():
             raise L.SxError("gemm_nt: addend must be an fp32 tensor in the output's layout")
         g.addend = addend.data_ptr()
+    tout = None
     if ct is not None:
         t4 = _as4(ct)
         if ct.dtype != torch.float32 or tuple(t4.shape[-2:]) != (N, M) or t4.stride(-1) != 1 or round_after:
@@ -461,8 +462,8 @@ def _gemm_nt_1(a: torch.Tensor, b: torch.Tensor, *, out: Optional[torch.Tensor] 
         t.ldct = t4.stride(-2)
         t.ct_stride_z0 = t4.stride(1) if t4.shape[1] > 1 else 0
         t.ct_stride_z1 = t4.stride(0) if t4.shape[0] > 1 else 0
-        L.call("sx_gemm_set_tout", C.byref(t))             # consumed by the next sx_gemm call of this thread
-    L.call("sx_gemm", C.byref(g), _stream())
+        tout = C.byref(t)
+    L.call("sx_gemm", C.byref(g), tout, _stream())
     if round_after and fresh:                # (caller-provided accumulators are gradient buffers: never rounded)
         L.call("sx_convert", out.data_ptr(), L.SX_F32, out.numel(), out.data_ptr(), L.SX_F32, 1, _stream())
     return out

@@ -120,17 +120,20 @@ def test_valid_sigma_scales_still_need_a_gpu():
                               gaussian_sigma_scale=s)
 
 
-def test_header_declares_the_weight_entry_point():
+def test_header_declares_the_weight_descriptor():
+    import ctypes
     from segtran_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "segtran_b200.h")).read()
-    assert "int sx_sw_set_weights(const float* wx, int32_t nx, const float* wy, int32_t ny, const float* wz, int32_t nz);" \
-        in hdr
-    assert "sx_sw_set_weights" in _lib.EXPORTS and len(_lib._PROTOS["sx_sw_set_weights"]) == 6
-    assert _lib._LAUNCHES["sx_sw_set_weights"] == 0
-    assert hasattr(_lib.lib(), "sx_sw_set_weights")
+    assert ("typedef struct {\n  const float* wx;\n  const float* wy;\n  const float* wz;\n  int32_t nx, ny, nz, _pad;\n"
+            "} sx_sw_weights;") in hdr
+    assert ctypes.sizeof(_lib.sx_sw_weights) == 40
+    assert (_lib.sx_sw_weights.wy.offset, _lib.sx_sw_weights.wz.offset, _lib.sx_sw_weights.nx.offset,
+            _lib.sx_sw_weights.nz.offset) == (8, 16, 24, 32)
+    for name in ("sx_sw_accumulate", "sx_sw2d_accumulate"):
+        assert _lib._PROTOS[name][-2:] == [ctypes.POINTER(_lib.sx_sw_weights), ctypes.c_void_p]
     readme = open(os.path.join(ROOT, "README.md")).read()
-    line = next(ln for ln in readme.splitlines() if "(71 entry points)" in ln)
-    assert "sx_sw_set_weights" in line
+    line = next(ln for ln in readme.splitlines() if "include/segtran_b200.h" in ln)
+    assert "(%d entry points)" % len(_lib.EXPORTS) in line
 
 
 def _refused(name, *args):
@@ -140,21 +143,20 @@ def _refused(name, *args):
     return str(e.value)
 
 
-def _arm(*args):
+def _weights(wx, nx, wy, ny, wz, nz):
+    import ctypes
     from segtran_b200 import _lib as L
-    L.call("sx_sw_set_weights", *args)
+    return ctypes.byref(L.sx_sw_weights(wx, wy, wz, nx, ny, nz))
 
 
 def test_table_size_mismatch_is_refused_before_any_launch():
     """The pointers below are never dereferenced: every call is refused on the host."""
-    acc3 = (0, 4, 2, 2, 2, 0, 0, 4, 4, 4, 0, 0, 0, 0, None)                  # a valid 2x2x2 window in a 4x4x4 volume
-    acc2 = (0, 1, 3, 2, 2, 4, 4, 0, 0, 8, 8, 0, 0, 0, None)                  # a valid 4x4 window in an 8x8 image
+    acc3 = (0, 4, 2, 2, 2, 0, 0, 4, 4, 4, 0, 0, 0, 0)                        # a valid 2x2x2 window in a 4x4x4 volume
+    acc2 = (0, 1, 3, 2, 2, 4, 4, 0, 0, 8, 8, 0, 0, 0)                        # a valid 4x4 window in an 8x8 image
     for tables in [(8, 3, 8, 2, 8, 2), (8, 2, 8, 2, 8, 3), (8, 2, 8, 2, None, 1), (8, 2, 8, 4, 8, 2)]:
-        _arm(*tables)
-        assert "weight tables" in _refused("sx_sw_accumulate", *acc3)
+        assert "weight tables" in _refused("sx_sw_accumulate", *acc3, _weights(*tables), None)
     for tables in [(8, 4, 8, 3, None, 1), (8, 2, 8, 4, None, 1), (8, 4, 8, 4, 8, 2)]:
-        _arm(*tables)
-        assert "weight tables" in _refused("sx_sw2d_accumulate", *acc2)
-    assert "missing table" in _refused("sx_sw_set_weights", 8, 2, None, 2, None, 1)
-    assert "missing table" in _refused("sx_sw_set_weights", 8, 0, 8, 2, None, 1)
-    assert "missing table" in _refused("sx_sw_set_weights", 8, 2, 8, 2, 8, 0)
+        assert "weight tables" in _refused("sx_sw2d_accumulate", *acc2, _weights(*tables), None)
+    for tables in [(8, 2, None, 2, None, 1), (8, 0, 8, 2, None, 1), (8, 2, 8, 2, 8, 0), (None, 2, 8, 2, 8, 2)]:
+        assert "missing table" in _refused("sx_sw_accumulate", *acc3, _weights(*tables), None)
+        assert "missing table" in _refused("sx_sw2d_accumulate", *acc2, _weights(*tables), None)

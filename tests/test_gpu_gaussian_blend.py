@@ -1,8 +1,9 @@
 """Gaussian window blending of the sliding-window drop-ins (``gaussian_sigma_scale`` of segtran_b200.inference: the
-weighted instantiations of sx_sw_accumulate / sx_sw2d_accumulate, armed by sx_sw_set_weights) on the GPU: against the
-stock-PyTorch oracle (oracle/gauss_oracle.py) on the inference and TTA fixture inputs and at a BraTS-size volume and a
-REFUGE-size batch, with every mirror_axes combination, on nets whose scores are constant or depend on the position, run
-to run, the arming protocol at the C ABI, and peak memory."""
+weighted instantiations of sx_sw_accumulate / sx_sw2d_accumulate, given an sx_sw_weights descriptor) on the GPU: against
+the stock-PyTorch oracle (oracle/gauss_oracle.py) on the inference and TTA fixture inputs and at a BraTS-size volume and
+a REFUGE-size batch, with every mirror_axes combination, on nets whose scores are constant or depend on the position,
+run to run, weighted and unweighted calls at the C ABI, and peak memory."""
+import ctypes
 import itertools
 
 import pytest
@@ -173,37 +174,37 @@ def _st():
     return torch.cuda.current_stream().cuda_stream
 
 
-def test_an_accumulate_without_arming_is_unweighted():
-    """Each accumulate consumes the armed tables, also when it is refused: the next one adds sigmoid and 1."""
+def test_an_accumulate_without_weights_is_unweighted():
+    """An accumulate given tables adds w * sigmoid and w; one given none adds sigmoid and 1, also right after a refused
+    weighted call."""
     dev = "cuda"
     K, d = 2, (3, 4, 5)
     scores = torch.zeros((K,) + d, device=dev)                              # sigmoid(0) = 1/2
     tab = torch.cat([torch.full((n,), v, device=dev) for n, v in zip(d, (0.5, 0.25, 0.5))])
     px = tab.data_ptr()
+    wts = ctypes.byref(L.sx_sw_weights(px, px + 4 * d[0], px + 4 * (d[0] + d[1]), *d))
     preds = torch.zeros((K,) + d, device=dev)
     cnt = torch.zeros(d, device=dev)
-    acc3 = (scores.data_ptr(), K, *d, preds.data_ptr(), cnt.data_ptr(), *d, 0, 0, 0, 0, _st())
-    L.call("sx_sw_set_weights", px, d[0], px + 4 * d[0], d[1], px + 4 * (d[0] + d[1]), d[2])
-    L.call("sx_sw_accumulate", *acc3)
+    acc3 = (scores.data_ptr(), K, *d, preds.data_ptr(), cnt.data_ptr(), *d, 0, 0, 0)
+    L.call("sx_sw_accumulate", *acc3, 0, wts, _st())
     assert torch.equal(cnt, torch.full(d, 0.0625, device=dev)) and torch.equal(preds, torch.full_like(preds, 0.03125))
-    L.call("sx_sw_accumulate", *acc3)
+    L.call("sx_sw_accumulate", *acc3, 0, None, _st())
     assert torch.equal(cnt, torch.full(d, 1.0625, device=dev)) and torch.equal(preds, torch.full_like(preds, 0.53125))
-    L.call("sx_sw_set_weights", px, d[0], px + 4 * d[0], d[1], px + 4 * (d[0] + d[1]), d[2])
     with pytest.raises(L.SxError, match="mirror mask 8"):
-        L.call("sx_sw_accumulate", *acc3[:13], 8, _st())
-    L.call("sx_sw_accumulate", *acc3)
+        L.call("sx_sw_accumulate", *acc3, 8, wts, _st())
+    L.call("sx_sw_accumulate", *acc3, 0, None, _st())
     assert torch.equal(cnt, torch.full(d, 2.0625, device=dev))
 
-    # 2-D: the weight sits on the upsampled window; the same protocol
+    # 2-D: the weight sits on the upsampled window
     B, h, w, dx, dy = 2, 3, 5, 6, 10
     s2 = torch.zeros(B, K, h, w, device=dev)
     tab2 = torch.cat([torch.full((dx,), 0.5, device=dev), torch.full((dy,), 0.5, device=dev)])
+    wts2 = ctypes.byref(L.sx_sw_weights(tab2.data_ptr(), tab2.data_ptr() + 4 * dx, None, dx, dy, 1))
     p2 = torch.zeros(B, K, dx, dy, device=dev)
     c2 = torch.zeros(dx, dy, device=dev)
-    acc2 = (s2.data_ptr(), B, K, h, w, dx, dy, p2.data_ptr(), c2.data_ptr(), dx, dy, 0, 0, 0, _st())
-    L.call("sx_sw_set_weights", tab2.data_ptr(), dx, tab2.data_ptr() + 4 * dx, dy, None, 1)
-    L.call("sx_sw2d_accumulate", *acc2)
-    L.call("sx_sw2d_accumulate", *acc2)
+    acc2 = (s2.data_ptr(), B, K, h, w, dx, dy, p2.data_ptr(), c2.data_ptr(), dx, dy, 0, 0, 0)
+    L.call("sx_sw2d_accumulate", *acc2, wts2, _st())
+    L.call("sx_sw2d_accumulate", *acc2, None, _st())
     assert torch.equal(c2, torch.full((dx, dy), 1.25, device=dev)) and torch.equal(p2, torch.full_like(p2, 0.625))
 
 

@@ -159,8 +159,8 @@ def test_attn_pv_node_copies_on_and_off():
         assert torch.equal(x, y), (i, float((x - y).abs().max()))
 
 
-def test_armed_output_serves_one_call_only():
-    """the transposed output is consumed by the sx_gemm call after it is armed, also when that call is refused"""
+def test_ct_is_written_only_by_the_call_given_it():
+    """a refused call leaves ct untouched, and a call without ct never writes it, before or after one with it"""
     import segtran_b200._lib as L
     from segtran_b200 import ops
     a = tf32(torch.randn(1, 1, 256, 512, device="cuda"))

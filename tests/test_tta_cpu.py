@@ -81,7 +81,7 @@ def test_header_declares_the_mirror_entry_points():
     from segtran_b200 import _lib
     hdr = open(os.path.join(ROOT, "include", "segtran_b200.h")).read()
     assert "int sx_sw_gather(" in hdr and "sx_sw_gather" in _lib.EXPORTS
-    assert len(_lib._PROTOS["sx_sw_accumulate"]) == 15 and len(_lib._PROTOS["sx_sw2d_accumulate"]) == 15
+    assert len(_lib._PROTOS["sx_sw_accumulate"]) == 16 and len(_lib._PROTOS["sx_sw2d_accumulate"]) == 16
     assert len(_lib._PROTOS["sx_sw_gather"]) == 14
     readme = open(os.path.join(ROOT, "README.md")).read()
     assert "(71 entry points)" in readme
@@ -100,8 +100,8 @@ def test_kernels_refuse_bad_masks_and_windows_before_any_launch():
     assert "mirror mask -1" in _refused("sx_sw_gather", 0, 1, 2, 4, 4, 4, org, 2, 2, 2, 2, -1, 0, None)
     assert "window 1" in _refused("sx_sw_gather", 0, 1, 2, 4, 4, 4, org, 2, 3, 3, 3, 1, 0, None)
     assert "empty" in _refused("sx_sw_gather", 0, 1, 2, 4, 4, 4, None, 2, 2, 2, 2, 1, 0, None)
-    assert "mirror mask 8" in _refused("sx_sw_accumulate", 0, 4, 2, 2, 2, 0, 0, 4, 4, 4, 0, 0, 0, 8, None)
-    assert "mirror mask 4" in _refused("sx_sw2d_accumulate", 0, 1, 3, 2, 2, 4, 4, 0, 0, 8, 8, 0, 0, 4, None)
+    assert "mirror mask 8" in _refused("sx_sw_accumulate", 0, 4, 2, 2, 2, 0, 0, 4, 4, 4, 0, 0, 0, 8, None, None)
+    assert "mirror mask 4" in _refused("sx_sw2d_accumulate", 0, 1, 3, 2, 2, 4, 4, 0, 0, 8, 8, 0, 0, 4, None, None)
 
 
 @pytest.mark.parametrize("axes", [(0, 0), (3,), (-1,), (0, 1, 2, 0), 0, "01", {0, 1}, (True,), (0.0,), None])

@@ -10,7 +10,7 @@ net of the TTA fixtures, so the times are the sliding window itself rather than 
 gaussian_sigma_scale=0.125, with mirror_axes=() and with every axis.  Times are CUDA events around a call after
 --warmup calls, median over --reps.  Then the accumulate kernel alone: CUDA events around 200 back-to-back
 sx_sw_accumulate (one 112^3 window, K=4) or sx_sw2d_accumulate (288^2 scores upsampled to 576^2, B=6, K=3) launches,
-unweighted and armed.  Prints the device name and power limit read in the same run."""
+unweighted and weighted.  Prints the device name and power limit read in the same run."""
 from __future__ import annotations
 
 import argparse
@@ -65,14 +65,12 @@ def arms(name, run, axes, reps, warmup):
                                                                           100 * (gauss[0] / plain[0] - 1)))
 
 
-def kernel_loop(name, call, arm, n=200, reps=5):
+def kernel_loop(name, call, wts, n=200, reps=5):
     st = torch.cuda.current_stream().cuda_stream
 
     def loop(weighted):
         for _ in range(n):
-            if weighted:
-                L.call("sx_sw_set_weights", *arm)
-            L.call(*call(st))
+            L.call(*call(wts if weighted else None, st))
 
     res = {}
     for weighted in (False, True, False, True):                 # alternate the two, keep the last of each
@@ -121,17 +119,17 @@ def main():
     sc3 = torch.randn((4,) + d, device="cuda")
     pr3 = torch.zeros((4, 240, 240, 155), device="cuda")
     cn3 = torch.zeros((240, 240, 155), device="cuda")
-    tab3, arm3 = SI._window_weights(d, S, "cuda")
+    tab3, wts3 = SI._window_weights(d, S, "cuda")
     kernel_loop("sx_sw_accumulate 112^3 window, K=4",
-                lambda st: ("sx_sw_accumulate", sc3.data_ptr(), 4, *d, pr3.data_ptr(), cn3.data_ptr(), 240, 240, 155,
-                            56, 56, 43, 0, st), arm3)
+                lambda wts, st: ("sx_sw_accumulate", sc3.data_ptr(), 4, *d, pr3.data_ptr(), cn3.data_ptr(), 240, 240,
+                                 155, 56, 56, 43, 0, wts, st), wts3)
     sc2 = torch.randn(6, 3, 288, 288, device="cuda")
     pr2 = torch.zeros(6, 3, 576, 576, device="cuda")
     cn2 = torch.zeros(576, 576, device="cuda")
-    tab2, arm2 = SI._window_weights((576, 576), S, "cuda")
+    tab2, wts2 = SI._window_weights((576, 576), S, "cuda")
     kernel_loop("sx_sw2d_accumulate 288^2 -> 576^2, B=6, K=3",
-                lambda st: ("sx_sw2d_accumulate", sc2.data_ptr(), 6, 3, 288, 288, 576, 576, pr2.data_ptr(),
-                            cn2.data_ptr(), 576, 576, 0, 0, 0, st), arm2)
+                lambda wts, st: ("sx_sw2d_accumulate", sc2.data_ptr(), 6, 3, 288, 288, 576, 576, pr2.data_ptr(),
+                                 cn2.data_ptr(), 576, 576, 0, 0, 0, wts, st), wts2)
     del tab3, tab2
 
 
