@@ -165,7 +165,15 @@ typedef struct {
   const uint64_t* drop_seed_dev;
   sx_posbias posbias;            /* table == NULL: no positional bias */
 } sx_attn_probs_args;
-int sx_attn_probs_fwd(const sx_attn_probs_args* args, void* stream);
+
+/* Optional transposed probabilities (tout == NULL: none): pt[((b*M + m)*U2 + k)*ldpt + u] = P[b][m][u][k], the same final
+ * values (after clamp, bias, dropout and TF32 rounding), so the backward's P^T product reads them K-major.  ldpt >= U1
+ * (a multiple of 4 when a GEMM reads pt through TMA).  A separate block so that sx_attn_probs_args keeps its layout. */
+typedef struct {
+  float* pt;
+  int64_t ldpt;
+} sx_attn_probs_tout;
+int sx_attn_probs_fwd(const sx_attn_probs_args* args, const sx_attn_probs_tout* tout, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Attention-consistency loss of one layer (csrc/sx_consist.cu; train3d.py:426-449 and train2d.py:668-723), without

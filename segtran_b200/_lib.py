@@ -65,6 +65,10 @@ class sx_attn_probs_args(C.Structure):
                 ("_pad", C.c_uint32), ("drop_seed", C.c_uint64), ("drop_seed_dev", C.c_void_p), ("posbias", sx_posbias)]
 
 
+class sx_attn_probs_tout(C.Structure):
+    _fields_ = [("pt", C.c_void_p), ("ldpt", C.c_int64)]
+
+
 class sx_consist_args(C.Structure):
     _fields_ = [("B", C.c_int32), ("N", C.c_int32), ("A", C.c_int32), ("K", C.c_int32), ("variant", C.c_int32),
                 ("round_r", C.c_int32), ("Xo", C.c_void_p), ("xo_ld", C.c_int64), ("xo_bstride", C.c_int64),
@@ -95,7 +99,7 @@ _P, _I, _L, _F, _U64, _D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint
 _PROTOS = {
     "sx_gemm": [C.POINTER(sx_gemm_args), C.POINTER(sx_gemm_tout), _P],
     "sx_gemm_debug_set": [C.c_char_p, _L],
-    "sx_attn_probs_fwd": [C.POINTER(sx_attn_probs_args), _P],
+    "sx_attn_probs_fwd": [C.POINTER(sx_attn_probs_args), C.POINTER(sx_attn_probs_tout), _P],
     "sx_attn_consist_fwd": [C.POINTER(sx_consist_args), _P],
     "sx_attn_consist_bwd": [C.POINTER(sx_consist_args), _P, _P, _I, _I, _L, _L, _P, _P, _P, _L, _L, _P],
     "sx_clamp_if": [_P, _L, _I, _L, _P, _F, _P, _L, _P, _L, _P],

@@ -29,6 +29,12 @@
 // coordinates once per work item and steps the key coordinates along the chunk instead of dividing per element.  The raw
 // scores keep driving S, rowmax, stat[0] and the clamp; the low-row test widens by the bias range (header comment of
 // sx_attn_probs_args).  The unbiased instantiation is the kernel without any of this.
+//
+// Transposed probabilities (PT instantiations, sx_attn_probs_tout): the same final values (after clamp, bias, dropout and
+// TF32 rounding) also go to Pt[b][m][key][query], queries contiguous, so that the backward's dV = P^T dH reads P^T
+// K-major without a transpose pass.  The stores go straight from the fragments: for one (j, e) the 8 row threads of a
+// column hold 8 consecutive queries, so every warp store writes 4 complete 32-byte sectors, and no shared memory is
+// taken from the ring or the bias table.
 #include "sx_common.cuh"
 #include "sx_posbias.cuh"
 #include "sx_tc.cuh"
@@ -70,12 +76,14 @@ struct AttnParams {
   int round_tf32;
   const float* pb_table;          // HAS_BIAS only
   sxpb::Geom pb;
+  float* pt;                      // PT only: [B][M][U2][ldpt] transposed P
+  int ldpt;                       // U2 * ldpt < 2^31: offsets within a (b, m) slice are 32-bit
 };
 
 constexpr int PB_OFFSET = STAGES * STAGE_BYTES + 256;        // HAS_BIAS: w*log2(e)*table after the barriers
 constexpr int PB_MAX_FLOATS = 29 * 29 * 29;                   // 3-D R <= 14: the ring + table fit 227 KB
 
-template <bool HAS_BIAS>
+template <bool HAS_BIAS, bool PT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -323,6 +331,11 @@ sx_attn_probs_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
           }
           if (col + 1 < p.U2) *reinterpret_cast<float2*>(p.P + roff + col) = make_float2(f0, f1);
           else p.P[roff + col] = f0;
+          if constexpr (PT) {                // column col of P is row col of the (b, m) slice of Pt
+            float* pt = p.pt + ((long long)b * p.M + m) * p.U2 * p.ldpt;
+            pt[col * p.ldpt + grow[h]] = f0;
+            if (col + 1 < p.U2) pt[(col + 1) * p.ldpt + grow[h]] = f1;
+          }
         }
       }
     };
@@ -380,9 +393,23 @@ __global__ void attn_diag_kernel(float* stat, float clip, float* diag) {
   }
 }
 
+template <bool HAS_BIAS>
+int launch_probs(const CUtensorMap& tq, const CUtensorMap& tk, const AttnParams& p, int grid, cudaStream_t st) {
+  const int smem = HAS_BIAS ? PB_OFFSET + p.pb.T * 4 + 1024 : SMEM_BYTES;
+  constexpr int smem_max = HAS_BIAS ? PB_OFFSET + PB_MAX_FLOATS * 4 + 1024 : SMEM_BYTES;
+  if (p.pt) {
+    SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel<HAS_BIAS, true>, smem_max));
+    sx_attn_probs_kernel<HAS_BIAS, true><<<grid, NUM_THREADS, smem, st>>>(tq, tk, p);
+  } else {
+    SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel<HAS_BIAS, false>, smem_max));
+    sx_attn_probs_kernel<HAS_BIAS, false><<<grid, NUM_THREADS, smem, st>>>(tq, tk, p);
+  }
+  return 0;
+}
+
 }  // namespace
 
-extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, void* stream) {
+extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, const sx_attn_probs_tout* tout, void* stream) {
   SX_REQUIRE(a != nullptr, "sx_attn_probs_fwd: null args");
   SX_REQUIRE(a->B > 0 && a->M > 0 && a->U1 > 0 && a->U2 > 0 && a->d > 0, "sx_attn_probs_fwd: bad shape");
   SX_REQUIRE(a->Q && a->K && a->P && a->lse && a->stat, "sx_attn_probs_fwd: null pointer");
@@ -410,6 +437,13 @@ extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, void* stream) {
   p.drop_p = a->drop_p; p.drop_seed = a->drop_seed;
   p.drop_seed_dev = reinterpret_cast<const unsigned long long*>(a->drop_seed_dev);
   p.round_tf32 = a->round_tf32;
+  if (tout) {
+    SX_REQUIRE(tout->pt != nullptr, "sx_attn_probs_fwd: null pt");
+    SX_REQUIRE(tout->ldpt >= a->U1 && (long long)a->U2 * tout->ldpt < (1ll << 31),
+               "sx_attn_probs_fwd: ldpt must be at least U1, and U2 * ldpt below 2^31");
+    p.pt = tout->pt;
+    p.ldpt = (int)tout->ldpt;
+  }
   const bool has_bias = a->posbias.table != nullptr;
   if (has_bias) {
     SX_REQUIRE(a->U1 == a->U2, "sx_attn_probs_fwd: positional biases need self-attention (U1 == U2)");
@@ -434,14 +468,8 @@ extern "C" int sx_attn_probs_fwd(const sx_attn_probs_args* a, void* stream) {
 
   const int grid = p.items < sms ? p.items : sms;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (has_bias) {
-    constexpr int smem_pb = PB_OFFSET + PB_MAX_FLOATS * 4 + 1024;
-    SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel<true>, smem_pb));
-    sx_attn_probs_kernel<true><<<grid, NUM_THREADS, PB_OFFSET + p.pb.T * 4 + 1024, st>>>(tq, tk, p);
-  } else {
-    SX_CHECK_CUDA(set_max_smem_once(sx_attn_probs_kernel<false>, SMEM_BYTES));
-    sx_attn_probs_kernel<false><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tq, tk, p);
-  }
+  rc = has_bias ? launch_probs<true>(tq, tk, p, grid, st) : launch_probs<false>(tq, tk, p, grid, st);
+  if (rc) return rc;
   SX_CHECK_CUDA(cudaGetLastError());
   attn_diag_kernel<<<1, 1, 0, st>>>(a->stat, a->clip, a->diag);
   SX_CHECK_CUDA(cudaGetLastError());

@@ -338,9 +338,15 @@ class ExpandedFeatTrans(nn.Module):
         us = [ops.attn_pv(p, vv, M, round_out=False) for p, vv in zip(probs, vs)]     # [B,M,N_s,pad4(w_s)]
         return ops.resize_tokens_into(us, grid, grids, wins, Fd)                 # [B,M,N,F]
 
-    def forward(self, input_feat, attention_probs, in_geoshape=None):
+    def reads_transposed_probs(self, B, U1, U2):
+        """The fused P.V' node's backward reads P^T K-major (ops.pv_gelu_kmajor): forward() then takes it as probs_t."""
+        return self.supports_fused_attention() and self.num_scales == 0 and \
+            ops.pv_gelu_kmajor(B, self.num_modes, U1, U2, self.feat_dim)
+
+    def forward(self, input_feat, attention_probs, in_geoshape=None, probs_t=None):
         """input_feat [B,U2,C]; attention_probs [B,M,U1,U2] -> [B,U1,F].  With mince scales: attention_probs is the list
-        of per-scale probabilities and in_geoshape the token grid."""
+        of per-scale probabilities and in_geoshape the token grid.  probs_t: P^T [B,M,U2,U1] from the attention kernel,
+        when reads_transposed_probs() holds."""
         M = self.num_modes
         if self.num_scales > 0:
             if in_geoshape is None:
@@ -374,7 +380,8 @@ class ExpandedFeatTrans(nn.Module):
             # the dropout mask into the dG GEMM epilogue)
             gl = self.output.group_linear
             y = ops.attn_pv_gelu_group_linear(attention_probs, vp, M, mid.shared_linear.bias, p,
-                                              ops.new_dropout_seed(vp.device) if p > 0 else 0, gl.weight, gl.bias)
+                                              ops.new_dropout_seed(vp.device) if p > 0 else 0, gl.weight, gl.bias,
+                                              probs_t)
         else:
             u = ops.attn_pv(attention_probs, v, M)
             g = self.intermediate(u)
@@ -481,17 +488,21 @@ def _new_diag(device):
 
 
 def _attention_probs(q, k, M, clip, drop_p, diag, *, fused, posbias=None, alpha=None, row_bias=None, tag="big",
-                     kmajor_dq=False):
-    """P = dropout(softmax(clamp_if(alpha Q K^T [+ row_bias]) [+ posbias])) per mode -> (P, S, amax).
+                     kmajor_dq=False, transposed=False, key_t=None):
+    """P = dropout(softmax(clamp_if(alpha Q K^T [+ row_bias]) [+ posbias])) per mode -> (P, S, amax, Pt).
     fused: one sx_attn_probs_fwd kernel (ops.attn_probs), S = amax = None; with kmajor_dq its backward's dQ = dS K reads
-    a K-major copy of the keys.  Otherwise the raw scores S (ops.attn_scores, their maximum tracked on the device in
-    amax), then ops.softmax."""
+    a K-major copy of the keys; with transposed (and autograd recording) the kernel also writes Pt = P^T [B,M,U2,U1].
+    Otherwise the raw scores S (ops.attn_scores, their maximum tracked on the device in amax; key_t: the keys'
+    ops.tokens_t() twin for its dQ), then ops.softmax, and Pt = None."""
     seed = ops.new_dropout_seed(q.device) if drop_p > 0 else 0
     if fused:
-        return ops.attn_probs(q, k, M, alpha, clip, drop_p, seed, diag, posbias, kmajor_dq=kmajor_dq), None, None
+        if transposed and torch.is_grad_enabled():
+            P, Pt = ops.attn_probs(q, k, M, alpha, clip, drop_p, seed, diag, posbias, kmajor_dq=kmajor_dq, transposed=True)
+            return P, None, None, Pt
+        return ops.attn_probs(q, k, M, alpha, clip, drop_p, seed, diag, posbias, kmajor_dq=kmajor_dq), None, None, None
     amax = torch.full((1,), -3.0e38, device=q.device)
-    S = ops.attn_scores(q, k, M, amax, row_bias, tag, alpha)
-    return ops.softmax(S, amax, clip, drop_p, seed, diag, posbias), S, amax
+    S = ops.attn_scores(q, k, M, amax, row_bias, tag, alpha, kt=key_t)
+    return ops.softmax(S, amax, clip, drop_p, seed, diag, posbias), S, amax, None
 
 
 class CrossAttFeatTrans(nn.Module):
@@ -568,9 +579,10 @@ class CrossAttFeatTrans(nn.Module):
     def clamp_count(self):
         return self._diag_values()[1]
 
-    def forward(self, in_query, in_key=None, pos_biases=None):
+    def forward(self, in_query, in_key=None, pos_biases=None, query_t=None):
         """pos_biases: an ops.PosBias over the tokens of a self-attention (the reference's [1,1,N,N] bias matrix, kept
-        as its window table); it is added to the scores after the clamp, scaled by pos_code_weight (:589-592)."""
+        as its window table); it is added to the scores after the clamp, scaled by pos_code_weight (:589-592).
+        query_t: in_query's ops.tokens_t() twin (or None), for the query projection's weight gradient."""
         if in_key is None:
             in_key = in_query
         pb = None
@@ -589,7 +601,7 @@ class CrossAttFeatTrans(nn.Module):
         nq, nk = in_query.shape[1], in_key.shape[1]
         tq = ops.small_tag(nq, nk) if nq < nk else "proj"
         tk = ops.small_tag(nk, nq) if nk < nq else "proj"
-        q = ops.linear(in_query, self.query.weight, self.query.bias, tag=tq)
+        q = ops.linear(in_query, self.query.weight, self.query.bias, tag=tq, xt=query_t)
         k = ops.linear(in_key, self.key.weight, self.key.bias, tag=tk)
         dev = q.device
         if self._diag is None or self._diag.device != dev:
@@ -599,9 +611,12 @@ class CrossAttFeatTrans(nn.Module):
         fused = ops.attn_fusion_enabled() and not self.keep_attn_scores and not diag_call and q.is_cuda and \
             self.attention_mode_dim % 4 == 0 and self.out_trans.supports_fused_attention()
         # the expansion block's dQ = dS K reads a K-major copy of the keys (the squeeze-out's attractor keys are small
-        # against dS); multi-head reads its keys in place (DESIGN §4.3)
-        probs, s, amax = _attention_probs(q, k, M, float(self.attn_clip), p, self._diag, fused=fused, posbias=pb,
-                                          kmajor_dq=isinstance(self.out_trans, ExpandedFeatTrans))
+        # against dS); multi-head reads its keys in place (DESIGN §4.3).  When the expansion block's dV' = P^T dH reads
+        # K-major operands, the attention kernel also writes P^T for it.
+        expanded = isinstance(self.out_trans, ExpandedFeatTrans)
+        transposed = fused and expanded and self.out_trans.reads_transposed_probs(k.shape[0], nq, nk)
+        probs, s, amax, probs_t = _attention_probs(q, k, M, float(self.attn_clip), p, self._diag, fused=fused,
+                                                   posbias=pb, kmajor_dq=expanded, transposed=transposed)
         # kept after the conditional clamp, as the reference keeps them (:578-598)
         self.attention_scores = ops.clamp_if(s, amax, float(self.attn_clip)) if self.keep_attn_scores else None
         if self.training:
@@ -612,6 +627,8 @@ class CrossAttFeatTrans(nn.Module):
                 mx, cc = self._diag_values()
                 print("max-attn: {:.2f}, avg-attn: {:.2f}, clamp-count: {}".format(mx, avg, cc))
                 self._diag = _new_diag(dev)
+        if probs_t is not None:
+            return self.out_trans(in_key, probs, probs_t=probs_t)
         return self.out_trans(in_key, probs)
 
 
@@ -726,7 +743,7 @@ class CrossMinceAttFeatTrans(nn.Module):
         fused = ops.attn_fusion_enabled() and not diag_call and q.is_cuda
         probs = []
         for s in range(self.num_scales):
-            P, sc, _ = _attention_probs(qs[s], ks[s], M, float(self.attn_clip), p, self._diag[s], fused=fused,
+            P, sc, _, _ = _attention_probs(qs[s], ks[s], M, float(self.attn_clip), p, self._diag[s], fused=fused,
                                         posbias=pbs[s], alpha=alpha)  # [B,M,N_s,N_s]
             probs.append(P)
             if diag_call:
@@ -762,12 +779,13 @@ class SqueezedAttFeatTrans(nn.Module):
         self.attractors = nn.Parameter(torch.randn(1, self.num_attractors, self.in_feat_dim))
         self.attention_scores = None
 
-    def _in_squeeze_reassociated(self, in_feat):
+    def _in_squeeze_reassociated(self, in_feat, ht):
         """In-squeeze (reference :813 -> CrossAttFeatTrans.forward with M=1, no FFN) with the two token-sized
         projections re-associated away (SURVEY §7): with Q1 = Att Wq^T + bq,
             S1 = Q1 (h Wk^T + bk)^T / sqrt(C) = ((Q1 Wk) h^T + (Q1 . bk) 1^T) / sqrt(C)
             Z  = P1 (h Wv^T)                  = (P1 h) Wv^T
-        so the [N x C x C] key and value GEMMs become [A x C x C] ones; exact up to fp rounding."""
+        so the [N x C x C] key and value GEMMs become [A x C x C] ones; exact up to fp rounding.
+        ht: in_feat's ops.tokens_t() twin (or None), read K-major by P1 h and by the backward's dS1 h."""
         t = self.in_ator_trans
         C = self.in_feat_dim
         st = ops.small_tag(self.num_attractors, in_feat.shape[1])
@@ -781,12 +799,12 @@ class SqueezedAttFeatTrans(nn.Module):
         if t._diag is None or t._diag.device != dev:
             t._diag = _new_diag(dev)
         p = t.att_dropout.p if t.training else 0.0
-        probs, s, amax = _attention_probs(qw, in_feat, 1, float(t.attn_clip), p, t._diag, fused=False, row_bias=rb,
-                                          tag="insq")                                  # [B,1,A,N]
+        probs, s, amax, _ = _attention_probs(qw, in_feat, 1, float(t.attn_clip), p, t._diag, fused=False, row_bias=rb,
+                                             tag="insq", key_t=ht)                     # [B,1,A,N]
         t.attention_scores = ops.clamp_if(s, amax, float(t.attn_clip)) if t.keep_attn_scores else None
         if t.training:
             t.call_count += 1
-        u = ops.attn_pv(probs, in_feat, 1, tag="insq", round_out=not x3)               # P1 h            [B,1,A,C]
+        u = ops.attn_pv(probs, in_feat, 1, tag="insq", round_out=not x3, vt=ht)        # P1 h            [B,1,A,C]
         ot = t.out_trans
         z = ops.linear(u[:, 0], ot.first_linear.weight, tag=st, round_out=False)       # (P1 h) Wv^T     [B,A,C]
         # the updated attractors feed the squeeze-out key projection and the value bank (same precision class)
@@ -796,13 +814,17 @@ class SqueezedAttFeatTrans(nn.Module):
         if pos_biases is not None:
             _unsupported("positional biases with squeezed attention")
         t = self.in_ator_trans
+        ht = None
         if t.num_modes == 1 and not t.out_trans.has_FFN and t.out_trans.first_linear.bias is None \
                 and t.feat_dim == self.in_feat_dim:
-            att = self._in_squeeze_reassociated(in_feat)
+            # the tokens transposed once, when the in-squeeze's token contractions read them K-major: P1 h and dS1 h
+            # per sample, and the squeeze-out query projection's weight gradient over all B*N token rows
+            ht = ops.tokens_t(in_feat, self.num_attractors, "insq")
+            att = self._in_squeeze_reassociated(in_feat, ht)
         else:
             att = t(self.attractors, in_feat)       # attractors are batch-invariant: projected once
         ops.grad_ready(att, self.ator_out_trans.parameters())       # backward past `att`: the squeeze-out weights are final
-        out = self.ator_out_trans(in_feat, att)
+        out = self.ator_out_trans(in_feat, att, query_t=ht)
         self.attention_scores = self.ator_out_trans.attention_scores
         return out
 

@@ -600,6 +600,25 @@ def _weight_t(Wr: torch.Tensor, Z: int, O: int, I: int) -> torch.Tensor:
     return Wr.reshape(Z, O, I).transpose(-1, -2)
 
 
+def tokens_t(x: torch.Tensor, rows: int, tag: str = "big") -> Optional[torch.Tensor]:
+    """K-major twin of the token-major activations x [B,N,C] for products that contract over its tokens: x^T [C, B*N]
+    (one transposed copy, tokens contiguous), or None unless _token_kmajor takes the contraction of `rows` rows against
+    x per sample and N is a multiple of 4 (16-byte sample strides).  As one matrix it is the K operand of a weight
+    gradient over all B*N token rows (linear(..., xt=)); tokens_t_heads() views it per sample for the products that
+    contract over each sample's tokens (attn_pv(..., vt=), attn_scores(..., kt=)).  Not differentiable."""
+    B, N, C = x.shape
+    if N % 4 or not _token_kmajor(rows, C, N, B, tag):
+        return None
+    with torch.no_grad():
+        return _transposed(x, 1, B * N, C)[0]
+
+
+def tokens_t_heads(xt: torch.Tensor, B: int, M: int) -> torch.Tensor:
+    """[B, M, C/M, N] per-sample, per-mode view of a tokens_t() twin [C, B*N]: the "N x K" operand, K-major."""
+    C = xt.shape[0]
+    return xt.view(M, C // M, B, xt.shape[1] // B).permute(2, 0, 1, 3)
+
+
 def colsum(x2d: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out[c] += sum_r x2d[r, c] (rows uniformly strided)."""
     if out is None:
@@ -616,10 +635,11 @@ class _Linear(torch.autograd.Function):
     """y = dropout(act(x W^T + b [+ addend])).  nn.Linear call sites segtran_shared.py:243, :414, :559-560; a weight with
     trailing unit dims (a 1x1 Conv1d, [O, I, 1]) is read as [O, I].  addend (shape of y): a residual added before the
     activation and the dropout (segtran_ablation.py:175-176).  `tag` = precision class of the three products (forward, dx,
-    dW), see the precision policy above."""
+    dW), see the precision policy above.  xt (optional, not differentiable): x^T [I, rows] from tokens_t(); the forward
+    saves it instead of x, and dW = dY^T X reads it and a transposed copy of dY, both K-major."""
 
     @staticmethod
-    def forward(ctx, x, W, b, gelu, drop_p, seed, tag, round_y, addend):
+    def forward(ctx, x, W, b, gelu, drop_p, seed, tag, round_y, addend, xt):
         shp = x.shape
         x2 = x.reshape(-1, shp[-1])
         if not x2.is_contiguous():
@@ -635,15 +655,17 @@ class _Linear(torch.autograd.Function):
                 a2 = a2.contiguous()
         gemm_nt(x2, Wr.view(O, -1), out=y, bias=b, gelu=gelu, preact=h, drop_p=drop_p, seed=seed, tag=tag,
                 round_out=round_y, addend=a2)
-        ctx.save_for_backward(x2, Wr, h)
-        ctx.meta = (shp, b is not None, gelu, drop_p, seed, tag, None if addend is None else addend.shape)
+        if xt is not None and tuple(xt.shape) != (x2.shape[1], x2.shape[0]):
+            raise L.SxError("linear: xt must be x^T [%d, %d]" % (x2.shape[1], x2.shape[0]))
+        ctx.save_for_backward(x2 if xt is None else xt, Wr, h)
+        ctx.meta = (shp, b is not None, gelu, drop_p, seed, tag, None if addend is None else addend.shape, xt is not None)
         ctx.leaves = (W, b)
         return y.view(*shp[:-1], O)
 
     @staticmethod
     def backward(ctx, dy):
         x2, Wr, h = ctx.saved_tensors
-        shp, has_b, gelu, drop_p, seed, tag, add_shape = ctx.meta
+        shp, has_b, gelu, drop_p, seed, tag, add_shape, transposed = ctx.meta
         W, b = ctx.leaves
         if _three_pass(tag) and _PRECISION == "tf32":       # 3-pass forward, single-pass backward: TF32-rounded weight
             Wr = round_tf32(W)
@@ -659,7 +681,12 @@ class _Linear(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = gemm_nt(dy2, _weight_t(Wr2, 1, *Wr2.shape)[0], round_out=False).view(shp)
         if ctx.needs_input_grad[1]:
-            dW = _param_grad(W, dy2.t(), x2.t(), (O, -1))
+            if transposed:                                  # x2 holds x^T
+                dy2t = _transposed(dy2, 1, dy2.shape[0], O)[0]
+                dW = _param_grad(W, dy2t, x2, (O, -1))
+                del dy2t
+            else:
+                dW = _param_grad(W, dy2.t(), x2.t(), (O, -1))
         if has_b and ctx.needs_input_grad[2]:
             tgt = _grad_target(b)
             if tgt is not None:
@@ -668,13 +695,14 @@ class _Linear(torch.autograd.Function):
                 db = colsum(dy2)
         if add_shape is not None and ctx.needs_input_grad[8]:
             da = dy2.view(add_shape)
-        return dx, dW, db, None, None, None, None, None, da
+        return dx, dW, db, None, None, None, None, None, da, None
 
 
-def linear(x, W, b=None, gelu=False, drop_p=0.0, seed=0, tag="big", round_out=True, addend=None):
+def linear(x, W, b=None, gelu=False, drop_p=0.0, seed=0, tag="big", round_out=True, addend=None, xt=None):
     """round_out: round y to TF32 (set False when every consumer of y is a 3-pass contraction or not a GEMM).
-    addend: a tensor of y's shape added to x W^T + b before the activation and the dropout."""
-    return _Linear.apply(x, W, b, gelu, drop_p, seed, tag, round_out, addend)
+    addend: a tensor of y's shape added to x W^T + b before the activation and the dropout.
+    xt: x^T from tokens_t() (or None), for the weight gradient."""
+    return _Linear.apply(x, W, b, gelu, drop_p, seed, tag, round_out, addend, xt)
 
 
 def _heads_aligned(dh: int, Fd: int) -> bool:
@@ -703,10 +731,11 @@ class _AttnScores(torch.autograd.Function):
     A per-mode width d that is not a multiple of 4 (16-byte TMA alignment) reads padded copies of the mode slices.
     q may have batch 1 (the batch-invariant attractor queries): it is broadcast, and its gradient reduced over b.
     row_bias [U1] (single-mode only) is the per-query constant of the re-associated in-squeeze (see
-    SqueezedAttFeatTrans): it is added after the scaling, so it must already be scaled."""
+    SqueezedAttFeatTrans): it is added after the scaling, so it must already be scaled.
+    kt (optional, not differentiable): k^T [M*d, B*U2] from tokens_t(), which dQ = dS K then reads K-major."""
 
     @staticmethod
-    def forward(ctx, q, k, M, amax, row_bias, tag, alpha=None):
+    def forward(ctx, q, k, M, amax, row_bias, tag, alpha=None, kt=None):
         Bq, U1, Cq = q.shape
         B, U2 = k.shape[0], k.shape[1]
         d = Cq // M
@@ -718,31 +747,34 @@ class _AttnScores(torch.autograd.Function):
             raise L.SxError("attn_scores: row_bias needs a single mode")
         rb = row_bias.contiguous().view(-1) if row_bias is not None else None
         gemm_nt(qv, kv, out=S, alpha=scale, amax=amax, round_out=False, bias=rb, bias_mode=L.SX_BIAS_M, tag=tag)
-        ctx.save_for_backward(q, k)
+        ctx.save_for_backward(q, k, kt)
         ctx.meta = (M, d, scale, row_bias.shape if row_bias is not None else None)
         ctx.tag = tag
         return S
 
     @staticmethod
     def backward(ctx, dS):
-        q, k = ctx.saved_tensors
+        q, k, kt = ctx.saved_tensors
         M, d, scale, rb_shape = ctx.meta
         Bq, U1, Cq = q.shape
         B, U2 = k.shape[0], k.shape[1]
         dS = _rowpad(dS)
-        dq, dk = _score_grads(dS, q, k, M, scale, ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.tag)
+        dq, dk = _score_grads(dS, q, k, M, scale, ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.tag, kt=kt)
         drb = None
         if rb_shape is not None and ctx.needs_input_grad[4]:
             drb = _zeros((U1,), q.device)     # sum over batch and keys
             L.call("sx_rowsum", dS.data_ptr(), B * U1, U2, dS.stride(-2), U1, drb.data_ptr(), *_part_args(dS.device), _stream())
             drb = drb.view(rb_shape)
-        return dq, dk, None, None, drb, None, None
+        return dq, dk, None, None, drb, None, None, None
 
 
-def _score_grads(dS, q, k, M, scale, need_q, need_k, tag="big", kmajor_k=False):
+def _score_grads(dS, q, k, M, scale, need_q, need_k, tag="big", kmajor_k=False, kt=None):
     """Gradients of S = scale * Q K^T per mode: dQ = scale dS K, dK = scale dS^T Q (q may have batch 1: broadcast).
-    Both read the MN-major views of the keys and queries (padded K-major copies when the mode slices are not TMA-aligned);
-    kmajor_k: dQ reads a K-major copy of the keys instead (the squeeze-out's attractor keys, small against dS)."""
+    Both read the MN-major views of the keys and queries (padded K-major copies when the mode slices are not TMA-aligned),
+    or K-major copies where _token_kmajor takes them: of the keys for dQ, of dS and the queries for dK (the in-squeeze's
+    [B,1,A,N] scores: dS is 45 MB at cfg 4, while the squeeze-out's dK = dS^T Q, over 180 MB of dS with 256-wide
+    modes, stays MN-major).  kmajor_k: dQ reads a K-major copy of the keys in any case (the squeeze-out's attractor keys,
+    small against dS).  kt: the keys' tokens_t() twin, which dQ then reads instead of a copy."""
     Bq, U1, Cq = q.shape
     B, U2 = k.shape[0], k.shape[1]
     d = Cq // M
@@ -751,12 +783,19 @@ def _score_grads(dS, q, k, M, scale, need_q, need_k, tag="big", kmajor_k=False):
         # dQ[b,m] (U1 x d) = scale * dS[b,m] (U1 x U2) . K[b,m] (U2 x d)
         bcast = Bq == 1 and B > 1
         dq = _zeros_like(q) if bcast else torch.empty_like(q)
-        gemm_nt(dS, _head_cols(k, B, U2, M, d, kmajor_k), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3), alpha=scale,
-                round_out=False, reduce_z1=bcast, split_k=1, tag=tag)
+        gemm_nt(dS, _head_cols(k, B, U2, M, d, kmajor_k or _token_kmajor(U1, d, U2, B * M, tag)) if kt is None else
+                tokens_t_heads(kt, B, M), out=dq.view(Bq, U1, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False,
+                reduce_z1=bcast, split_k=1, tag=tag)
     if need_k:
         dk = torch.empty_like(k)
-        gemm_nt(dS.transpose(-1, -2), _head_cols(q, Bq, U1, M, d, False), out=dk.view(B, U2, M, d).permute(0, 2, 1, 3),
-                alpha=scale, round_out=False, tag=tag)
+        if _token_kmajor(U2, d, U1, B * M, tag):
+            dSt = _transposed(dS, B * M, U1, U2).unflatten(0, (B, M))
+            gemm_nt(dSt, _head_cols(q, Bq, U1, M, d, True), out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale,
+                    round_out=False, tag=tag)
+            del dSt
+        else:
+            gemm_nt(dS.transpose(-1, -2), _head_cols(q, Bq, U1, M, d, False),
+                    out=dk.view(B, U2, M, d).permute(0, 2, 1, 3), alpha=scale, round_out=False, tag=tag)
     return dq, dk
 
 
@@ -803,7 +842,7 @@ def _posbias_table(pb):
 
 
 def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_scores=False, round_out=True, posbias=None,
-                     alpha=None):
+                     alpha=None, pt=None):
     """P = dropout(softmax(min(Q K^T / sqrt(d), clip))) per mode in ONE wgmma kernel (csrc/sx_attn.cu): the scores stay
     in registers and the softmax runs on the accumulator fragments (reference segtran_shared.py:566-567, :569-580, :601, :605).
     q [Bq,U1,M*d] (Bq = 1 broadcasts), k [B,U2,M*d], both contiguous fp32 (TF32-rounded by their producers).
@@ -811,6 +850,8 @@ def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_sc
     and the clamp statistics stay on the raw scores (its table gradient comes from softmax_backward).
     alpha: the score scale (default 1/sqrt(d) of the per-mode width; the mince transformer scales zero-padded channel
     windows by the full width).
+    pt: optional [B,M,U2,U1] view (queries contiguous, row pitch a multiple of 4) that receives P transposed, the same
+    values, from the same kernel.
     -> (P [B,M,U1,U2] view of a row-padded buffer, S or None (raw scaled scores, same layout), lse [B,M,U1],
         rowmax [B,M,U1], stat [2])."""
     _req_cuda(q, k)
@@ -838,7 +879,14 @@ def attn_probs_fused(q, k, M, clip=500.0, drop_p=0.0, seed=0, diag=None, need_sc
     a.drop_seed, a.drop_seed_dev = _seed_args(seed)
     if posbias is not None:
         a.posbias = _posbias_desc(_posbias_table(posbias), posbias.R, posbias.grid, posbias.w)
-    L.call("sx_attn_probs_fwd", C.byref(a), _stream())
+    tout = None
+    if pt is not None:
+        if tuple(pt.shape) != (B, M, U2, U1) or not _rows_ok(pt):
+            raise L.SxError("attn_probs_fused: pt must be a [B,M,U2,U1] view with dense 16-byte-pitched rows")
+        t = L.sx_attn_probs_tout()
+        t.pt, t.ldpt = pt.data_ptr(), pt.stride(-2)
+        tout = C.byref(t)
+    L.call("sx_attn_probs_fwd", C.byref(a), tout, _stream())
     return P, S, lse, rowmax, stat
 
 
@@ -973,10 +1021,11 @@ class _Softmax(torch.autograd.Function):
 class _AttnPV(torch.autograd.Function):
     """U[b,m] = P[b,m] V[b,:,m]   with V [B,U2,M*F], channel = m*F+f  (segtran_shared.py:414-419, :447).
     heads: U is written head-concatenated, [B,U1,M*F] with U[b,:,m*F+f] (MultiHeadFeatTrans, segtran_ablation.py:230-240),
-    straight from the GEMM epilogue (row pitch M*F, head stride F), so the Linear that consumes it reads it K-major."""
+    straight from the GEMM epilogue (row pitch M*F, head stride F), so the Linear that consumes it reads it K-major.
+    vt (optional, not differentiable): v's tokens_t() twin, read in place of a transposed copy of v."""
 
     @staticmethod
-    def forward(ctx, P, v, M, tag, round_out, heads):
+    def forward(ctx, P, v, M, tag, round_out, heads, vt):
         B, _, U1, U2 = P.shape
         Fd = v.shape[-1] // M
         P = _rowpad(P)
@@ -986,7 +1035,10 @@ class _AttnPV(torch.autograd.Function):
                     tag=tag, round_out=round_out)
         else:
             # [B,M,F,U2]: the "N x K" operand, F contiguous (or a K-major copy, when the token contraction pays for it)
-            vv = _head_cols(v, B, U2, M, Fd, _token_kmajor(U1, Fd, U2, B * M, tag))
+            if vt is not None:
+                vv = tokens_t_heads(vt, B, M)
+            else:
+                vv = _head_cols(v, B, U2, M, Fd, _token_kmajor(U1, Fd, U2, B * M, tag))
             U = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
             gemm_nt(P, vv, out=U, tag=tag, round_out=round_out)
         ctx.save_for_backward(P, v)
@@ -1011,27 +1063,32 @@ class _AttnPV(torch.autograd.Function):
                 dv = torch.empty_like(v)
                 gemm_nt(P.transpose(-1, -2), _head_cols(dU, B, U1, M, Fd, False),
                         out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3), round_out=False, tag=ctx.tag)
-            return dP, dv, None, None, None, None
+            return dP, dv, None, None, None, None, None
         dP, dv = _pv_grads(dU, P, v, M, Fd, ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.tag)
-        return dP, dv, None, None, None, None
+        return dP, dv, None, None, None, None, None
 
 
-def _pv_grads(dU, P, v, M, Fd, need_p, need_v, tag, dUt=None):
+def _pv_grads(dU, P, v, M, Fd, need_p, need_v, tag, dUt=None, Pt=None):
     """Gradients of U[b,m] = P[b,m] V[b,:,m] (v [B,U2,M*F], dU [B,M,U1,F] contiguous):
     dP[b,m] = dU[b,m] V[b,:,m]^T (row-padded like P) and dV[b,:,m] = P[b,m]^T dU[b,m].  dUt [B,M,F,U1] (U1
-    contiguous): dU transposed; dV then reads K-major operands (P through a transposed copy).  Without dUt, both are
-    transposed copies where _token_kmajor takes them."""
-    B, _, U1, U2 = P.shape
+    contiguous): dU transposed; dV then reads K-major operands (P through a transposed copy, or Pt [B,M,U2,U1] when the
+    attention kernel wrote it; P may then be None).  Without dUt, both are transposed copies where _token_kmajor takes
+    them."""
+    if Pt is not None:
+        B, _, U2, U1 = Pt.shape
+    else:
+        B, _, U1, U2 = P.shape
     dP = dv = None
     if need_p:
-        dP = _rowpad_empty((B, M, U1, U2), P.device)
+        dP = _rowpad_empty((B, M, U1, U2), dU.device)
         gemm_nt(dU, v.view(B, U2, M, Fd).permute(0, 2, 1, 3), out=dP, round_out=False, tag=tag)
     if need_v:
         dv = torch.empty_like(v)
         if dUt is None and _token_kmajor(U2, Fd, U1, B * M, tag):
             dUt = _transposed(dU, B * M, U1, Fd).unflatten(0, (B, M))
         if dUt is not None:
-            Pt = _transposed(P, B * M, U1, U2).unflatten(0, (B, M))
+            if Pt is None:
+                Pt = _transposed(P, B * M, U1, U2).unflatten(0, (B, M))
             gemm_nt(Pt, dUt, out=dv.view(B, U2, M, Fd).permute(0, 2, 1, 3), round_out=False, tag=tag)
             del Pt
         else:
@@ -1077,11 +1134,25 @@ class _FoldedValueBank(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             da = gemm_nt(d2, _weight_t(Wf, 1, M * Fd, Cd)[0], round_out=False)[0, 0].view(B, A, Cd)
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            dWf = gemm_nt(d2.t(), a2.t(), round_out=False).view(M, 1, Fd, Cd)          # [m, o, c]
+            # dW' = dV'^T a over the B*A bank rows: K-major copies of both where _token_kmajor takes them; that
+            # product then also writes dW'^T [c, m*F+o] (`ct`) for dWv, which contracts over o
+            dWft = None
+            if _token_kmajor(M * Fd, Cd, B * A, 1):
+                if ctx.needs_input_grad[1] and _token_kmajor(Fd, Cd, Fd, M):
+                    dWft = _rowpad_empty((Cd, M * Fd), d2.device)
+                dWf = gemm_nt(_transposed(d2, 1, B * A, M * Fd)[0], _transposed(a2, 1, B * A, Cd)[0], round_out=False,
+                              ct=dWft)
+            else:
+                dWf = gemm_nt(d2.t(), a2.t(), round_out=False)
+            dWf = dWf.view(M, 1, Fd, Cd)                                        # [m, o, c]
             if ctx.needs_input_grad[2]:                               # dWm[o,f] = sum_m dW'_m[o,:] . Wv_m[f,:]
                 dWm = _param_grad(Wm, dWf, Wvr, (1, 1, Fd, Fd), reduce_z1=True)
             if ctx.needs_input_grad[1]:                               # dWv_m[f,c] = sum_o Wm[o,f] dW'_m[o,c]
-                dWv = _param_grad(Wv, Wmr.t().view(1, 1, Fd, Fd), dWf.transpose(-1, -2), (M, 1, Fd, Cd))
+                if dWft is not None:                                  # Wm^T and dW'^T, both K-major
+                    dWv = _param_grad(Wv, _transposed(Wmr, 1, Fd, Fd).view(1, 1, Fd, Fd),
+                                      dWft.view(Cd, M, Fd).permute(1, 0, 2).unsqueeze(1), (M, 1, Fd, Cd))
+                else:
+                    dWv = _param_grad(Wv, Wmr.t().view(1, 1, Fd, Fd), dWf.transpose(-1, -2), (M, 1, Fd, Cd))
         return da, dWv, dWm, None, None
 
 
@@ -1126,31 +1197,40 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
     autograd node, so that backward can fuse gelu'(h) * dropout mask into the epilogue of the dG = dY Wo GEMM
     (SX_ACT_GELU_BWD) instead of writing dG, re-reading it with the pre-activation and writing dH in a separate pass.
     V' = V Wm^T is the value bank already pushed through the shared mid Linear (re-association (P V) Wm^T = P (V Wm^T):
-    A rows instead of N, see ExpandedFeatTrans.forward)."""
+    A rows instead of N, see ExpandedFeatTrans.forward).
+    Pt (optional, non-differentiable): P^T [B,M,U2,U1] from the attention kernel (attn_probs(..., transposed=True)),
+    passed when pv_gelu_kmajor() holds; backward then reads it instead of P."""
 
     @staticmethod
-    def forward(ctx, P, v, M, bm, drop_p, seed, Wo, bo):
+    def forward(ctx, P, v, M, bm, drop_p, seed, Wo, bo, Pt):
         B, _, U1, U2 = P.shape
         Fd = v.shape[-1] // M
         P = _rowpad(P)
         G = torch.empty((B, M, U1, Fd), device=P.device, dtype=torch.float32)
         H = torch.empty_like(G)
         # the token contractions of backward (dWo = dY^T G, dV' = P^T dH) read K-major operands when that pays: G and dH
-        # come transposed out of the epilogues of the GEMMs that make them, P and dY through transposed copies
-        kt = _token_kmajor(Fd, Fd, U1, M) and _token_kmajor(U2, Fd, U1, B * M)
+        # come transposed out of the epilogues of the GEMMs that make them, P^T out of the attention kernel (or through
+        # a transposed copy) and dY through a transposed copy
+        kt = pv_gelu_kmajor(B, M, U1, U2, Fd)
+        if Pt is not None and not kt:
+            raise L.SxError("attn_pv_gelu_group_linear: P^T given for a product that reads P MN-major")
         Gt = _rowpad_empty((B, M, Fd, U1), P.device) if kt else None
         gemm_nt(P, _head_cols(v, B, U2, M, Fd, _kmajor_copies()), out=G, bias=bm, gelu=True, preact=H, drop_p=drop_p,
                 seed=seed, ct=Gt)
         Y, Wr = _group_linear_fwd(G, Wo, bo)
-        ctx.save_for_backward(P, v, H, Gt if kt else G, Wr)      # backward reads G only through one of the two
-        ctx.meta = (M, Fd, drop_p, seed, kt)
+        # backward reads G only through one of the two, and P through P^T when it has it
+        ctx.save_for_backward(P if Pt is None else Pt, v, H, Gt if kt else G, Wr)
+        ctx.meta = (M, Fd, drop_p, seed, kt, Pt is not None)
         ctx.leaves = (bm, Wo, bo)
         return Y
 
     @staticmethod
     def backward(ctx, dY):
         P, v, H, G, Wr = ctx.saved_tensors
-        M, Fd, drop_p, seed, kt = ctx.meta
+        M, Fd, drop_p, seed, kt, transposed = ctx.meta
+        Pt = P if transposed else None
+        if transposed:
+            P = None
         bm, Wo, bo = ctx.leaves
         dY = dY.contiguous()
         dbm_buf = dbm = None
@@ -1160,19 +1240,25 @@ class _AttnPVGeluGroupLinear(torch.autograd.Function):
             dbm = None if tgt is not None else dbm_buf
         # dH = mask * (dY Wo) * gelu'(H), TF32-rounded for the two GEMMs that consume it
         dH = torch.empty_like(H)
-        B, _, U1, _ = P.shape
+        B, U1 = H.shape[0], H.shape[2]
         dHt = _rowpad_empty((B, M, Fd, U1), dY.device) if kt and ctx.needs_input_grad[1] else None
         gemm_nt(dY, _weight_t(Wr, M, Fd, Fd).unsqueeze(0), out=dH, gelu_bwd=H, drop_p=drop_p, seed=seed, ct=dHt)
         if dbm_buf is not None:             # column sums of dH = the gradient of MMSharedMid's bias
             colsum(dH.view(-1, Fd), out=dbm_buf)
         dW, dbo = _group_linear_param_grads(dY, None if kt else G, Wo, bo, ctx.needs_input_grad[6],
                                             ctx.needs_input_grad[7], Gt=G if kt else None)
-        dP, dv = _pv_grads(dH, P, v, M, Fd, ctx.needs_input_grad[0], ctx.needs_input_grad[1], "big", dUt=dHt)
-        return dP, dv, None, dbm, None, None, dW, dbo
+        dP, dv = _pv_grads(dH, P, v, M, Fd, ctx.needs_input_grad[0], ctx.needs_input_grad[1], "big", dUt=dHt, Pt=Pt)
+        return dP, dv, None, dbm, None, None, dW, dbo, None
 
 
-def attn_pv_gelu_group_linear(P, v, M, bm, drop_p, seed, Wo, bo):
-    return _AttnPVGeluGroupLinear.apply(P, v, M, bm, drop_p, seed, Wo, bo)
+def pv_gelu_kmajor(B, M, U1, U2, Fd) -> bool:
+    """Whether attn_pv_gelu_group_linear's backward token contractions read K-major operands (P [B,M,U1,U2], Fd
+    channels per mode): the caller of the attention kernel then asks it for P^T."""
+    return _token_kmajor(Fd, Fd, U1, M) and _token_kmajor(U2, Fd, U1, B * M)
+
+
+def attn_pv_gelu_group_linear(P, v, M, bm, drop_p, seed, Wo, bo, Pt=None):
+    return _AttnPVGeluGroupLinear.apply(P, v, M, bm, drop_p, seed, Wo, bo, Pt)
 
 
 # Fused squeeze-out attention (opt-out: set_attn_fusion(False)): scores + clamp + softmax + attention dropout run in
@@ -1437,9 +1523,9 @@ def dot(x, w):
     return _Dot.apply(x, w.contiguous())
 
 
-def attn_scores(q, k, M, amax=None, row_bias=None, tag="big", alpha=None):
-    """alpha: score scale (default 1/sqrt(d) of the per-mode width)."""
-    return _AttnScores.apply(q, k, M, amax, row_bias, tag, alpha)
+def attn_scores(q, k, M, amax=None, row_bias=None, tag="big", alpha=None, kt=None):
+    """alpha: score scale (default 1/sqrt(d) of the per-mode width).  kt: k's tokens_t() twin (or None)."""
+    return _AttnScores.apply(q, k, M, amax, row_bias, tag, alpha, kt)
 
 
 def softmax(S, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None):
@@ -1450,9 +1536,10 @@ def softmax(S, amax=None, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=Non
     return _Softmax.apply(S, amax, clip, drop_p, seed, diag, *_pb_args(posbias))
 
 
-def attn_pv(P, v, M, tag="big", round_out=True, heads=False):
-    """P [B,M,U1,U2], v [B,U2,M*F] -> [B,M,U1,F], or with heads=True the head-concatenated [B,U1,M*F]."""
-    return _AttnPV.apply(P, v, M, tag, round_out, bool(heads))
+def attn_pv(P, v, M, tag="big", round_out=True, heads=False, vt=None):
+    """P [B,M,U1,U2], v [B,U2,M*F] -> [B,M,U1,F], or with heads=True the head-concatenated [B,U1,M*F].  vt: v's
+    tokens_t() twin (or None; not with heads)."""
+    return _AttnPV.apply(P, v, M, tag, round_out, bool(heads), vt)
 
 
 def layer_norm(x, g, b, consumer_tag=None, producer_tag=None, round_out=True):
@@ -1700,37 +1787,44 @@ def resize_tokens_into(us, grid, grids_in, windows, Fd, round_out=True):
 class _AttnProbs(torch.autograd.Function):
     """P = dropout(softmax(clamp_if(alpha Q K^T) [+ w bias])) per mode as one node over the fused kernel
     (attn_probs_fused): backward = softmax backward on the saved raw scores (softmax_backward, with the table gradient)
-    -> dQ, dK products.  kmajor_dq: dQ reads a K-major copy of the keys (when the copies are on, see _kmajor_copies)."""
+    -> dQ, dK products.  kmajor_dq: dQ reads a K-major copy of the keys (when the copies are on, see _kmajor_copies).
+    transposed: also returns P^T [B,M,U2,U1] (queries contiguous) from the same kernel, a non-differentiable output for
+    the backward of the P.V product that follows (dV = P^T dH reads it K-major)."""
 
     @staticmethod
-    def forward(ctx, q, k, M, alpha, clip, drop_p, seed, diag, table, pb_geom, kmajor_dq):
+    def forward(ctx, q, k, M, alpha, clip, drop_p, seed, diag, table, pb_geom, kmajor_dq, transposed):
         pb = PosBias(table, *pb_geom) if table is not None else None
         need_bwd = any(ctx.needs_input_grad)
+        Pt = _rowpad_empty((k.shape[0], M, k.shape[1], q.shape[1]), q.device) if transposed else None
         P, S, lse, _rowmax, stat = attn_probs_fused(q, k, M, clip, drop_p, seed, diag, need_scores=need_bwd, posbias=pb,
-                                                    alpha=alpha)
+                                                    alpha=alpha, pt=Pt)
         ctx.save_for_backward(q, k, S, lse, stat)
         ctx.meta = (M, alpha, clip, drop_p, seed, P.stride(-2), pb_geom, kmajor_dq)
         ctx.leaf = table
-        return P
+        if Pt is None:
+            return P
+        ctx.mark_non_differentiable(Pt)
+        return P, Pt
 
     @staticmethod
-    def backward(ctx, dP):
+    def backward(ctx, dP, *_dPt):
         q, k, S, lse, stat = ctx.saved_tensors
         M, alpha, clip, drop_p, seed, ldp, pb_geom, kmajor_dq = ctx.meta
         dS, dT = softmax_backward(dP, S, lse, stat[2:], clip, drop_p, seed, ldp, ctx.leaf, pb_geom, ctx.needs_input_grad[8])
         dq, dk = _score_grads(dS, q, k, M, alpha, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
                               kmajor_k=kmajor_dq and _kmajor_copies())
-        return dq, dk, None, None, None, None, None, None, dT, None, None
+        return dq, dk, None, None, None, None, None, None, dT, None, None, None
 
 
-def attn_probs(q, k, M, alpha=None, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None, *, kmajor_dq=False):
+def attn_probs(q, k, M, alpha=None, clip=500.0, drop_p=0.0, seed=0, diag=None, posbias=None, *, kmajor_dq=False,
+               transposed=False):
     """Differentiable fused attention probabilities (see _AttnProbs); q, k [B, U, M*d] contiguous, TF32-rounded.
     alpha: score scale (default 1/sqrt(d) of the per-mode width).  posbias (PosBias): sliding-window positional bias
-    inside the softmax; its table receives a gradient."""
+    inside the softmax; its table receives a gradient.  transposed: -> (P, P^T) (see _AttnProbs), else P."""
     if alpha is None:
         alpha = 1.0 / math.sqrt(q.shape[-1] // M)
     return _AttnProbs.apply(q.contiguous(), k.contiguous(), M, float(alpha), float(clip), drop_p, seed, diag,
-                            *_pb_args(posbias), bool(kmajor_dq))
+                            *_pb_args(posbias), bool(kmajor_dq), bool(transposed))
 
 
 def _sgemm(A, B, M, N, K, sa, sb, out=None, alpha=1.0, accumulate=False, Z=1, zs=(0, 0, 0)):
