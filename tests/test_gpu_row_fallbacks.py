@@ -6,12 +6,9 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.helpers import close, close_on_scale, ln_softaggr64, prologue64, reference, run_twice
+
 pytestmark = pytest.mark.gpu
-
-
-def close(a, b, tol):
-    err = float((a.double() - b).abs().max() / b.abs().max().clamp_min(1e-30))
-    assert err < tol, err
 
 
 @pytest.fixture(autouse=True)
@@ -19,32 +16,6 @@ def _seed():
     torch.manual_seed(0)
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
-
-
-def run_twice(fn, inputs, seed=1):
-    """fn(*leaves) -> output, then backward with a fixed upstream gradient; done twice on fresh leaves.  Asserts that
-    both runs agree bit for bit and returns (output, [grads]) of the first run."""
-    runs = []
-    for _ in range(2):
-        leaves = [t.detach().clone().requires_grad_() for t in inputs]
-        out = fn(*leaves)
-        gen = torch.Generator(device=out.device).manual_seed(seed)
-        out.backward(torch.randn(out.shape, device=out.device, generator=gen))
-        runs.append((out.detach(), [t.grad for t in leaves]))
-    (o1, g1), (o2, g2) = runs
-    assert torch.equal(o1, o2)
-    for a, b in zip(g1, g2):
-        assert torch.equal(a, b)
-    return o1, g1
-
-
-def reference(fn, inputs, out_shape, seed=1):
-    """fp64 output and gradients of fn on the same inputs and upstream gradient as run_twice."""
-    leaves = [t.detach().double().requires_grad_() for t in inputs]
-    out = fn(*leaves)
-    gen = torch.Generator(device=out.device).manual_seed(seed)
-    out.backward(torch.randn(out_shape, device=out.device, generator=gen).double())
-    return out.detach(), [t.grad for t in leaves]
 
 
 @pytest.mark.parametrize("C,C0,per_sample", [(98, 128, False), (2056, 2056, True)])
@@ -58,10 +29,7 @@ def test_prologue_with_positional_code(C, C0, per_sample):
               torch.randn(*((B,) if per_sample else ()), N, C0, device="cuda")]
     h, grads = run_twice(lambda x, g, b, pe: ops.prologue(x, g, b, pe, 0.7, mask), inputs)
 
-    def ref(x, g, b, pe):
-        t = F.layer_norm(x, (C,), g, b, 1e-12) + 0.7 * pe[..., :C]
-        return F.layer_norm(t, (C,), None, None, 1e-12) * mask.view(B, N, 1).double()
-    hr, grads_r = reference(ref, inputs, h.shape)
+    hr, grads_r = reference(lambda x, g, b, pe: prologue64(x, g, b, pe, 0.7, mask), inputs, h.shape)
     close(h, hr, 1e-3)            # h is rounded to TF32 for the following GEMMs
     for a, b in zip(grads, grads_r):
         close(a, b, 1e-4)
@@ -88,16 +56,13 @@ def test_ln_softaggr_generic(M, F_):
               torch.randn(1, F_, device="cuda"), torch.randn(1, device="cuda")]
     out, grads = run_twice(ops.ln_softaggr, inputs)
 
-    def ref(Y, g, b, ws, bs):
-        yn = F.layer_norm(Y, (F_,), g, b, 1e-12)
-        return (yn * torch.softmax(F.linear(yn, ws, bs), dim=1)).sum(1)
-    outr, grads_r = reference(ref, inputs, out.shape)
+    outr, grads_r = reference(ln_softaggr64, inputs, out.shape)
     close(out, outr, 1e-5)
     close(grads[0], grads_r[0], 1e-3)      # dY is rounded to TF32
     for a, b in zip(grads[1:4], grads_r[1:4]):
         close(a, b, 1e-4)
     # d bs is a sum of score gradients whose sum over the modes of each token is zero: compare on the scale of d ws
-    assert float((grads[4].double() - grads_r[4]).abs().max()) < 1e-4 * float(grads_r[3].abs().max())
+    close_on_scale(grads[4], grads_r[4], float(grads_r[3].abs().max()), 1e-4)
 
 
 def test_colsum_odd_width():
